@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- agent observations per second of the step+render hot path on B200 (BASELINE.json metric).
+"""bench.py -- agent observations per second of the step+render hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            our arm (CUDA engine through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...  the reference arm: the CPU restatement (oracle/) on the box's
                                                            host cores -- the real reference cannot be built here
                                                            (Bullet 2.89 / Vulkan / EGL absent, DESIGN.md)
   python bench.py --config {2,3,4}                         headline another single-GPU BASELINE config
+  python bench.py --dump-outputs DIR                       also write what the headline's last timed step computed, as .npy
 
 A "step" is one pass of the hot path over one batch.  The HEADLINE workload is BASELINE.json configs[3], Collect 1024 envs x
 4 agents at 128x72 per GPU: 4096 agent views = 151 MB of RGBA8 observations per step -- the largest single-GPU config by
@@ -28,6 +29,7 @@ import time
 
 import numpy as np
 
+sys.dont_write_bytecode = True  # the bench runs from the built tree and leaves it as it found it (it may be read-only)
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 os.environ.setdefault("BOXOBAN_LEVELS", os.path.join(ROOT, "tests", "golden", "boxoban"))  # Sokoban (config 5) reads level files
@@ -43,24 +45,8 @@ CONFIGS = {
 HEADLINE = 4
 MEGAVERSE8 = ["TowerBuilding", "ObstaclesEasy", "ObstaclesHard", "Collect", "Sokoban", "HexMemory", "HexExplore", "Rearrange"]  # megaverse_env.py:12-20
 MIXED_ENVS_PER_GPU = 1024
-
-
-def measured_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(cfg_id):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the raster kernel per launch, from the committed ncu capture of this config"""
-    try:
-        with open(os.path.join(ROOT, "profiles", "dram_traffic.json")) as f:
-            rec = json.load(f)[str(cfg_id)]
-        return float(rec["bytes_per_launch"]), rec.get("source")
-    except Exception:  # noqa: BLE001
-        return None, None
+HBM_PEAK_GBS, HBM_PEAK_SOURCE = 3350.0, "NVIDIA H100 SXM data sheet (HBM3), not measured"
+DUMP_VIEWS = 256  # views of the obs (and depth) tensor written by --dump-outputs: 256 x 36 864 x 4 B = 38 MB of float32 RGBA
 
 
 class ClockSampler:
@@ -100,6 +86,15 @@ class ClockSampler:
             except Exception:  # noqa: BLE001
                 pass
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def power_limit(gpu):
+    """the card's power limit in W (part of every number this bench prints), None where nvidia-smi cannot tell"""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(gpu), "--query-gpu=power.limit", "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        return float(out.stdout.strip())
+    except Exception:  # noqa: BLE001
+        return None
 
 
 def dist_env():
@@ -261,7 +256,28 @@ class Harness:
         return self.max_ms(total * 1e3)
 
 
-def measure_config(hz, cfg_id, K, Wm, rank, cores, sample_clocks=False):
+def dump_outputs(eng, depth, out_dir):
+    """what the device-resident step hands its caller (obs, depth, rewards, dones) as float32 / float64 .npy files: rewards, dones and a
+    per-view sum of the obs tensor in full, the obs (and depth) of DUMP_VIEWS views picked by a fixed seed"""
+    import torch
+
+    obs = torch.as_tensor(eng.device_array("obs"), device="cuda")
+    idx = np.sort(np.random.default_rng(0).choice(eng.N, size=min(eng.N, DUMP_VIEWS), replace=False))
+    tidx = torch.from_numpy(idx).cuda()
+    out = {"obs_sample": obs.index_select(0, tidx).float(), "obs_sample_index": torch.from_numpy(idx.astype(np.float64)),
+           "obs_view_sum": obs.reshape(eng.N, -1).sum(dim=1, dtype=torch.int64).double(),
+           "rewards": torch.as_tensor(eng.device_array("rewards"), device="cuda").clone(),
+           "dones": torch.as_tensor(eng.device_array("dones"), device="cuda").float()}
+    if depth:
+        out["depth_sample"] = torch.as_tensor(eng.device_array("depth"), device="cuda").index_select(0, tidx)
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+    return sorted(out)
+
+
+def measure_config(hz, cfg_id, K, Wm, rank, cores, sample_clocks=False, dump_dir=None):
     """one BASELINE single-GPU config on this rank's GPU: device-resident value, e2e through host buffers, roofline of the raster kernel"""
     from megaverse_b200 import capi, sharding
 
@@ -299,19 +315,19 @@ def measure_config(hz, cfg_id, K, Wm, rank, cores, sample_clocks=False):
     ms_warm = hz.timed(stream, dev_step, K, Wm)
     eng.sync()
     clocks = sampler.stop() if sampler else None
+    dumped = dump_outputs(eng, depth, dump_dir) if dump_dir else None
 
     # ---- end-to-end through host buffers
-    Ke = max(20, min(K, 200))
     for t in range(3):
         host_step(t)
-    ms_e = hz.timed_host_flushed(stream, host_step, Ke, Wm)
-    ms_e_warm = hz.timed(stream, host_step, Ke, Wm)
+    ms_e = hz.timed_host_flushed(stream, host_step, K, Wm)
+    ms_e_warm = hz.timed(stream, host_step, K, Wm)
 
     # ---- roofline of the dominant kernel (rasteriser): CUDA events around the kernel on the engine stream, L2 flushed before
-    peak, peak_src = measured_peaks()
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
     eng.set_option("overlap", 0)  # kernels back to back so that each can be timed on its own
     ras, stp = [], []
-    for t in range(24):
+    for t in range(4 + K):  # the first 4 settle the serialised mode and are not counted
         with torch.cuda.stream(stream):
             hz.flush.zero_()
         dev_step(Wm + t)
@@ -320,9 +336,8 @@ def measure_config(hz, cfg_id, K, Wm, rank, cores, sample_clocks=False):
         stp.append(s_ms); ras.append(r_ms)
     ras_ms, stp_ms = float(np.mean(ras[4:])), float(np.mean(stp[4:]))
     achieved = obs_bytes / (ras_ms / 1e3) / 1e9
-    traffic, traffic_src = ncu_traffic(cfg_id)
-    roofline = {"bound": "hbm", "kernel": "mvr::viewKernel", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_launch": obs_bytes, "kernel_ms": ras_ms, "step_kernel_ms": stp_ms,
+    roofline = {"bound": "hbm", "kernel": "mvr::viewKernel", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+                "peak_source": peak_src, "algorithmic_bytes_per_launch": obs_bytes, "kernel_ms": ras_ms, "step_kernel_ms": stp_ms,
                 "note": "obs(+depth) bytes written per launch / raster kernel duration (CUDA events, L2 flushed, kernels serialised); the kernel is "
                         "issue / latency bound (geometry, coverage and shading all run from shared memory), not HBM bound: DESIGN.md"}
     faults = eng.faults()
@@ -330,9 +345,10 @@ def measure_config(hz, cfg_id, K, Wm, rank, cores, sample_clocks=False):
     eng.close()
     return {"workload": cfg["name"] + " per GPU, random one-bit actions, resets included",
             "value": N * world * K / (ms / 1e3), "ms_per_step": ms / K, "value_l2_warm": N * world * K / (ms_warm / 1e3), "ms_per_step_l2_warm": ms_warm / K,
-            "e2e": {"value": N * world * Ke / (ms_e / 1e3), "unit": UNIT, "h2d_bytes_per_step": N * 4, "d2h_bytes_per_step": obs_bytes + N * 8 + E, "steps": Ke,
-                    "ms_per_step": ms_e / Ke, "value_l2_warm": N * world * Ke / (ms_e_warm / 1e3), "d2h_gbs": obs_bytes / (ms_e / Ke / 1e3) / 1e9},
-            "roofline": roofline, "gpu_launches": int(launches), "faults": int(faults), "clocks": clocks, "raster": rcfg, "views_per_gpu": N}
+            "e2e": {"value": N * world * K / (ms_e / 1e3), "unit": UNIT, "h2d_bytes_per_step": N * 4, "d2h_bytes_per_step": obs_bytes + N * 8 + E, "steps": K,
+                    "ms_per_step": ms_e / K, "value_l2_warm": N * world * K / (ms_e_warm / 1e3), "d2h_gbs": obs_bytes / (ms_e / K / 1e3) / 1e9},
+            "roofline": roofline, "gpu_launches": int(launches), "faults": int(faults), "clocks": clocks, "raster": rcfg, "views_per_gpu": N,
+            "dumped": dumped}
 
 
 def measure_mixed(hz, K, Wm, rank, cores, gather, overlap_gather=False, grid_share=False):
@@ -444,6 +460,7 @@ def main():
     ap.add_argument("--config", type=int, default=HEADLINE, choices=sorted(CONFIGS), help="BASELINE config to headline (default: the largest)")
     ap.add_argument("--only-headline", action="store_true", help="skip the other configs' sub-records")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline's last timed step (obs sample, per-view obs sums, rewards, dones) as .npy")
     args = ap.parse_args()
     rank, local_rank, world = dist_env()
     K, Wm = args.steps, max(args.warmup, 3)
@@ -459,7 +476,7 @@ def main():
         # the reference's own CPU path cannot be built here; the port (oracle) stands in.  Rank 0 only.
         if rank != 0:
             return
-        v, dt, n = run_cpu(head, cores, seconds=max(6.0, min(60.0, 0.05 * K)), warmup=min(Wm, 3), min_steps=min(K, 50))
+        v, dt, n = run_cpu(head, cores, seconds=0.0, warmup=min(Wm, 3), min_steps=K)
         line = {"impl": "reference", "metric": METRIC, "value": v, "unit": UNIT, "n_gpus": args.gpus, "steps": n, "warmup": min(Wm, 3),
                 "ms_per_step": dt / n * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                 "config": config,
@@ -473,7 +490,8 @@ def main():
     import torch.distributed as dist
     from megaverse_b200 import _build
 
-    _build.build_all()
+    if not _build._newer(_build.LIB, _build._sources()):  # the bench never builds (the tree may be read-only): say what it measures
+        print("bench.py: warning: %s is missing or older than its sources; run `python -m megaverse_b200._build`" % _build.LIB, file=sys.stderr)
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs a CUDA device (the product has no CPU fallback)")
     torch.cuda.set_device(local_rank)
@@ -482,7 +500,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     hz = Harness(torch, dist, world, local_rank)
 
-    main_rec = measure_config(hz, args.config, K, Wm, rank, cores, sample_clocks=True)
+    main_rec = measure_config(hz, args.config, K, Wm, rank, cores, sample_clocks=True, dump_dir=args.dump_outputs if rank == 0 else None)
     others = {}
     if world == 1 and not args.only_headline:
         for cid in sorted(CONFIGS):
@@ -514,7 +532,8 @@ def main():
                 "roofline": main_rec["roofline"], "cpu_baseline": main_rec.get("cpu_baseline"),
                 "value_l2_warm": main_rec["value_l2_warm"], "ms_per_step_l2_warm": main_rec["ms_per_step_l2_warm"],
                 "e2e": main_rec["e2e"], "clocks": main_rec["clocks"], "gpu_launches": main_rec["gpu_launches"], "faults": main_rec["faults"],
-                "raster": main_rec["raster"], "numa": numa, "configs": others, "config5": config5}
+                "raster": main_rec["raster"], "numa": numa, "configs": others, "config5": config5,
+                "gpu": {"name": torch.cuda.get_device_name(local_rank), "power_limit_w": power_limit(local_rank)}, "dumped": main_rec["dumped"]}
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

@@ -1,4 +1,4 @@
-/* megaverse_b200 -- thin C ABI of the B200 batched voxel-world step + render engine.
+/* megaverse_b200 -- thin C ABI of the H100 batched voxel-world step + render engine.
  *
  * Drop-in boundary for the reference's per-step hot path.  Each entry point replaces what the reference's pybind11
  * class MegaverseGym (src/libs/bindings/megaverse.cpp:36-263) reaches through VectorEnv (src/libs/env/src/vector_env.cpp)

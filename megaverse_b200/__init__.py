@@ -1,4 +1,4 @@
-"""megaverse_b200: B200-native batched voxel-world step + render engine behind the Megaverse env API.
+"""megaverse_b200: H100-native batched voxel-world step + render engine behind the Megaverse env API.
 
 Only the per-step hot path is here (agent kinematics + collision, carry/place, reward/done, first-person rasteriser);
 see DESIGN.md.  `MegaverseEnv` mirrors megaverse/megaverse_env.py of the reference."""

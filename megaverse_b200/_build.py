@@ -1,7 +1,7 @@
 """In-tree build of the native code (no JIT cache: the built .so files travel to the GPU box with the repo snapshot).
 
-  libmegaverse_b200.so                         C-ABI engine: sm_100a kernels + host level generation   (nvcc)
-  extension/megaverse.cpython-*.so             pybind11 module `megaverse_b200.extension.megaverse`     (g++)
+  libmegaverse_b200.so                         C-ABI engine: sm_90a (H100) kernels + host level generation   (nvcc)
+  extension/megaverse.cpython-*.so             pybind11 module `megaverse_b200.extension.megaverse`           (g++)
 """
 import os
 import shutil
@@ -15,7 +15,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libmegaverse_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     # no FMA contraction on either side: device results must equal a plain IEEE CPU evaluation (parity with the oracle)
     "-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
 ]

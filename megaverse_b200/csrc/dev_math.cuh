@@ -1,4 +1,4 @@
-// Device float math for the step / raster kernels (sm_100a).  Compiled with -fmad=false: every +,-,*,/ and sqrt is a
+// Device float math for the step / raster kernels (sm_90a).  Compiled with -fmad=false: every +,-,*,/ and sqrt is a
 // single IEEE-754 round-to-nearest operation in the order written, so results are reproducible against a CPU that also
 // keeps contraction off.  Accumulation orders follow the reference's libraries:
 //   4x4 product / inverse / rotation : Magnum (Math/RectangularMatrix.h:753-764, Math/Matrix.h:379-421,491-522,

@@ -137,7 +137,7 @@ struct mv_engine {
     bool skipUnfitLevels = false;  // option "skip_unfit_levels": replace a level that exceeds a fixed capacity by the stream's next one
     std::atomic<int> levelsSkipped{0};
     // host delivery of the obs tensor (host-facing steps).  zero copy (default): the raster kernel stores the rows straight into pinned
-    // host memory, the PCIe writes overlap the drawing (measured best from 9 MB to 151 MB per step: 40 GB/s effective at Collect 1024 x 4).
+    // host memory, the PCIe writes overlap the drawing (measured best at 9 MB and at 151 MB per step on an H100: 45 GB/s effective at Collect 1024 x 4).
     // Otherwise: rasterise into HBM in host_slices launches, each slice's download on the copy engine while the next is drawn.
     int zeroCopyOpt = 1, hostSlicesOpt = 0;
     bool rasterToHost = false;
@@ -153,7 +153,7 @@ struct mv_engine {
     WaitValue32Fn waitValue32 = nullptr;
     cudaStream_t copyStream = nullptr;
     std::vector<cudaEvent_t> sliceEv;
-    int numSMs = 148;
+    int numSMs = 132;              // H100 SXM; replaced by the device's count in mv_create
     MvConsts consts{};
 
     cudaStream_t stream = nullptr;
@@ -475,7 +475,7 @@ struct mv_engine {
         const bool zc = zeroCopyOpt != 0;
         if (zc) return 0;
         if (hostSlicesOpt > 0) return std::min(hostSlicesOpt, E);
-        return int(std::max<size_t>(1, std::min<size_t>({size_t(2), size_t(E), bytes / (size_t(32) << 20)})));  // two slices measured best at 151 MB
+        return int(std::max<size_t>(1, std::min<size_t>({size_t(4), size_t(E), bytes / (size_t(32) << 20)})));  // four slices: the best copy-engine form at 151 MB (H100)
     }
     // draw_hires (megaverse.cpp:154-177): every agent view once more, at (w, h), from the instance lists and camera matrices of
     // the last step -- the same kernel over row bands of the large frame.  Result in hires.h_obs, uint8[N][h][w][4].
@@ -798,9 +798,9 @@ int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents, 
             (void)cudaGetLastError();
     }
     if (e->instCap > mvr::kMaxInstancesPerEnv) { e->setError("instance capacity exceeds the draw-order key range"); return fail(MV_ERR_CAPACITY); }
-    // few views: split every view into row bands so that the persistent grid (2 CTAs per SM) has something to balance.  With the
-    // cost-ordered queue finer items pay up to about two views per CTA (measured: 256 views 3 bands 0.128 ms per step, 2 bands 0.144, 6 bands
-    // 0.144; 512 views 2 bands 0.169, 1 band 0.188; 1024 views 1 band 0.241, 2 bands 0.273 -- every band repeats the view's geometry)
+    // few views: split every view into row bands so that the persistent grid (2 CTAs per SM) has something to balance; every band repeats
+    // the view's geometry.  Measured on an H100 (ms per step, 1 / 2 / 3 bands): TowerBuilding 64 views 0.106 / 0.091 / 0.085, 256 views
+    // 0.135 / 0.148 / 0.139, 512 views 0.185 / 0.185; Collect 256 views 0.546 / 0.425 / 0.387, 512 views 0.564 / 0.421
     e->rasterBands = N <= 320 ? 3 : (N <= 640 ? 2 : 1);
     while (e->rasterBands > 1 && (h / 4) % e->rasterBands) --e->rasterBands;
     if (ok && e->configureRaster() != MV_OK) return fail(MV_ERR_CUDA);

@@ -1,4 +1,4 @@
-// Shared host/device plain-old-data layouts for the B200 voxel-world engine.
+// Shared host/device plain-old-data layouts for the H100 voxel-world engine.
 //
 // HBM layout (one GPU, E envs, A agents per env, N = E*A views):
 //   levels   MvLevel[E][2]          double-buffered immutable level description (host-generated, H2D on reset only)

@@ -73,7 +73,7 @@ constexpr int kSmallList = 128;   // small triangles of a tile collected before 
 #ifndef MV_SMALL_AREA
 #define MV_SMALL_AREA 4
 #endif
-constexpr int kSmallArea = MV_SMALL_AREA;    // triangles covering at most this many pixels of a tile are evaluated by one lane (swept 0..64: profiles/r2e_summary.txt)
+constexpr int kSmallArea = MV_SMALL_AREA;    // triangles covering at most this many pixels of a tile are evaluated by one lane (chosen by a sweep over 0..64)
 // a fragment is (~depth bits << 32) | (draw-order key << kIdxBits) | index in the CTA's triangle list
 constexpr int kIdxBits = 10;
 constexpr uint32_t kStaleIdx = (1u << kIdxBits) - 1u;  // "already shaded in an earlier batch"
@@ -561,7 +561,7 @@ __device__ __forceinline__ unsigned long long packFrag(float z, uint32_t key, in
 // batches repaint only the pixels they win.  Unless `final`, the per-pixel best fragment is parked in the CTA's spill slab with its
 // list index replaced by kStaleIdx (the list is about to be overwritten).
 // out of line on purpose: the tile pass is called from two places (a full triangle list in mid-view, the end of the view) and two inlined
-// copies of it pushed the kernel's hot code out of the instruction cache (Collect 1024 x 4: 2.65 ms inlined, 1.70 ms called)
+// copies of it pushed the kernel's hot code out of the instruction cache (the inlined form was markedly slower)
 #ifdef MV_TILE_FORCEINLINE
 #define MV_TILE_INLINE __forceinline__
 #else
@@ -585,7 +585,7 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
         if (lane == 0) tile = atomicAdd(tileCtr, 1);
         tile = __shfl_sync(0xffffffffu, tile, 0);
         if (tile >= bandTiles) break;
-        const int tk = tile / tilesX, ty = tk;  // (drawing the tile rows from the middle outwards -- horizon first, sky and floor last -- was measured: no effect)
+        const int tk = tile / tilesX, ty = tk;  // (drawing the tile rows from the middle outwards -- horizon first, sky and floor last -- was tried: no effect)
         const int tx0 = (tile - tk * tilesX) * 32, ty0 = rowLo + ty * 4;
         const int px = tx0 + (lane & 7) * 4, py = ty0 + (lane >> 3);
         const int sx32 = px * 256 + 128, sy32 = py * 256 + 128;
@@ -720,7 +720,7 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
         uint32_t o0 = 0xff000000u, o1 = 0xff000000u, o2 = 0xff000000u, o3 = 0xff000000u;
         float w0 = 0.0f, w1 = 0.0f, w2 = 0.0f, w3 = 0.0f;
         // (keeping the records of the previous pixel's triangle in registers across the iterations -- the lane's four pixels mostly belong
-        // to one triangle -- was measured: 20 % SLOWER, the loop then spills)
+        // to one triangle -- was tried: SLOWER, the loop then spills)
 #pragma unroll 1
         for (int k = 0; k < 4; ++k) {
             const uint32_t ti = uint32_t(winners >> (16 * k)) & 0xffffu;

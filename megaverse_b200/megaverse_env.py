@@ -1,4 +1,4 @@
-"""MegaverseEnv: the reference's Python env class (megaverse/megaverse_env.py:42-201) over the B200 engine.
+"""MegaverseEnv: the reference's Python env class (megaverse/megaverse_env.py:42-201) over the H100 engine.
 
 Same constructor, attributes and methods, so Sample-Factory's Wrapper (megaverse_rl/megaverse_utils.py:48-88) drives it
 unchanged.  The per-agent pybind loops of the reference (megaverse_env.py:121-162) are replaced by one batched call each;

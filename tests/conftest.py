@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `pytest -m gpu`)")
 
 
 # Sokoban reads Boxoban level files (scenario_sokoban.cpp:39-81); the dataset is not available offline, so the tests point

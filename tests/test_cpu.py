@@ -26,6 +26,17 @@ def test_abi_exports_every_declared_symbol(built):
         assert hasattr(L, name), name
 
 
+def test_library_holds_sm90a_code(built):
+    """the kernels are compiled for the H100 (sm_90a) and for nothing else: a cubin for another architecture does not load there"""
+    import shutil
+    from megaverse_b200 import capi
+
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    out = subprocess.run([cuobjdump, "--list-elf", capi.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    archs = sorted(set(ln.rsplit(".", 2)[-2] for ln in out.splitlines() if ln.strip().endswith(".cubin")))
+    assert archs == ["sm_90a"], out
+
+
 def test_no_cpu_fallback(built):
     """without a CUDA device the product must fail loudly (no oracle / CPU path behind the ABI)"""
     import torch

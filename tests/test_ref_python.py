@@ -123,6 +123,24 @@ class _OracleEnv:
 
 
 @pytest.mark.parametrize("case", CASES)
+def test_product_default_reward_shaping_matches_the_reference_golden(built, case):
+    """the tables the engine is built from (host-only accessor, no GPU) hold the default reward shaping the reference's class returned,
+    key for key and bit for bit"""
+    import ctypes as C
+
+    from megaverse_b200 import capi
+
+    g = np.load(GOLDEN)
+    L = capi.lib()
+    L.mv_debug_defaults.argtypes = [C.c_char_p, C.c_char_p, C.c_int]
+    buf = C.create_string_buffer(8192)
+    assert L.mv_debug_defaults(str(g[case + "/scenario"]).encode(), buf, 8192) > 0
+    ours = dict(ln[2:].split("=") for ln in buf.value.decode().splitlines() if ln.startswith("R "))
+    ref = {str(k): "%08x" % v for k, v in zip(g[case + "/shaping_keys"], g[case + "/shaping_default"].view(np.uint32))}
+    assert ours == ref, "reward shaping:\nreference %s\nproduct   %s" % (ref, ours)
+
+
+@pytest.mark.parametrize("case", CASES)
 def test_oracle_replays_the_reference_python_golden(built, case):
     _replay(_OracleEnv, case)
 
