@@ -132,6 +132,28 @@ int mv_dones_device(mv_handle h, uint8_t **d_dones);
 /* the CUDA stream (cudaStream_t) all engine work is ordered on */
 int mv_stream(mv_handle h, void **stream);
 
+/* Env state store: save envs mid-episode and rewind or clone them later, on the device.  A store holds `rows` env states; a row is the
+ * complete state of one env -- every per-env device array (env, agents, objects, object grid, instance list, views, both level slots,
+ * rewards, dones, true objectives, fault bits) and the host state (the env's level generator and RNG, its live slot and episode index,
+ * the host mirrors of both levels).  Reward shaping (it belongs to the agent index a policy sees), options, the engine-wide fault word
+ * (mv_fault_word) and mv_levels_skipped stay with the engine.
+ * mv_states_create: a store of `rows` rows, its id in *store; freed by mv_states_destroy or mv_close.
+ * mv_states_save: copies env envs[i] into row rows[i] (rows distinct).
+ * mv_states_load: env envs[i] continues exactly as the env saved into row rows[i] would have (same frames, rewards, dones and later
+ * levels for the same actions); envs distinct, a row may go to several envs (clones run the same level stream).  Other envs are untouched.
+ * Afterwards every view is drawn again and delivered as a step would (host buffer, HBM or mv_set_obs_buffer's, depth included): the
+ * loaded views show the frames of the saved step, and rewards / dones / true objectives read as they did after it.  A load is not an
+ * episode end.
+ * Save and load are synchronisation points: they retire outstanding mv_step_device steps and wait for the level generators.  Both need
+ * mv_reset first and refuse an outstanding mv_step_begin (MV_ERR_STATE).  After either, mv_last_kernel_ms gives [0] the copy kernel
+ * and [1] the re-render (0 after a save).  Stores belong to the engine that made them. */
+int mv_states_create(mv_handle h, int rows, int *store);
+int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *rows, int n);
+int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *envs, int n);
+int mv_states_destroy(mv_handle h, int store);
+/* device bytes one row holds (grows with the static-box arrays, see option "static_cap") */
+int mv_state_row_bytes(mv_handle h, int64_t *out);
+
 /* sticky per-env fault bits ORed over all envs (MV_FAULT_* in mv_types.h); 0 = healthy */
 int mv_faults(mv_handle h, int32_t *out);
 /* the same bits without a device round trip: the step kernel ORs every fault it raises into a pinned host word (sticky).  Valid for

@@ -51,6 +51,11 @@ def lib():
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
         L.mv_debug_bzset.argtypes = [vp, ci, vp, ci]
         L.mv_debug_generate_level.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp, ci]
+        L.mv_states_create.argtypes = [vp, ci, C.POINTER(ci)]
+        L.mv_states_save.argtypes = [vp, ci, vp, vp, ci]
+        L.mv_states_load.argtypes = [vp, ci, vp, vp, ci]
+        L.mv_states_destroy.argtypes = [vp, ci]
+        L.mv_state_row_bytes.argtypes = [vp, C.POINTER(C.c_int64)]
         _lib = L
     return _lib
 
@@ -61,6 +66,7 @@ EXPORTS = [
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
     "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view",
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
+    "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes",
 ]
 
 
@@ -236,6 +242,32 @@ class Engine:
         self._ck(lib().mv_debug_raster_stats(self._h, out if read else None, 1 if enable else 0))
         names = ["work_items", "instances", "visible_instances", "items", "clipped_items", "triangles", "batches", "sub_passes", "cyc_head", "cyc_tma_wait", "cyc_instance", "cyc_item", "cyc_tile", "cyc_total"]
         return {n: int(out[i]) for i, n in enumerate(names)}
+
+    # ---- env state store (mv_states_*)
+    def states_create(self, rows):
+        sid = C.c_int()
+        self._ck(lib().mv_states_create(self._h, int(rows), C.byref(sid)))
+        return sid.value
+
+    def states_save(self, store, envs, rows):
+        """env envs[i] -> row rows[i] of the store"""
+        e, r = np.ascontiguousarray(envs, dtype=np.int32), np.ascontiguousarray(rows, dtype=np.int32)
+        assert e.size == r.size
+        self._ck(lib().mv_states_save(self._h, int(store), e.ctypes.data, r.ctypes.data, e.size))
+
+    def states_load(self, store, rows, envs):
+        """row rows[i] of the store -> env envs[i]; obs() / rewards() / dones() then read as after the saved step"""
+        r, e = np.ascontiguousarray(rows, dtype=np.int32), np.ascontiguousarray(envs, dtype=np.int32)
+        assert e.size == r.size
+        self._ck(lib().mv_states_load(self._h, int(store), r.ctypes.data, e.ctypes.data, e.size))
+
+    def states_destroy(self, store):
+        self._ck(lib().mv_states_destroy(self._h, int(store)))
+
+    def state_row_bytes(self):
+        n = C.c_int64()
+        self._ck(lib().mv_state_row_bytes(self._h, C.byref(n)))
+        return n.value
 
     def last_kernel_ms(self):
         out = (C.c_float * 2)()

@@ -16,7 +16,9 @@
 #include <cstdio>
 #include <cstring>
 #include <functional>
+#include <memory>
 #include <mutex>
+#include <optional>
 #include <queue>
 #include <string>
 #include <thread>
@@ -26,6 +28,7 @@
 #include "hostmath.hpp"
 #include "levelgen.hpp"
 #include "raster_view.cuh"
+#include "state_copy.h"
 #include "step_kernel.cuh"
 
 namespace {
@@ -110,6 +113,34 @@ template <typename T> struct PinBuf {
     size_t n = 0;
     cudaError_t alloc(size_t count) { n = count; return cudaMallocHost(reinterpret_cast<void **>(&p), sizeof(T) * (count ? count : 1)); }
     void free() { if (p) cudaFreeHost(p); p = nullptr; }
+};
+
+// one per-env device array as the state store sees it: `units` rows per env (2 for the arrays that hold both level slots) of unitBytes
+struct EnvSlab {
+    uint8_t *base;
+    int units;
+    size_t unitBytes;
+    size_t rowBytes() const { return size_t(units) * unitBytes; }
+};
+// indices into mv_engine::envSlabs() of the arrays that growStatics re-pitches
+enum { kSlabInst = 4, kSlabStatics = 8, kSlabStaticRot = 9, kSlabCount = 16 };
+
+// saved env states (mv_states_*): every per-env device row in arrays of `rows` rows with the engine's pitch, plus the host state
+struct StateStore {
+    int rows = 0;
+    DevBuf<uint8_t> slabs[kSlabCount];  // same order as mv_engine::envSlabs()
+    struct HostRow {
+        std::optional<mv::LevelGenerator> gen;  // empty: the row was never saved
+        int slot = 0, episode = 0, words[2] = {0, 0};
+        // the host mirrors of both level slots that the debug dumps and the uploads read
+        MvLevel level[2];
+        std::vector<MvBox> statics[2];
+        std::vector<float> staticRot[2];
+        std::vector<MvDeco> deco[2];
+        std::vector<uint32_t> solid[2];  // the three bit planes, levelWords words each
+    };
+    std::vector<HostRow> host;
+    void free() { for (auto &s : slabs) s.free(); }
 };
 
 }  // namespace
@@ -240,6 +271,10 @@ struct mv_engine {
     std::mutex genMutex;
     bool rtableDirty = true;
 
+    std::vector<std::unique_ptr<StateStore>> stores;  // mv_states_create ids; null once destroyed
+    PinBuf<int2> h_pairs;                              // (source row, destination row) of the last save / load
+    DevBuf<int2> d_pairs;
+
     // ------------------------------------------------------------------ level generation scheduling
     // generate the level for episode `serial` of env e into staging slot s (worker thread)
     void scheduleGen(int e, int s, int serial) {
@@ -298,11 +333,29 @@ struct mv_engine {
         MV_CUDA(cudaStreamSynchronize(stream));
         DevBuf<MvBox> nStat; DevBuf<float> nRot; DevBuf<MvInstance> nInst; PinBuf<MvBox> hStat; PinBuf<float> hRot;
         const size_t rows = size_t(E) * 2;
-        if (nStat.alloc(rows * newCap) != cudaSuccess || nRot.alloc(rows * newCap * 2) != cudaSuccess || nInst.alloc(size_t(E) * newInstCap) != cudaSuccess ||
+        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside
+        struct Repitch { DevBuf<uint8_t> *buf; DevBuf<uint8_t> next; size_t rows, oldPitch, newPitch; };
+        std::vector<Repitch> storeGrow;
+        for (auto &st : stores) {
+            if (!st) continue;
+            const size_t r = size_t(st->rows);
+            storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * 2, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
+            storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * 2, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
+            storeGrow.push_back({&st->slabs[kSlabInst], {}, r, sizeof(MvInstance) * instCap, sizeof(MvInstance) * newInstCap});
+        }
+        bool storesOk = true;
+        for (auto &g : storeGrow) storesOk = storesOk && g.next.alloc(g.rows * g.newPitch) == cudaSuccess;
+        if (!storesOk || nStat.alloc(rows * newCap) != cudaSuccess || nRot.alloc(rows * newCap * 2) != cudaSuccess || nInst.alloc(size_t(E) * newInstCap) != cudaSuccess ||
             hStat.alloc(rows * newCap) != cudaSuccess || hRot.alloc(rows * newCap * 2) != cudaSuccess) {
             nStat.free(); nRot.free(); nInst.free(); hStat.free(); hRot.free();
+            for (auto &g : storeGrow) g.next.free();
             setError("growing the static-box arrays: allocation failed");
             return MV_ERR_CUDA;
+        }
+        for (auto &g : storeGrow) {
+            MV_CUDA(cudaMemcpy2D(g.next.p, g.newPitch, g.buf->p, g.oldPitch, g.oldPitch, g.rows, cudaMemcpyDeviceToDevice));
+            g.buf->free();
+            *g.buf = g.next;
         }
         MV_CUDA(cudaMemcpy2D(nStat.p, sizeof(MvBox) * newCap, d_statics.p, sizeof(MvBox) * staticCap, sizeof(MvBox) * staticCap, rows, cudaMemcpyDeviceToDevice));
         MV_CUDA(cudaMemcpy2D(nRot.p, sizeof(float) * 2 * newCap, d_staticRot.p, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * staticCap, rows, cudaMemcpyDeviceToDevice));
@@ -411,7 +464,9 @@ struct mv_engine {
         for (int e = 0; e < E; ++e) init[costItems() + size_t(e)] = uint32_t(e);
         return cudaMemcpy(d_viewCost.p, init.data(), sizeof(uint32_t) * init.size(), cudaMemcpyHostToDevice);
     }
-    int launchRaster() {
+    // dependent = false: a launch that follows no step kernel (the re-render after mv_states_load)
+    int launchRaster(bool dependent = true) {
+        const bool dep = overlap && dependent;
         mvr::ViewParams vp = {};
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p; vp.instStride = instCap;
         // pinned allocations are mapped into the device address space (UVA), so the kernel can store through the host pointer
@@ -420,7 +475,7 @@ struct mv_engine {
         vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4; vp.triCap = triCap;
         vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
         // programmatic dependent launch: the grid may start before the step kernel has drained; a CTA waits for its env's stamp
-        vp.ready = overlap ? d_ready.p : nullptr; vp.readyStamp = overlap ? readyStamp : 0;
+        vp.ready = dep ? d_ready.p : nullptr; vp.readyStamp = dep ? readyStamp : 0;
         deviceObsFresh = !rasterToHost;
         if (sliceCount <= 1) {
             vp.viewBase = 0; vp.N = N;
@@ -429,7 +484,7 @@ struct mv_engine {
                 vp.viewCost = d_viewCost.p; vp.order = d_viewCost.p + costItems(); vp.exitCounter = d_viewCost.p + costItems() + size_t(E);
             }
             if (progSlices > 0) { vp.sliceDone = d_sliceDone.p; vp.envsPerSlice = (E + progSlices - 1) / progSlices; }
-            const int rcl = launchView(vp, grid, overlap);
+            const int rcl = launchView(vp, grid, dep);
             if (rcl || progSlices <= 0) return rcl;
             // downloads: slice k as soon as all of its work items are drawn (cyclic >= comparison on the device counter)
             const size_t px = size_t(W) * H;
@@ -452,7 +507,7 @@ struct mv_engine {
         for (int base = 0, si = 0; base < N; base += perSlice, ++si) {
             const int cnt = std::min(perSlice, N - base);
             vp.viewBase = base; vp.N = cnt;
-            const int rc = launchView(vp, std::min(rasterGrid, cnt * rasterBands), overlap && si == 0);
+            const int rc = launchView(vp, std::min(rasterGrid, cnt * rasterBands), dep && si == 0);
             if (rc) return rc;
             while (int(sliceEv.size()) <= si) { cudaEvent_t e2; MV_CUDA(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming)); sliceEv.push_back(e2); }
             MV_CUDA(cudaEventRecord(sliceEv[size_t(si)], stream));
@@ -661,8 +716,130 @@ struct mv_engine {
         return MV_OK;
     }
 
+    // ------------------------------------------------------------------ state stores (mv_states_*)
+    // every per-env device row, in the order of StateStore::slabs
+    std::array<EnvSlab, kSlabCount> envSlabs() {
+        auto s = [](void *p, int units, size_t bytes) { return EnvSlab{static_cast<uint8_t *>(p), units, bytes}; };
+        return {{s(d_envs.p, 1, sizeof(MvEnvState)), s(d_agents.p, 1, sizeof(MvAgent) * A), s(d_objects.p, 1, sizeof(MvObject) * MV_MAX_OBJECTS),
+                 s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instCap), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
+                 s(d_views.p, 1, sizeof(float) * 16 * A), s(d_levels.p, 2, sizeof(MvLevel)), s(d_statics.p, 2, sizeof(MvBox) * staticCap),
+                 s(d_staticRot.p, 2, sizeof(float) * 2 * staticCap), s(d_deco.p, 2, sizeof(MvDeco) * decoCap), s(d_solid.p, 2, sizeof(uint32_t) * 3 * gridWords),
+                 s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t))}};
+    }
+    size_t stateRowBytes() {
+        size_t b = 0;
+        for (const EnvSlab &s : envSlabs()) b += s.rowBytes();
+        return b;
+    }
+    int statesCreate(int rows, int *id) {
+        auto st = std::make_unique<StateStore>();
+        st->rows = rows;
+        const auto sl = envSlabs();
+        for (int k = 0; k < kSlabCount; ++k)
+            if (st->slabs[k].alloc(size_t(rows) * sl[size_t(k)].rowBytes()) != cudaSuccess) { st->free(); setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
+        st->host.resize(size_t(rows));
+        stores.push_back(std::move(st));
+        *id = int(stores.size()) - 1;
+        return MV_OK;
+    }
+    // a save or load is a synchronisation point: outstanding asynchronous steps are retired and every generated level is uploaded first,
+    // so that no generation job still in flight can later overwrite a restored pre-staged slot
+    int quiesce() {
+        const int rc = drain();
+        return rc ? rc : flushUploads();
+    }
+    // one copy kernel over all listed rows, ev[0] / ev[1] around it.  toStore: engine row pairs[i].x -> store row pairs[i].y, else back.
+    int copyStateRows(StateStore &st, const int32_t *from, const int32_t *to, int n, bool toStore) {
+        if (size_t(n) > h_pairs.n) {
+            MV_CUDA(cudaStreamSynchronize(stream));  // the previous upload may still read the pinned pairs
+            h_pairs.free(); d_pairs.free();
+            if (h_pairs.alloc(size_t(n)) != cudaSuccess || d_pairs.alloc(size_t(n)) != cudaSuccess) { h_pairs.free(); d_pairs.free(); setError("state pairs: allocation failed"); return MV_ERR_CUDA; }
+        }
+        for (int i = 0; i < n; ++i) h_pairs.p[i] = make_int2(from[i], to[i]);
+        MV_CUDA(cudaMemcpyAsync(d_pairs.p, h_pairs.p, sizeof(int2) * size_t(n), cudaMemcpyHostToDevice, stream));
+        const auto sl = envSlabs();
+        mvs::Slab table[kSlabCount];
+        for (int k = 0; k < kSlabCount; ++k) {
+            uint8_t *eng = sl[size_t(k)].base, *sto = st.slabs[k].p;
+            const size_t rb = sl[size_t(k)].rowBytes();
+            table[k] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
+        }
+        MV_CUDA(cudaEventRecord(ev[0], stream));
+        MV_CUDA(mvs::copyRows(table, kSlabCount, d_pairs.p, n, stream));
+        MV_CUDA(cudaEventRecord(ev[1], stream));
+        launches += 1;
+        return MV_OK;
+    }
+    int statesSave(StateStore &st, const int32_t *envs, const int32_t *rows, int n) {
+        int rc = quiesce();
+        if (rc) return rc;
+        rc = copyStateRows(st, envs, rows, n, true);
+        if (rc) return rc;
+        for (int i = 0; i < n; ++i) {  // host state; the workers are idle (flushUploads waited for them)
+            const int e = envs[i];
+            StateStore::HostRow &r = st.host[size_t(rows[i])];
+            r.gen = gens[size_t(e)];
+            r.slot = hostSlot[size_t(e)]; r.episode = hostEpisode[size_t(e)];
+            for (int s = 0; s < 2; ++s) {
+                const size_t id = size_t(e) * 2 + s;
+                const MvLevel &L = h_levels.p[id];
+                r.level[s] = L;
+                r.words[s] = levelWords[id];
+                r.statics[s].assign(h_statics.p + id * staticCap, h_statics.p + id * staticCap + L.n_static);
+                r.staticRot[s].assign(h_staticRot.p + id * staticCap * 2, h_staticRot.p + (id * staticCap + L.n_static) * 2);
+                r.deco[s].assign(h_deco.p + id * decoCap, h_deco.p + id * decoCap + std::max(0, L.n_deco));
+                r.solid[s].clear();
+                for (int plane = 0; plane < 3; ++plane) {
+                    const uint32_t *src = h_solid.p + (id * 3 + plane) * gridWords;
+                    r.solid[s].insert(r.solid[s].end(), src, src + r.words[s]);
+                }
+            }
+        }
+        MV_CUDA(cudaStreamSynchronize(stream));
+        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
+        lastMs[1] = 0.0f;
+        return MV_OK;
+    }
+    int statesLoad(StateStore &st, const int32_t *rows, const int32_t *envs, int n) {
+        int rc = quiesce();
+        if (rc) return rc;
+        rc = copyStateRows(st, rows, envs, n, false);
+        if (rc) return rc;
+        // re-render every view (the others yield the same bytes again) and deliver as a step would: the loaded views then show the frames
+        // the saved step returned, and rewards / dones / true objectives read as they did after it
+        chooseDelivery(obsToHost);
+        rc = launchRaster(false);
+        if (rc) return rc;
+        MV_CUDA(cudaEventRecord(ev[2], stream));
+        for (int i = 0; i < n; ++i) {  // host state and mirrors, while the device copies and draws; no episode end: no afterFlip, no generation job
+            const int e = envs[i];
+            const StateStore::HostRow &r = st.host[size_t(rows[i])];
+            gens[size_t(e)] = *r.gen;
+            hostSlot[size_t(e)] = r.slot; hostEpisode[size_t(e)] = r.episode;
+            for (int s = 0; s < 2; ++s) {
+                const size_t id = size_t(e) * 2 + s;
+                h_levels.p[id] = r.level[s];
+                levelWords[id] = r.words[s];
+                std::copy(r.statics[s].begin(), r.statics[s].end(), h_statics.p + id * staticCap);
+                std::copy(r.staticRot[s].begin(), r.staticRot[s].end(), h_staticRot.p + id * staticCap * 2);
+                std::copy(r.deco[s].begin(), r.deco[s].end(), h_deco.p + id * decoCap);
+                for (int plane = 0; plane < 3; ++plane)
+                    std::copy_n(r.solid[s].begin() + ptrdiff_t(plane) * r.words[s], r.words[s], h_solid.p + (id * 3 + plane) * gridWords);
+            }
+            if (!lastAsyncDone.empty()) lastAsyncDone[size_t(e)] = -1000;  // the loaded env's last episode end is not this engine's
+        }
+        rc = finishStep(obsToHost);
+        if (rc) return rc;
+        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
+        cudaEventElapsedTime(&lastMs[1], ev[1], ev[2]);
+        return MV_OK;
+    }
+
     void freeAll() {
         if (pool) { pool->waitAll(); pool.reset(); }
+        for (auto &st : stores) if (st) st->free();
+        stores.clear();
+        h_pairs.free(); d_pairs.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
         d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_faults.free();
         hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free(); d_sliceDone.free();
@@ -1066,6 +1243,85 @@ int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out) {
     const int rc = h->drawHires(w, hgt);
     if (rc) return rc;
     if (out) *out = h->hires.h_obs.p;
+    return MV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ state stores
+static int statesCallState(mv_handle h, const char *fn) {
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    if (h->hostStepPending) { h->setError(std::string(fn) + ": mv_step_begin is outstanding, call mv_step_end first"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+static StateStore *findStore(mv_handle h, int store, const char *fn) {
+    if (store < 0 || store >= int(h->stores.size()) || !h->stores[size_t(store)]) { h->setError(std::string(fn) + ": no state store " + std::to_string(store)); return nullptr; }
+    return h->stores[size_t(store)].get();
+}
+// envs[i] in [0, E), rows[i] in [0, rows), and no destination twice: envs of a load (uniqueEnvs), rows of a save
+static int checkStatePairs(mv_handle h, const StateStore &st, const int32_t *envs, const int32_t *rows, int n, bool uniqueEnvs, const char *fn) {
+    if (n < 0 || (n > 0 && (!envs || !rows))) { h->setError(std::string(fn) + ": bad env / row arrays"); return MV_ERR_ARG; }
+    std::vector<uint8_t> seen(size_t(uniqueEnvs ? h->E : st.rows), 0);
+    for (int i = 0; i < n; ++i) {
+        if (envs[i] < 0 || envs[i] >= h->E) { h->setError(std::string(fn) + ": env " + std::to_string(envs[i]) + " out of range"); return MV_ERR_ARG; }
+        if (rows[i] < 0 || rows[i] >= st.rows) { h->setError(std::string(fn) + ": row " + std::to_string(rows[i]) + " out of range"); return MV_ERR_ARG; }
+        const int d = uniqueEnvs ? envs[i] : rows[i];
+        if (seen[size_t(d)]++) { h->setError(std::string(fn) + (uniqueEnvs ? ": env " : ": row ") + std::to_string(d) + " is a destination twice"); return MV_ERR_ARG; }
+    }
+    return MV_OK;
+}
+
+int mv_states_create(mv_handle h, int rows, int *store) {
+    if (!h || !store) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    int rc = statesCallState(h, "mv_states_create");
+    if (rc) return rc;
+    if (rows < 1) { h->setError("mv_states_create: rows must be positive"); return MV_ERR_ARG; }
+    return h->statesCreate(rows, store);
+}
+
+int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *rows, int n) {
+    if (!h) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    int rc = statesCallState(h, "mv_states_save");
+    if (rc) return rc;
+    StateStore *st = findStore(h, store, "mv_states_save");
+    if (!st) return MV_ERR_ARG;
+    rc = checkStatePairs(h, *st, envs, rows, n, false, "mv_states_save");
+    if (rc || n == 0) return rc;
+    return h->statesSave(*st, envs, rows, n);
+}
+
+int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *envs, int n) {
+    if (!h) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    int rc = statesCallState(h, "mv_states_load");
+    if (rc) return rc;
+    StateStore *st = findStore(h, store, "mv_states_load");
+    if (!st) return MV_ERR_ARG;
+    rc = checkStatePairs(h, *st, envs, rows, n, true, "mv_states_load");
+    if (rc || n == 0) return rc;
+    for (int i = 0; i < n; ++i)
+        if (!st->host[size_t(rows[i])].gen) { h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was never saved"); return MV_ERR_ARG; }
+    return h->statesLoad(*st, rows, envs, n);
+}
+
+int mv_states_destroy(mv_handle h, int store) {
+    if (!h) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    StateStore *st = findStore(h, store, "mv_states_destroy");
+    if (!st) return MV_ERR_ARG;
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
+    st->free();
+    h->stores[size_t(store)].reset();
+    return MV_OK;
+}
+
+int mv_state_row_bytes(mv_handle h, int64_t *out) {
+    if (!h || !out) return MV_ERR_ARG;
+    *out = int64_t(h->stateRowBytes());
     return MV_OK;
 }
 

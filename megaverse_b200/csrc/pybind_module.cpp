@@ -7,7 +7,7 @@
 //     (the reference would exit(-1) through TLOG(FATAL)).
 //   * extra batched methods (set_actions_batch, get_observations, get_dones, ...) next to the per-agent ones, because the
 //     reference's 2N+E+2 pybind round trips per step (SURVEY.md 3.2) would cap throughput far below the kernels.
-//   * the GIL is released around reset()/step().
+//   * the GIL is released around reset()/step() and around states_save()/states_load() (env state store, not in the reference).
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
@@ -184,6 +184,23 @@ public:
     int faultWord() { alive(); int32_t f; check(mv_fault_word(h__, &f)); return f; }
     void setOption(const std::string &key, int value) { alive(); check(mv_set_option(h__, key.c_str(), value)); }
     int levelsSkipped() { alive(); return mv_levels_skipped(h__); }
+    // env state store (include/megaverse_b200.h): save / load copy on the device and wait for it, so they run without the GIL
+    int statesCreate(int rows) { alive(); int id = -1; check(mv_states_create(h__, rows, &id)); return id; }
+    void statesSave(int store, const std::vector<int32_t> &envs, const std::vector<int32_t> &rows) {
+        alive();
+        if (envs.size() != rows.size()) throw std::invalid_argument("states_save: envs and rows differ in length");
+        int rc;
+        { py::gil_scoped_release nogil; rc = mv_states_save(h__, store, envs.data(), rows.data(), int(envs.size())); }
+        check(rc);
+    }
+    void statesLoad(int store, const std::vector<int32_t> &rows, const std::vector<int32_t> &envs) {
+        alive();
+        if (envs.size() != rows.size()) throw std::invalid_argument("states_load: rows and envs differ in length");
+        int rc;
+        { py::gil_scoped_release nogil; rc = mv_states_load(h__, store, rows.data(), envs.data(), int(envs.size())); }
+        check(rc);
+    }
+    void statesDestroy(int store) { alive(); check(mv_states_destroy(h__, store)); }
 
     void close() {
         if (h__) { mv_close(h__); h__ = nullptr; }
@@ -231,5 +248,9 @@ PYBIND11_MODULE(megaverse, m) {
         .def("faults", &MegaverseGym::faults)
         .def("fault_word", &MegaverseGym::faultWord)
         .def("set_option", &MegaverseGym::setOption)
-        .def("levels_skipped", &MegaverseGym::levelsSkipped);
+        .def("levels_skipped", &MegaverseGym::levelsSkipped)
+        .def("states_create", &MegaverseGym::statesCreate)
+        .def("states_save", &MegaverseGym::statesSave)
+        .def("states_load", &MegaverseGym::statesLoad)
+        .def("states_destroy", &MegaverseGym::statesDestroy);
 }

@@ -34,6 +34,24 @@ class MegaverseFault(RuntimeError):
     a NaN position, a level that arrived late): frames, rewards and dones from here on are not trustworthy"""
 
 
+class EnvState:
+    """(extension) env states saved by MegaverseEnv.save_state: owns one state store of the engine that made it; row i holds env envs[i]"""
+
+    def __init__(self, gym, store, envs):
+        self._gym, self._store, self.envs = gym, store, list(envs)
+
+    def close(self):
+        if self._store is not None:
+            self._gym.states_destroy(self._store)
+            self._store = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001  (the engine was closed first: mv_close freed the store)
+            pass
+
+
 class MegaverseEnv(Env):
     # The number of static boxes of a level is unbounded, as in the reference; the remaining fixed capacities (movable objects, reward
     # objects, terrain slabs) were never exceeded on hundreds of thousands of generated levels.  Should one be, the strict default makes
@@ -153,6 +171,28 @@ class MegaverseEnv(Env):
         env_idx = actor_idx // self.num_agents_per_env
         agent_idx = actor_idx % self.num_agents_per_env
         return self.env.set_reward_shaping(env_idx, agent_idx, reward_shaping)
+
+    def save_state(self, envs=None):
+        """(extension) save the complete state of `envs` (default: all) mid-episode; load_state rewinds to it or clones it"""
+        envs = list(range(self.num_envs)) if envs is None else [int(e) for e in envs]
+        store = self.env.states_create(len(envs))
+        state = EnvState(self.env, store, envs)
+        self.env.states_save(store, envs, list(range(len(envs))))
+        self.check_faults()
+        return state
+
+    def load_state(self, state, envs=None, rows=None):
+        """(extension) env envs[i] continues from the env saved in row rows[i] of `state` (row i = state.envs[i]); default: every row back into
+        the env it was saved from.  A row may go to several envs (clones).  Returns the observations, which equal the saved step's."""
+        if state._gym is not self.env:
+            raise ValueError("load_state: the state was saved by another env")
+        if rows is None:
+            rows = list(range(len(state.envs) if envs is None else len(envs)))
+        if envs is None:
+            envs = [state.envs[r] for r in rows]
+        self.env.states_load(state._store, [int(r) for r in rows], [int(e) for e in envs])
+        self.check_faults()
+        return self.observations()
 
     def levels_skipped(self):
         """(extension) levels replaced because they exceeded an engine capacity, see __init__"""
