@@ -31,6 +31,18 @@ typedef struct mv_engine *mv_handle;
  * numSimulationThreads drove Bullet on the CPU, vector_env.cpp:6-40).  device = CUDA ordinal. */
 int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents_per_env, int num_threads, int device,
               const char *const *param_keys, const float *param_vals, int nparams, mv_handle *out);
+/* Mixed-scenario engine (a multi-task batch, e.g. Megaverse-8, in ONE engine: one step kernel and one raster launch per step for all
+ * envs).  scenarios[e] names env e's scenario: any registered name (case-insensitive), repeated in any layout.  One render size, agent
+ * count and params dict for every env: each env starts from its own scenario's defaults and then takes the overrides.  Env e behaves
+ * exactly as env e of a single-scenario engine of its name (same levels, frames, rewards, dones for the same seed and actions), and
+ * reward shaping (mv_get / mv_set_reward_shaping) uses the keys of the env's scenario.  mv_create is this call with num_envs copies
+ * of one name.  Errors (MV_ERR_ARG, before any CUDA call): a null list, a null or unknown name (the message names the env), bad sizes,
+ * useUIRewardIndicators > 0.
+ * Memory: the per-env arrays keep one pitch per engine, that of the largest capacity among its scenarios.  With any Obstacles env in
+ * the batch every env costs 512 KiB of object grid plus 384 KiB of bit planes in HBM and 384 KiB of pinned host staging (1 024 envs:
+ * about 0.9 GiB of HBM and 384 MiB pinned); state-store rows grow to match (mv_state_row_bytes). */
+int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, int num_agents_per_env, int num_threads, int device,
+                    const char *const *param_keys, const float *param_vals, int nparams, mv_handle *out);
 /* message of the last failed call; pass NULL for a failed mv_create */
 const char *mv_last_error(mv_handle h);
 
@@ -141,6 +153,8 @@ int mv_stream(mv_handle h, void **stream);
  * mv_states_save: copies env envs[i] into row rows[i] (rows distinct).
  * mv_states_load: env envs[i] continues exactly as the env saved into row rows[i] would have (same frames, rewards, dones and later
  * levels for the same actions); envs distinct, a row may go to several envs (clones run the same level stream).  Other envs are untouched.
+ * A row loads only into an env of the saved env's scenario name (in a mixed engine, mv_create_mixed); otherwise the call is MV_ERR_ARG,
+ * names both scenarios and changes nothing.
  * Afterwards every view is drawn again and delivered as a step would (host buffer, HBM or mv_set_obs_buffer's, depth included): the
  * loaded views show the frames of the saved step, and rewards / dones / true objectives read as they did after it.  A load is not an
  * episode end.

@@ -3,7 +3,7 @@
 Only the per-step hot path is here (agent kinematics + collision, carry/place, reward/done, first-person rasteriser);
 see DESIGN.md.  `MegaverseEnv` mirrors megaverse/megaverse_env.py of the reference."""
 
-__all__ = ["MegaverseEnv", "make_env_multitask", "MEGAVERSE8"]
+__all__ = ["MegaverseEnv", "make_env_multitask", "make_env_mixed", "MEGAVERSE8"]
 
 
 def __getattr__(name):

@@ -27,6 +27,7 @@ def lib():
         L = C.CDLL(LIB_PATH)
         vp, ci, cf = C.c_void_p, C.c_int, C.c_float
         L.mv_create.argtypes = [C.c_char_p, ci, ci, ci, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(vp)]
+        L.mv_create_mixed.argtypes = [C.POINTER(C.c_char_p), ci, ci, ci, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(vp)]
         L.mv_last_error.argtypes = [vp]
         L.mv_last_error.restype = C.c_char_p
         for name in ("mv_reset", "mv_step", "mv_step_begin", "mv_step_end", "mv_close", "mv_sync", "mv_fetch_obs"):
@@ -61,7 +62,7 @@ def lib():
 
 
 EXPORTS = [
-    "mv_create", "mv_last_error", "mv_seed", "mv_seed_env", "mv_reset", "mv_set_actions", "mv_encode_action", "mv_step", "mv_step_begin", "mv_step_end", "mv_obs_host", "mv_depth_host",
+    "mv_create", "mv_create_mixed", "mv_last_error", "mv_seed", "mv_seed_env", "mv_reset", "mv_set_actions", "mv_encode_action", "mv_step", "mv_step_begin", "mv_step_end", "mv_obs_host", "mv_depth_host",
     "mv_rewards", "mv_dones", "mv_true_objectives", "mv_get_reward_shaping", "mv_set_reward_shaping", "mv_set_option", "mv_step_device", "mv_set_obs_buffer",
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
     "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view",
@@ -74,12 +75,20 @@ class Engine:
     """Thin object wrapper: one method per C entry point, numpy views over engine-owned host memory."""
 
     def __init__(self, scenario, num_envs, num_agents, w=128, h=72, num_threads=1, device=0, params=None, depth=False):
+        """scenario: one name for every env, or a list of num_envs names (env e runs scenario[e]: mv_create_mixed)"""
         L = lib()
         params = params or {}
         keys = (C.c_char_p * max(1, len(params)))(*[k.encode() for k in params])
         vals = (C.c_float * max(1, len(params)))(*[float(v) for v in params.values()])
         self._h = C.c_void_p()
-        rc = L.mv_create(scenario.encode(), w, h, num_envs, num_agents, num_threads, device, keys, vals, len(params), C.byref(self._h))
+        if isinstance(scenario, str):
+            rc = L.mv_create(scenario.encode(), w, h, num_envs, num_agents, num_threads, device, keys, vals, len(params), C.byref(self._h))
+        else:
+            names = list(scenario)
+            if len(names) != num_envs:
+                raise MegaverseError(MV_ERR_ARG, "%d scenario names for %d envs" % (len(names), num_envs))
+            arr = (C.c_char_p * max(1, num_envs))(*[n.encode() for n in names])
+            rc = L.mv_create_mixed(arr, w, h, num_envs, num_agents, num_threads, device, keys, vals, len(params), C.byref(self._h))
         if rc != MV_OK:
             raise MegaverseError(rc, (L.mv_last_error(None) or b"").decode())
         self.E, self.A, self.N, self.w, self.h = num_envs, num_agents, num_envs * num_agents, w, h

@@ -11,11 +11,14 @@
 // previous generation), and the step kernel flips to it by itself when the episode ends.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
+#include <cctype>
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
 #include <functional>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <optional>
@@ -131,6 +134,7 @@ struct StateStore {
     DevBuf<uint8_t> slabs[kSlabCount];  // same order as mv_engine::envSlabs()
     struct HostRow {
         std::optional<mv::LevelGenerator> gen;  // empty: the row was never saved
+        std::string scenario;                   // the saved env's scenario name: only an env of the same name may load the row
         int slot = 0, episode = 0, words[2] = {0, 0};
         // the host mirrors of both level slots that the debug dumps and the uploads read
         MvLevel level[2];
@@ -152,14 +156,16 @@ struct mv_engine {
     std::string error;
     void setError(const std::string &e) { error = e; }
 
-    std::string scenarioName;
-    int scenario = 0, W = 0, H = 0, E = 0, A = 0, N = 0, threads = 1, device = 0;
-    mv::FloatParams params;
+    int W = 0, H = 0, E = 0, A = 0, N = 0, threads = 1, device = 0;
+    // every env runs its own scenario (mv_create_mixed); mv_create gives all envs the same one
+    std::vector<std::string> envScenarioName;  // [E] the registered name the env was created with
+    std::vector<int> envScenario;              // [E] MV_SCENARIO_* of that name
     std::vector<std::vector<std::pair<std::string, float>>> shaping;  // per agent view: ordered key list (std::map order)
     std::vector<mv::LevelGenerator> gens;
     std::mt19937 master{std::random_device{}()};
     std::unique_ptr<WorkerPool> pool;
 
+    // pitch of the per-env grid arrays: the largest dense-grid capacity among the engine's scenarios (one pitch for all envs)
     int gridCells = 0, gridWords = 0;
     int triCap = 368;              // triangle-list capacity of one raster CTA (shared memory); larger views are drawn in several batches
     std::atomic<int> maxObjSeen{0};
@@ -280,12 +286,14 @@ struct mv_engine {
     void scheduleGen(int e, int s, int serial) {
         pool->submit([this, e, s, serial] {
             mv::LevelOut out;
+            // the env's own scenario's capacity, not the engine's pitch: a level is accepted exactly as in a single-scenario engine
+            const int cap = mv::gridCapacity(envScenario[size_t(e)]);
             try {
                 if (skipUnfitLevels) {
-                    const int skipped = gens[size_t(e)].generateFitting(out, serial, gridCells);
+                    const int skipped = gens[size_t(e)].generateFitting(out, serial, cap);
                     if (skipped) levelsSkipped.fetch_add(skipped);
                 } else {
-                    gens[size_t(e)].generate(out, serial, gridCells);
+                    gens[size_t(e)].generate(out, serial, cap);
                 }
             } catch (const std::exception &ex) {
                 std::lock_guard<std::mutex> lk(genMutex);
@@ -397,7 +405,8 @@ struct mv_engine {
             if (h_levels.p[id].n_deco > 0)
                 MV_CUDA(cudaMemcpyAsync(&d_deco.p[size_t(id) * size_t(decoCap)], &h_deco.p[size_t(id) * size_t(decoCap)], sizeof(MvDeco) * size_t(h_levels.p[id].n_deco), cudaMemcpyHostToDevice, stream));
             const size_t nw = size_t(levelWords[size_t(id)]);  // only the words this level's grid uses
-            for (int plane = 0; plane < ((scenario == MV_SCENARIO_TOWER || scenario == MV_SCENARIO_REARRANGE) ? 1 : 3); ++plane)
+            const int sc = h_levels.p[id].scenario;
+            for (int plane = 0; plane < ((sc == MV_SCENARIO_TOWER || sc == MV_SCENARIO_REARRANGE) ? 1 : 3); ++plane)
                 MV_CUDA(cudaMemcpyAsync(d_solid.p + (size_t(id) * 3 + plane) * gridWords, h_solid.p + (size_t(id) * 3 + plane) * gridWords, sizeof(uint32_t) * nw, cudaMemcpyHostToDevice, stream));
         }
         return MV_OK;
@@ -406,8 +415,9 @@ struct mv_engine {
     void fillRtableRow(int view) {
         float *row = h_rtable.p + size_t(view) * MV_R_COUNT;
         for (int i = 0; i < MV_R_COUNT; ++i) row[i] = 0.0f;
+        const int sc = envScenario[size_t(view / A)];
         for (auto &kv : shaping[size_t(view)]) {
-            const int slot = mv::rewardSlot(scenario, kv.first);
+            const int slot = mv::rewardSlot(sc, kv.first);
             if (slot >= 0) row[slot] = kv.second;
         }
     }
@@ -779,6 +789,7 @@ struct mv_engine {
             const int e = envs[i];
             StateStore::HostRow &r = st.host[size_t(rows[i])];
             r.gen = gens[size_t(e)];
+            r.scenario = envScenarioName[size_t(e)];
             r.slot = hostSlot[size_t(e)]; r.episode = hostEpisode[size_t(e)];
             for (int s = 0; s < 2; ++s) {
                 const size_t id = size_t(e) * 2 + s;
@@ -903,12 +914,26 @@ const char *mv_last_error(mv_handle h) { return h ? h->error.c_str() : g_createE
 
 int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents, int num_threads, int device, const char *const *keys, const float *vals,
               int nparams, mv_handle *out) {
+    const std::vector<const char *> names(size_t(std::max(num_envs, 0)), scenario);
+    return mv_create_mixed(names.data(), w, h, num_envs, num_agents, num_threads, device, keys, vals, nparams, out);
+}
+
+int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, int num_agents, int num_threads, int device, const char *const *keys,
+                    const float *vals, int nparams, mv_handle *out) {
     if (!out) return MV_ERR_ARG;
     *out = nullptr;
-    const int sc = scenario ? mv::scenarioFromName(scenario) : -1;
-    if (sc < 0) { g_createError = std::string("unknown scenario ") + (scenario ? scenario : "(null)"); return MV_ERR_ARG; }
-    if (w <= 0 || h <= 0 || w % 32 != 0 || h % 4 != 0 || (w / 32) * (h / 4) > 128) { g_createError = "render size must be a multiple of 32x4 with at most 128 tiles"; return MV_ERR_ARG; }
     if (num_envs <= 0 || num_agents <= 0 || num_agents > MV_MAX_AGENTS) { g_createError = "bad num_envs / num_agents_per_env"; return MV_ERR_ARG; }
+    if (!scenarios) { g_createError = "null scenario list"; return MV_ERR_ARG; }
+    std::vector<std::string> names(static_cast<size_t>(num_envs));
+    std::vector<int> scs(static_cast<size_t>(num_envs));
+    for (int i = 0; i < num_envs; ++i) {
+        const char *s = scenarios[i];
+        scs[size_t(i)] = s ? mv::scenarioFromName(s) : -1;
+        if (scs[size_t(i)] < 0) { g_createError = std::string("unknown scenario ") + (s ? s : "(null)") + " for env " + std::to_string(i); return MV_ERR_ARG; }
+        names[size_t(i)] = s;
+        for (char &c : names[size_t(i)]) c = char(std::tolower(static_cast<unsigned char>(c)));  // one spelling per scenario (the state store compares them)
+    }
+    if (w <= 0 || h <= 0 || w % 32 != 0 || h % 4 != 0 || (w / 32) * (h / 4) > 128) { g_createError = "render size must be a multiple of 32x4 with at most 128 tiles"; return MV_ERR_ARG; }
     for (int i = 0; i < nparams; ++i) {
         if (!keys || !keys[i] || !vals) { g_createError = "null parameter key / value array"; return MV_ERR_ARG; }
         // the interactive viewer's reward-indicator HUD (scenario_default.hpp:144-160, set by viewer_app.cpp:147 only) adds drawables this
@@ -925,28 +950,37 @@ int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents, 
     auto fail = [&](int code) { g_createError = e->error; e->freeAll(); delete e; return code; };
     DeviceGuard dg__(device);
     if (!dg__.ok) { e->setError("cudaSetDevice failed"); return fail(MV_ERR_CUDA); }
-    e->scenario = sc; e->W = w; e->H = h; e->E = num_envs; e->A = num_agents; e->N = num_envs * num_agents; e->device = device;
+    e->W = w; e->H = h; e->E = num_envs; e->A = num_agents; e->N = num_envs * num_agents; e->device = device;
     e->threads = num_threads < 1 ? 1 : num_threads;
-    e->scenarioName = scenario;
-    e->params = mv::defaultFloatParams(e->scenarioName);
-    for (int i = 0; i < nparams; ++i) e->params[keys[i]] = vals[i];
-    {
-        auto def = mv::defaultRewardShaping(e->scenarioName);
-        std::map<std::string, float> m{{"teamSpirit", 0.0f}};
-        for (auto &kv : def) m[kv.first] = kv.second;
-        std::vector<std::pair<std::string, float>> ordered(m.begin(), m.end());
-        e->shaping.assign(size_t(e->N), ordered);
-    }
+    e->envScenarioName = names;
+    e->envScenario = scs;
+    e->shaping.resize(size_t(e->N));
     try {
-        for (int i = 0; i < e->E; ++i) e->gens.emplace_back(e->scenarioName, e->A, e->params);
+        // every env starts from its own scenario's defaults and then takes the overrides (make_env_multitask passes one dict to every task)
+        std::map<std::string, mv::FloatParams> params;
+        std::map<std::string, std::vector<std::pair<std::string, float>>> shaping;
+        for (int i = 0; i < e->E; ++i) {
+            const std::string &name = names[size_t(i)];
+            if (!params.count(name)) {
+                mv::FloatParams &p = params[name];
+                p = mv::defaultFloatParams(name);
+                for (int k = 0; k < nparams; ++k) p[keys[k]] = vals[k];
+                std::map<std::string, float> m{{"teamSpirit", 0.0f}};
+                for (auto &kv : mv::defaultRewardShaping(name)) m[kv.first] = kv.second;
+                shaping[name].assign(m.begin(), m.end());
+            }
+            e->gens.emplace_back(name, e->A, params[name]);
+            for (int a = 0; a < e->A; ++a) e->shaping[size_t(i) * e->A + a] = shaping[name];
+        }
     } catch (const std::exception &ex) {  // e.g. Sokoban without a Boxoban dataset (the reference exit()s here, scenario_sokoban.cpp:76-78)
         e->setError(ex.what());
         return fail(MV_ERR_ARG);
     }
     e->levelWords.assign(size_t(e->E) * 2, 0);
     e->pool.reset(new WorkerPool(e->threads));
-    e->gridCells = mv::gridCapacity(sc);
-    e->decoCap = mv::decoCapacity(sc);
+    // one pitch for all envs: the largest capacity among the engine's scenarios
+    e->gridCells = 0; e->decoCap = 0;
+    for (int sc : scs) { e->gridCells = std::max(e->gridCells, mv::gridCapacity(sc)); e->decoCap = std::max(e->decoCap, mv::decoCapacity(sc)); }
     e->instCap = MV_DYN_INSTANCES + e->staticCap + e->decoCap;
     e->gridWords = e->gridCells / 32;
     fillConsts(e->consts, w, h);
@@ -1302,8 +1336,17 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
     if (!st) return MV_ERR_ARG;
     rc = checkStatePairs(h, *st, envs, rows, n, true, "mv_states_load");
     if (rc || n == 0) return rc;
-    for (int i = 0; i < n; ++i)
-        if (!st->host[size_t(rows[i])].gen) { h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was never saved"); return MV_ERR_ARG; }
+    for (int i = 0; i < n; ++i) {
+        const StateStore::HostRow &r = st->host[size_t(rows[i])];
+        if (!r.gen) { h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was never saved"); return MV_ERR_ARG; }
+        // the generator travels by value and the reward-shaping row stays with the env: a row of another scenario would turn the env into
+        // that scenario with a reward table that does not fit it
+        if (r.scenario != h->envScenarioName[size_t(envs[i])]) {
+            h->setError("mv_states_load: row " + std::to_string(rows[i]) + " holds a " + r.scenario + " env, env " + std::to_string(envs[i]) + " runs " +
+                        h->envScenarioName[size_t(envs[i])]);
+            return MV_ERR_ARG;
+        }
+    }
     return h->statesLoad(*st, rows, envs, n);
 }
 
@@ -1411,8 +1454,8 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
     // makes the reference throw std::out_of_range at the next reward event (scenario.hpp:253) -> reject it up front
     std::map<std::string, float> m;
     for (int i = 0; i < n; ++i) m[keys[i]] = vals[i];
-    for (auto &kv : mv::defaultRewardShaping(h->scenarioName))
-        if (!m.count(kv.first)) { h->setError("reward shaping lacks key " + kv.first); return MV_ERR_ARG; }
+    for (auto &kv : mv::defaultRewardShaping(h->envScenarioName[size_t(env)]))  // the keys of this env's scenario
+        if (!m.count(kv.first)) { h->setError("reward shaping lacks key " + kv.first + " of env " + std::to_string(env) + "'s scenario " + h->envScenarioName[size_t(env)]); return MV_ERR_ARG; }
     const size_t view = size_t(env) * h->A + agent;
     h->shaping[view].assign(m.begin(), m.end());
     h->fillRtableRow(int(view));

@@ -8,10 +8,12 @@
 //   * extra batched methods (set_actions_batch, get_observations, get_dones, ...) next to the per-agent ones, because the
 //     reference's 2N+E+2 pybind round trips per step (SURVEY.md 3.2) would cap throughput far below the kernels.
 //   * the GIL is released around reset()/step() and around states_save()/states_load() (env state store, not in the reference).
+//   * a second constructor takes a list of num_envs scenario names: a mixed-scenario batch in one engine (mv_create_mixed).
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -32,16 +34,22 @@ class MegaverseGym {
 public:
     MegaverseGym(const std::string &scenario, int w, int h, int numEnvs, int numAgentsPerEnv, int numSimulationThreads, bool useVulkan,
                  const std::map<std::string, float> &floatParams)
+        : MegaverseGym(std::vector<std::string>(size_t(std::max(numEnvs, 0)), scenario), w, h, numEnvs, numAgentsPerEnv, numSimulationThreads, useVulkan, floatParams) {}
+    // (extension) a mixed-scenario batch: env e runs scenarios[e] (mv_create_mixed)
+    MegaverseGym(const std::vector<std::string> &scenarios, int w, int h, int numEnvs, int numAgentsPerEnv, int numSimulationThreads, bool useVulkan,
+                 const std::map<std::string, float> &floatParams)
         : numEnvs_(numEnvs), numAgentsPerEnv_(numAgentsPerEnv), w_(w), h_(h) {
         (void)useVulkan;
-        std::vector<const char *> keys;
+        if (numEnvs > 0 && int(scenarios.size()) != numEnvs) throw std::invalid_argument("MegaverseGym: one scenario name per env expected");
+        std::vector<const char *> names, keys;
         std::vector<float> vals;
+        for (auto &s : scenarios) names.push_back(s.c_str());
         for (auto &kv : floatParams) { keys.push_back(kv.first.c_str()); vals.push_back(kv.second); }
         // the reference's constructor has no device argument (one process per GPU, CUDA_VISIBLE_DEVICES): MEGAVERSE_B200_DEVICE picks the
         // ordinal for processes that see several GPUs
         int device = 0;
         if (const char *dv = std::getenv("MEGAVERSE_B200_DEVICE")) device = std::atoi(dv);
-        const int rc = mv_create(scenario.c_str(), w, h, numEnvs, numAgentsPerEnv, numSimulationThreads, device, keys.data(), vals.data(), int(keys.size()), &h__);
+        const int rc = mv_create_mixed(names.data(), w, h, numEnvs, numAgentsPerEnv, numSimulationThreads, device, keys.data(), vals.data(), int(keys.size()), &h__);
         if (rc != MV_OK) throw std::runtime_error(std::string("MegaverseGym: ") + mv_last_error(nullptr));
         masks_.assign(size_t(numEnvs) * numAgentsPerEnv, 0);
     }
@@ -221,6 +229,7 @@ PYBIND11_MODULE(megaverse, m) {
     m.def("set_megaverse_log_level", &setMegaverseLogLevel, "Megaverse Log Level (0 to disable all logs, 2 for warnings");
     py::class_<MegaverseGym>(m, "MegaverseGym")
         .def(py::init<const std::string &, int, int, int, int, int, bool, const std::map<std::string, float> &>())
+        .def(py::init<const std::vector<std::string> &, int, int, int, int, int, bool, const std::map<std::string, float> &>())
         .def("num_agents", &MegaverseGym::numAgents)
         .def("action_space_sizes", &MegaverseGym::actionSpaceSizes)
         .def("seed", &MegaverseGym::seed)

@@ -666,11 +666,14 @@ __device__ int rearrangeCountMatches(const WarpShared &S, const MvLevel &L) {
 }
 
 // ---------------------------------------------------------------- episode (re)initialisation from a level slot
-__device__ void resetEnv(WarpShared &S, const MvLevel &L, uint8_t *objGrid, int gridCells, int A, int lane) {
-    // voxel -> object map
+__device__ void resetEnv(WarpShared &S, const MvLevel &L, uint8_t *objGrid, int A, int lane) {
+    // voxel -> object map: only the words that cover this level's grid.  Every reader bounds its index by grid_dim (gridIndex), so the
+    // bytes beyond it are never read; the product fits the scenario's capacity (the generator checks it) and the row pitch is a
+    // multiple of 128 cells, so rounding up to whole words stays inside the row.
     {
         uint32_t *g32 = reinterpret_cast<uint32_t *>(objGrid);
-        for (int i = lane; i < gridCells / 4; i += 32) g32[i] = 0xffffffffu;
+        const int words = (L.grid_dim[0] * L.grid_dim[1] * L.grid_dim[2] + 3) / 4;
+        for (int i = lane; i < words; i += 32) g32[i] = 0xffffffffu;
         __syncwarp();
     }
     for (int i = lane; i < L.n_obj; i += 32) {
@@ -1418,7 +1421,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
         }
         __syncwarp();
         ns = L->n_static; no = L->n_obj;
-        resetEnv(S, *L, objGrid, P.gridCells, A, lane);
+        resetEnv(S, *L, objGrid, A, lane);
         // all objects are fresh: write the whole array back
         {
             const uint32_t *src = reinterpret_cast<const uint32_t *>(&S.objects[0]);

@@ -14,16 +14,26 @@ MEGAVERSE8 = ['TowerBuilding', 'ObstaclesEasy', 'ObstaclesHard', 'Collect', 'Sok
 OBSTACLES_MULTITASK = ['ObstaclesWalls', 'ObstaclesSteps', 'ObstaclesLava', 'ObstaclesEasy', 'ObstaclesHard']
 
 
-def make_env_multitask(multitask_name, task_idx, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None):
+def _multitask_tasks(multitask_name):
     assert 'multitask' in multitask_name
     if multitask_name.endswith('megaverse8'):
-        tasks = MEGAVERSE8
+        return MEGAVERSE8
     elif multitask_name.endswith('obstacles'):
-        tasks = OBSTACLES_MULTITASK
+        return OBSTACLES_MULTITASK
     else:
         raise NotImplementedError()
+
+
+def make_env_multitask(multitask_name, task_idx, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None):
+    tasks = _multitask_tasks(multitask_name)
     scenario = tasks[task_idx % len(tasks)]
     return MegaverseEnv(scenario, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan, params)
+
+
+def make_env_mixed(multitask_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None):
+    """(extension) the whole multi-task set in ONE env: env i runs tasks[i % len(tasks)], all stepped and drawn by one engine"""
+    tasks = _multitask_tasks(multitask_name)
+    return MegaverseEnv([tasks[i % len(tasks)] for i in range(num_envs)], num_envs, num_agents_per_env, num_simulation_threads, use_vulkan, params)
 
 
 FAULT_NAMES = {1: "LEVEL_NOT_READY", 2: "TRI_OVERFLOW", 4: "GRID_RANGE", 8: "NAN", 16: "ENVELOPE", 32: "CAND_OVERFLOW"}  # csrc/mv_types.h
@@ -60,7 +70,15 @@ class MegaverseEnv(Env):
     SKIP_UNFIT_LEVELS = False
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None):
-        scenario_name = scenario_name.casefold()
+        # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
+        if isinstance(scenario_name, str):
+            scenario_name = scenario_name.casefold()
+            self.scenarios = [scenario_name] * num_envs
+        else:
+            scenario_name = [s.casefold() for s in scenario_name]
+            if len(scenario_name) != num_envs:
+                raise ValueError('%d scenario names for %d envs' % (len(scenario_name), num_envs))
+            self.scenarios = list(scenario_name)
         self.scenario_name = scenario_name
         self.is_multiagent = True
         set_megaverse_log_level(2)
@@ -84,6 +102,11 @@ class MegaverseEnv(Env):
         if self.SKIP_UNFIT_LEVELS:
             self.env.set_option("skip_unfit_levels", 1)
         self.default_shaping_scheme = self.env.get_reward_shaping(0, 0)
+        # each scenario's default scheme, read from its first env before anyone could change it
+        self._default_shaping = {}
+        for env_i, s in enumerate(self.scenarios):
+            if s not in self._default_shaping:
+                self._default_shaping[s] = self.env.get_reward_shaping(env_i, 0)
         self.action_space = self.generate_action_space(self.env.action_space_sizes())
         self.observation_space = Box(0, 255, (self.channels, self.img_h, self.img_w), dtype=np.uint8)
 
@@ -159,8 +182,11 @@ class MegaverseEnv(Env):
                 pass
         return obs_final
 
-    def get_default_reward_shaping(self):
-        return self.default_shaping_scheme
+    def get_default_reward_shaping(self, actor_idx=None):
+        """env 0's default scheme; with actor_idx, the default of that actor's scenario (they differ in a mixed batch)"""
+        if actor_idx is None:
+            return self.default_shaping_scheme
+        return dict(self._default_shaping[self.scenarios[actor_idx // self.num_agents_per_env]])
 
     def get_current_reward_shaping(self, actor_idx: int):
         env_idx = actor_idx // self.num_agents_per_env
