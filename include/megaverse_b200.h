@@ -117,6 +117,24 @@ int mv_set_option(mv_handle h, const char *key, int value);
  * mv_step_device: like mv_step but takes the action masks from DEVICE memory (NULL = the engine's own buffer, see
  * mv_actions_device) and leaves the observation tensor on the device; rewards/dones still land on the host. */
 int mv_step_device(mv_handle h, const int32_t *d_masks);
+/* mv_step_device with per-env episode ends requested from the device: d_ends = uint8[num_envs] in DEVICE memory (NULL = none, which is
+ * mv_step_device), read in the engine stream's order (mv_stream).  An env with d_ends[e] != 0 ends its episode at this step, after this
+ * step's actions and scenario rules ran, exactly as a timer end: done = 1, reward 0, the true objective reported, flip to the pre-staged
+ * next level, and the frame of this step is the new episode's first.  A request for an env whose current episode has run fewer than 3
+ * steps (its step counter is below 3 after this step) is ignored: this call retires step k-2 at call k, so the next level of an env that
+ * ended one or two steps ago is not staged yet.  The rule depends on the step count only, never on host timing. */
+int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends);
+/* Restart chosen envs now: envs[i] start a new episode.  seeds == NULL: each continues its own level stream (it takes its pre-staged
+ * next level, as at a natural episode end); else env envs[i] is first reseeded with seeds[i] and plays the first level of that stream --
+ * it then behaves exactly as env envs[i] of a fresh engine after mv_seed_env and mv_reset (unlike mv_seed_env, a Sokoban env also drops
+ * the rest of its shuffled level list, as a fresh engine has none).  Other envs are untouched.
+ * Every view is drawn again and delivered as a step would (host buffer, HBM or mv_set_obs_buffer's, depth included; the other views
+ * yield the same bytes); the restarted envs read reward 0 and done 0, as after mv_reset.  The episode counter keeps counting.
+ * A synchronisation point like mv_states_load: it retires outstanding mv_step_device steps, and on return the restarted envs' levels after
+ * next are generated and uploaded.  MV_ERR_ARG (n < 0, a null list with n > 0, an env out of range or listed twice) and MV_ERR_STATE
+ * (before mv_reset, an outstanding mv_step_begin) change nothing; n == 0 does nothing.  Afterwards mv_last_kernel_ms gives [0] the
+ * reset kernel and [1] the re-render. */
+int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n);
 /* Redirect the HBM output of the rasteriser into caller-owned device memory: d_obs = uint8[N][h][w][4] (and d_depth = float[N][h][w]
  * when option depth is on; NULL keeps the engine's own).  Lets several engines -- one per scenario of a multi-task batch, reference
  * megaverse_env.py:27-39 -- write into slices of ONE contiguous tensor that a consumer or an NCCL gather reads without a staging copy.

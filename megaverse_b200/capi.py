@@ -37,6 +37,8 @@ def lib():
         L.mv_set_actions.argtypes = [vp, vp]
         L.mv_encode_action.argtypes = [vp]
         L.mv_step_device.argtypes = [vp, vp]
+        L.mv_step_device_ends.argtypes = [vp, vp, vp]
+        L.mv_reset_envs.argtypes = [vp, vp, vp, ci]
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
@@ -67,7 +69,7 @@ EXPORTS = [
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
     "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view",
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
-    "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes",
+    "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
 ]
 
 
@@ -133,8 +135,20 @@ class Engine:
         """second half: wait; obs() / rewards() / dones() are then valid as after step()"""
         self._ck(lib().mv_step_end(self._h))
 
-    def step_device(self, d_masks_ptr=None):
-        self._ck(lib().mv_step_device(self._h, C.c_void_p(d_masks_ptr) if d_masks_ptr else None))
+    def step_device(self, d_masks_ptr=None, d_ends_ptr=None):
+        """d_ends_ptr: optional device uint8[E]; a non-zero entry ends that env's episode at this step (mv_step_device_ends)"""
+        m = C.c_void_p(d_masks_ptr) if d_masks_ptr else None
+        if d_ends_ptr is None:
+            self._ck(lib().mv_step_device(self._h, m))
+        else:
+            self._ck(lib().mv_step_device_ends(self._h, m, C.c_void_p(d_ends_ptr) if d_ends_ptr else None))
+
+    def reset_envs(self, envs, seeds=None):
+        """envs[i] start a new episode now; with seeds, env envs[i] is reseeded with seeds[i] first (mv_reset_envs)"""
+        e = np.ascontiguousarray(envs, dtype=np.int32)
+        s = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.int32)
+        assert s is None or s.size == e.size
+        self._ck(lib().mv_reset_envs(self._h, e.ctypes.data if e.size else None, None if s is None else s.ctypes.data, e.size))
 
     def set_obs_buffer(self, d_obs_ptr=None, d_depth_ptr=None):
         """rasterise into caller-owned device memory (a slice of a larger tensor) instead of the engine's own obs buffer"""

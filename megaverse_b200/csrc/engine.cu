@@ -280,6 +280,8 @@ struct mv_engine {
     std::vector<std::unique_ptr<StateStore>> stores;  // mv_states_create ids; null once destroyed
     PinBuf<int2> h_pairs;                              // (source row, destination row) of the last save / load
     DevBuf<int2> d_pairs;
+    PinBuf<uint32_t> h_envList;                        // [E] the envs of the last mv_reset_envs
+    DevBuf<uint32_t> d_envList;
 
     // ------------------------------------------------------------------ level generation scheduling
     // generate the level for episode `serial` of env e into staging slot s (worker thread)
@@ -422,7 +424,7 @@ struct mv_engine {
         }
     }
 
-    int launchStep(const int32_t *dActions, bool forceReset, Pending *mirror = nullptr) {
+    mvk::StepParams stepParams(const int32_t *dActions, bool forceReset, Pending *mirror, const uint8_t *dEnds) {
         mvk::StepParams sp;
         sp.hostRewards = mirror ? mirror->rewards.p : nullptr; sp.hostTrueObjectives = mirror ? mirror->trueObj.p : nullptr;
         sp.hostDones = mirror ? mirror->dones.p : nullptr;
@@ -434,16 +436,26 @@ struct mv_engine {
         sp.deco = d_deco.p; sp.decoCap = decoCap; sp.instStride = instCap;
         sp.ready = d_ready.p; sp.readyStamp = ++readyStamp;
         sp.envOrder = rasterSched ? d_viewCost.p + costItems() : nullptr;  // a permutation at all times (identity until a cost-ordered raster launch has sorted it)
+        sp.ends = dEnds;
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
         sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = gridWords; sp.forceReset = forceReset ? 1 : 0;
         sp.k = consts;
+        return sp;
+    }
+    // one warp per env of sp.E (sp.envOrder[w] when given)
+    int launchStepKernel(const mvk::StepParams &sp) {
         const int warpsPerBlock = 2;
-        const int blocks = (E + warpsPerBlock - 1) / warpsPerBlock;
+        const int blocks = (sp.E + warpsPerBlock - 1) / warpsPerBlock;
         const size_t smem = sizeof(mvk::WarpShared) * warpsPerBlock;
-        const bool timing = !(mirror && overlap);  // the asynchronous fast path carries no timing events
-        if (timing) MV_CUDA(cudaEventRecord(ev[0], stream));
         mvk::stepKernel<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
+        return MV_OK;
+    }
+    int launchStep(const int32_t *dActions, bool forceReset, Pending *mirror = nullptr, const uint8_t *dEnds = nullptr) {
+        const mvk::StepParams sp = stepParams(dActions, forceReset, mirror, dEnds);
+        const bool timing = !(mirror && overlap);  // the asynchronous fast path carries no timing events
+        if (timing) MV_CUDA(cudaEventRecord(ev[0], stream));
+        if (const int rck = launchStepKernel(sp)) return rck;
         if (!overlap) MV_CUDA(cudaEventRecord(ev[1], stream));  // an event between the two kernels would serialise them
         launches += 1;
         int rc = launchRaster();
@@ -666,7 +678,7 @@ struct mv_engine {
     }
     // asynchronous device-resident step: returns after enqueueing.  Episode bookkeeping lags two steps, which is safe
     // because an env cannot finish twice within four steps (doneWithTimer leaves 0.3 s = 4.5 steps, scenario.hpp:114-117)
-    int stepAsync(const int32_t *dActions) {
+    int stepAsync(const int32_t *dActions, const uint8_t *dEnds) {
         if (!didReset) { setError("mv_step_device before mv_reset"); return MV_ERR_STATE; }
         if (hostStepPending) { const int rcp = stepEnd(); if (rcp) return rcp; }
         if (asyncContractBroken) { setError("mv_step_device: an episode lasted fewer than 3 steps -- outside the asynchronous call's contract; use mv_step"); return MV_ERR_STATE; }
@@ -685,7 +697,7 @@ struct mv_engine {
             rtableDirty = false;
         }
         rasterToHost = false; sliceCount = 1; progSlices = 0;
-        rc = launchStep(dActions, false, &slotP);  // rewards / dones / true objectives land in the ring slot straight from the kernel
+        rc = launchStep(dActions, false, &slotP, dEnds);  // rewards / dones / true objectives land in the ring slot straight from the kernel
         if (rc) return rc;
         MV_CUDA(cudaEventRecord(slotP.ev, stream));
         slotP.valid = true;
@@ -846,11 +858,56 @@ struct mv_engine {
         return MV_OK;
     }
 
+    // ------------------------------------------------------------------ per-env restart (mv_reset_envs)
+    // The forced flip of mv_reset over the listed envs only (the step kernel steps sp.envOrder[0..n)), then a re-render of the batch as after
+    // a state load.  A synchronisation point: on return the restarted envs' levels after next are generated and uploaded, so the
+    // asynchronous call's three-step rule holds from the next mv_step_device on.
+    int resetEnvs(const int32_t *envs, const int32_t *seeds, int n) {
+        int rc = quiesce();
+        if (rc) return rc;
+        if (seeds) {  // the staged slot takes the first level of the new stream, as in a fresh engine; the workers are idle after quiesce
+            for (int i = 0; i < n; ++i) {
+                const int e = envs[i];
+                gens[size_t(e)].restart((unsigned long)seeds[i]);
+                scheduleGen(e, hostSlot[size_t(e)] ^ 1, hostEpisode[size_t(e)] + 1);
+            }
+            rc = flushUploads();
+            if (rc) return rc;
+        }
+        for (int i = 0; i < n; ++i) h_envList.p[i] = uint32_t(envs[i]);
+        MV_CUDA(cudaMemcpyAsync(d_envList.p, h_envList.p, sizeof(uint32_t) * size_t(n), cudaMemcpyHostToDevice, stream));
+        mvk::StepParams sp = stepParams(d_actions.p, true, nullptr, nullptr);
+        sp.envOrder = d_envList.p; sp.E = n;
+        MV_CUDA(cudaEventRecord(ev[0], stream));
+        rc = launchStepKernel(sp);
+        if (rc) return rc;
+        launches += 1;
+        MV_CUDA(cudaEventRecord(ev[1], stream));
+        // every view is drawn again (the others yield the same bytes) and delivered as a step would
+        chooseDelivery(obsToHost);
+        rc = launchRaster(false);
+        if (rc) return rc;
+        MV_CUDA(cudaEventRecord(ev[2], stream));
+        std::vector<uint8_t> flipped(size_t(E), 0);
+        for (int i = 0; i < n; ++i) {
+            flipped[size_t(envs[i])] = 1;
+            if (!lastAsyncDone.empty()) lastAsyncDone[size_t(envs[i])] = -1000;  // a restart is not an asynchronous episode end
+        }
+        afterFlip(flipped.data());  // the levels after next, generated while the device draws
+        rc = flushUploads();
+        if (rc) return rc;
+        rc = finishStep(obsToHost);
+        if (rc) return rc;
+        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
+        cudaEventElapsedTime(&lastMs[1], ev[1], ev[2]);
+        return MV_OK;
+    }
+
     void freeAll() {
         if (pool) { pool->waitAll(); pool.reset(); }
         for (auto &st : stores) if (st) st->free();
         stores.clear();
-        h_pairs.free(); d_pairs.free();
+        h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
         d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_faults.free();
         hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free(); d_sliceDone.free();
@@ -1017,7 +1074,8 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     if (ok && e->configureRaster() != MV_OK) return fail(MV_ERR_CUDA);
     ok = ok && ck(e->h_levels.alloc(E * 2), "h_levels") && ck(e->h_solid.alloc(E * 2 * 3 * e->gridWords), "h_solid") && ck(e->h_actions.alloc(N), "h_actions") &&
          ck(e->h_rtable.alloc(N * MV_R_COUNT), "h_rtable") && ck(e->h_rewards.alloc(N), "h_rewards") && ck(e->h_dones.alloc(E), "h_dones") &&
-         ck(e->h_trueObj.alloc(N), "h_trueObj") && ck(e->h_obs.alloc(N * px * 4), "h_obs") && ck(e->h_faults.alloc(E), "h_faults") && ck(e->h_faultWord.alloc(1), "h_faultWord");
+         ck(e->h_trueObj.alloc(N), "h_trueObj") && ck(e->h_obs.alloc(N * px * 4), "h_obs") && ck(e->h_faults.alloc(E), "h_faults") && ck(e->h_faultWord.alloc(1), "h_faultWord") &&
+         ck(e->h_envList.alloc(E), "h_envList") && ck(e->d_envList.alloc(E), "envList");
     for (auto &p : e->ring) ok = ok && ck(cudaEventCreateWithFlags(&p.ev, cudaEventDisableTiming), "event") && ck(p.rewards.alloc(N), "ring") && ck(p.trueObj.alloc(N), "ring") && ck(p.dones.alloc(E), "ring");
     if (!ok) return fail(MV_ERR_CUDA);
     std::memset(e->h_actions.p, 0, sizeof(int32_t) * N);
@@ -1213,11 +1271,13 @@ int mv_step_end(mv_handle h) {
     return h->stepEnd();
 }
 
-int mv_step_device(mv_handle h, const int32_t *d_masks) {
+int mv_step_device(mv_handle h, const int32_t *d_masks) { return mv_step_device_ends(h, d_masks, nullptr); }
+
+int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends) {
     if (!h) return MV_ERR_ARG;
     DeviceGuard dg__(h->device);
     if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
-    return h->stepAsync(d_masks ? d_masks : h->d_actions.p);
+    return h->stepAsync(d_masks ? d_masks : h->d_actions.p, d_ends);
 }
 
 // host-only: the colour tables of the level generators followed by the rasteriser's palette (float bit patterns), in the layout of
@@ -1348,6 +1408,22 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
         }
     }
     return h->statesLoad(*st, rows, envs, n);
+}
+
+int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n) {
+    if (!h) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    int rc = statesCallState(h, "mv_reset_envs");
+    if (rc) return rc;
+    if (n < 0 || (n > 0 && !envs)) { h->setError("mv_reset_envs: bad env array"); return MV_ERR_ARG; }
+    std::vector<uint8_t> seen(size_t(h->E), 0);
+    for (int i = 0; i < n; ++i) {
+        if (envs[i] < 0 || envs[i] >= h->E) { h->setError("mv_reset_envs: env " + std::to_string(envs[i]) + " out of range"); return MV_ERR_ARG; }
+        if (seen[size_t(envs[i])]++) { h->setError("mv_reset_envs: env " + std::to_string(envs[i]) + " is listed twice"); return MV_ERR_ARG; }
+    }
+    if (n == 0) return MV_OK;
+    return h->resetEnvs(envs, seeds, n);
 }
 
 int mv_states_destroy(mv_handle h, int store) {

@@ -33,6 +33,9 @@ class LevelGenerator {
 public:
     LevelGenerator(const std::string &scenarioName, int numAgents, const FloatParams &params);
     void seed(unsigned long s) { rng_.seed(s); }
+    // the generator as constructed and then seeded: its stream starts again from its first level (Sokoban draws a fresh shuffle of its
+    // level files instead of continuing the unplayed ones)
+    void restart(unsigned long s) { rng_.seed(s); sokobanLevels_.clear(); }
     // Generates the next episode's level.  gridCells = capacity of the dense grid (cells); throws std::runtime_error
     // if the level does not fit one of the engine's fixed capacities (the number of static boxes is not one of them).
     void generate(LevelOut &out, int serial, int gridCells);

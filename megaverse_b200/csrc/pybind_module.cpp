@@ -7,7 +7,8 @@
 //     (the reference would exit(-1) through TLOG(FATAL)).
 //   * extra batched methods (set_actions_batch, get_observations, get_dones, ...) next to the per-agent ones, because the
 //     reference's 2N+E+2 pybind round trips per step (SURVEY.md 3.2) would cap throughput far below the kernels.
-//   * the GIL is released around reset()/step() and around states_save()/states_load() (env state store, not in the reference).
+//   * the GIL is released around reset()/step(), around states_save()/states_load() (env state store, not in the reference) and around
+//     reset_envs() (restart chosen envs, not in the reference).
 //   * a second constructor takes a list of num_envs scenario names: a mixed-scenario batch in one engine (mv_create_mixed).
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
@@ -17,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -209,6 +211,14 @@ public:
         check(rc);
     }
     void statesDestroy(int store) { alive(); check(mv_states_destroy(h__, store)); }
+    // restart chosen envs now, optionally reseeded (mv_reset_envs); a synchronisation point like states_load, run without the GIL
+    void resetEnvs(const std::vector<int32_t> &envs, std::optional<std::vector<int32_t>> seeds) {
+        alive();
+        if (seeds && seeds->size() != envs.size()) throw std::invalid_argument("reset_envs: envs and seeds differ in length");
+        int rc;
+        { py::gil_scoped_release nogil; rc = mv_reset_envs(h__, envs.data(), seeds ? seeds->data() : nullptr, int(envs.size())); }
+        check(rc);
+    }
 
     void close() {
         if (h__) { mv_close(h__); h__ = nullptr; }
@@ -261,5 +271,6 @@ PYBIND11_MODULE(megaverse, m) {
         .def("states_create", &MegaverseGym::statesCreate)
         .def("states_save", &MegaverseGym::statesSave)
         .def("states_load", &MegaverseGym::statesLoad)
-        .def("states_destroy", &MegaverseGym::statesDestroy);
+        .def("states_destroy", &MegaverseGym::statesDestroy)
+        .def("reset_envs", &MegaverseGym::resetEnvs, py::arg("envs"), py::arg("seeds") = py::none());
 }

@@ -68,6 +68,7 @@ struct StepParams {
     uint32_t *ready;             // [E] completion stamps polled by the geometry kernel (programmatic dependent launch)
     uint32_t readyStamp;
     const uint32_t *envOrder;  // optional [E]: warp w of the grid steps env envOrder[w] (the order in which the rasteriser will ask for the envs)
+    const uint8_t *ends;         // optional [num_envs] (mv_step_device_ends): ends[env] != 0 ends the episode at this step, once it has run >= 3 steps
     int maxObj;                  // upper bound of n_obj over the live and staged levels (sizes the staging copy)
     uint32_t *prof;              // optional [E][16] per-phase cycle stamps (mv_debug_step_profile); nullptr in production
     MvConsts k;
@@ -1383,7 +1384,8 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
             }
             for (int i = 0; i < A; ++i) S.agents[i].total_reward += S.lastReward[i];
             e.num_frames += 1;
-            S.doneFlag = (e.episode_sec >= len) ? 1 : 0;
+            // a requested end (mv_step_device_ends) is a timer end; before the third step the env's next level may not be staged yet
+            S.doneFlag = (e.episode_sec >= len || (P.ends && P.ends[env] && e.num_frames >= 3)) ? 1 : 0;
         }
         __syncwarp();
         doneFlag = S.doneFlag != 0;

@@ -220,6 +220,13 @@ class MegaverseEnv(Env):
         self.check_faults()
         return self.observations()
 
+    def reset_envs(self, envs, seeds=None):
+        """(extension) envs[i] start a new episode now, the other envs keep going; with seeds, env envs[i] first takes seed seeds[i] and
+        plays the first level of that stream.  Returns the observations of every agent, like reset()."""
+        self.env.reset_envs([int(e) for e in envs], None if seeds is None else [int(s) for s in seeds])
+        self.check_faults()
+        return self.observations()
+
     def levels_skipped(self):
         """(extension) levels replaced because they exceeded an engine capacity, see __init__"""
         return self.env.levels_skipped()
