@@ -206,6 +206,13 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap);
 int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap);
 int mv_debug_get_instances(mv_handle h, int env, float *out, int cap);
 int mv_debug_get_view(mv_handle h, int env, int agent, float *out16);
+/* test hook: put agent `agent` of env `env` somewhere else, as the character controller's warp does (the oracle's orc_scen_warp):
+ * position pos[3] and basis9 (rows) are set, horizontal and vertical velocity become 0, nothing else changes.  The caller supplies all
+ * twelve floats (e.g. read back from the oracle after its warp), so no rounding happens here.  Nothing is drawn: the next step renders
+ * the warped agent.  A synchronisation point like mv_states_save: outstanding mv_step_device steps are retired first.  MV_ERR_STATE
+ * before mv_reset or with an mv_step_begin outstanding; MV_ERR_ARG for an env or agent out of range, a null pointer or a non-finite
+ * value.  On any error nothing changes. */
+int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]);
 /* render caller-supplied instances (18 floats each: mesh, colour, 16 model) with one view matrix through the CUDA
  * rasteriser: rgba uint8[h][w][4], depth float[h][w] or NULL.  Host pointers. */
 int mv_debug_render_instances(const float *view16, const float *inst18, int n, int w, int h, uint8_t *rgba, float *depth);

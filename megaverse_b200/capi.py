@@ -51,6 +51,7 @@ def lib():
         for name in ("mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances"):
             getattr(L, name).argtypes = [vp, ci, vp, ci]
         L.mv_debug_get_view.argtypes = [vp, ci, ci, vp]
+        L.mv_debug_warp_agent.argtypes = [vp, ci, ci, vp, vp]
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
         L.mv_debug_bzset.argtypes = [vp, ci, vp, ci]
         L.mv_debug_generate_level.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp, ci]
@@ -67,7 +68,7 @@ EXPORTS = [
     "mv_create", "mv_create_mixed", "mv_last_error", "mv_seed", "mv_seed_env", "mv_reset", "mv_set_actions", "mv_encode_action", "mv_step", "mv_step_begin", "mv_step_end", "mv_obs_host", "mv_depth_host",
     "mv_rewards", "mv_dones", "mv_true_objectives", "mv_get_reward_shaping", "mv_set_reward_shaping", "mv_set_option", "mv_step_device", "mv_set_obs_buffer",
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
-    "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view",
+    "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view", "mv_debug_warp_agent",
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
 ]
@@ -323,6 +324,13 @@ class Engine:
         out = np.zeros(16, dtype=np.float32)
         self._ck(lib().mv_debug_get_view(self._h, env, agent, out.ctypes.data))
         return out
+
+    def warp_agent(self, env, agent, pos, basis):
+        """test hook (mv_debug_warp_agent): set the agent's position and basis rows, zero its velocities; drawn by the next step"""
+        p = np.ascontiguousarray(pos, dtype=np.float32)
+        b = np.ascontiguousarray(basis, dtype=np.float32)
+        assert p.size == 3 and b.size == 9
+        self._ck(lib().mv_debug_warp_agent(self._h, int(env), int(agent), p.ctypes.data, b.ctypes.data))
 
 
 def render_instances(view16, inst18, w, h, want_depth=False):

@@ -14,7 +14,9 @@
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <cmath>
 #include <condition_variable>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <functional>
@@ -903,6 +905,18 @@ struct mv_engine {
         return MV_OK;
     }
 
+    // test hook (mv_debug_warp_agent): w16 = pos[3], basis[9], hvel[3], vvel -- the head of MvAgent, written in one copy after the
+    // asynchronous ring is retired.  Every other position-derived value (colliders, candidate lists, object_t, views) is rebuilt from
+    // MvAgent::pos by the next step kernel.
+    int warpAgent(int env, int agent, const float *w16) {
+        static_assert(offsetof(MvAgent, basis) == 12 && offsetof(MvAgent, hvel) == 48 && offsetof(MvAgent, vvel) == 60, "MvAgent head layout");
+        const int rc = quiesce();
+        if (rc) return rc;
+        MV_CUDA(cudaMemcpyAsync(&d_agents.p[size_t(env) * A + agent], w16, sizeof(float) * 16, cudaMemcpyHostToDevice, stream));
+        MV_CUDA(cudaStreamSynchronize(stream));
+        return MV_OK;
+    }
+
     void freeAll() {
         if (pool) { pool->waitAll(); pool.reset(); }
         for (auto &st : stores) if (st) st->free();
@@ -1745,6 +1759,23 @@ int mv_debug_get_view(mv_handle h, int env, int agent, float *out16) {
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(out16, h->d_views.p + (size_t(env) * h->A + agent) * 16, 64, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     return MV_OK;
+}
+
+int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]) {
+    if (!h) return MV_ERR_ARG;
+    DeviceGuard dg__(h->device);
+    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    int rc = statesCallState(h, "mv_debug_warp_agent");
+    if (rc) return rc;
+    if (env < 0 || env >= h->E || agent < 0 || agent >= h->A) { h->setError("mv_debug_warp_agent: env / agent out of range"); return MV_ERR_ARG; }
+    if (!pos || !basis9) { h->setError("mv_debug_warp_agent: null pointer"); return MV_ERR_ARG; }
+    // MvAgent starts with pos[3], basis[9], hvel[3], vvel: one contiguous 16-float write
+    float w[16] = {};
+    std::memcpy(w, pos, 12);
+    std::memcpy(w + 3, basis9, 36);
+    for (int k = 0; k < 12; ++k)
+        if (!std::isfinite(w[k])) { h->setError("mv_debug_warp_agent: non-finite value"); return MV_ERR_ARG; }
+    return h->warpAgent(env, agent, w);
 }
 
 int mv_debug_render_instances(const float *view16, const float *inst18, int n, int w, int h, uint8_t *rgba, float *depth) {
