@@ -27,6 +27,13 @@ typedef struct mv_engine *mv_handle;
 #define MV_ERR_CAPACITY -3     /* a generated level exceeds the engine's fixed capacities */
 #define MV_ERR_STATE -4        /* call order (e.g. step before reset) */
 
+/* why an episode ended (mv_done_reasons): one byte per env and step, beside the done flag */
+#define MV_END_NONE 0          /* not done (also every env after mv_reset, and the envs mv_reset_envs restarted) */
+#define MV_END_TIME 1          /* the episode clock ran out: truncated */
+#define MV_END_SOLVED 2        /* a scenario rule solved the level (doneWithTimer), also when a request or the clock ends it in the
+                                * 0.3 s grace that follows: terminal */
+#define MV_END_REQUESTED 3     /* the caller's end mask (mv_step_device_ends): truncated */
+
 /* MegaverseGym::MegaverseGym (megaverse.cpp:38-58).  num_threads = host level-generation workers (the reference's
  * numSimulationThreads drove Bullet on the CPU, vector_env.cpp:6-40).  device = CUDA ordinal. */
 int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents_per_env, int num_threads, int device,
@@ -81,6 +88,27 @@ int mv_rewards(mv_handle h, const float **out);
 int mv_dones(mv_handle h, const uint8_t **out);
 /* VectorEnv::trueObjectives / MegaverseGym::trueObjective (megaverse.cpp:209-212): float[N] */
 int mv_true_objectives(mv_handle h, const float **out);
+/* uint8[num_envs] MV_END_* of the last step, host memory, valid like mv_dones (non-zero exactly where dones is 1).  A state-store row carries
+ * them: after mv_states_load they read as after the saved step. */
+int mv_done_reasons(mv_handle h, const uint8_t **out);
+/* Terminal frames, option "final_obs" (before the first reset).  For every env that ends in a step (dones[e] == 1), views e*A .. e*A+A-1
+ * of the final-frame buffer get the frame that step would have drawn had the episode not ended: the scene after this step's actions,
+ * physics, scenario rules and HUD update, before the flip to the next level -- the s_T a truncated episode is bootstrapped from.  Same
+ * size and layout as the observation tensor (and the depth tensor when option depth is on).  Rows of envs that did not end are not
+ * written: a row keeps the terminal frame of the env's last end.
+ * Host-facing steps (mv_step, mv_step_begin/end with obs_to_host 1) store the rows straight into the host buffer (mv_final_obs_host), on
+ * return like the observations; mv_step_device[_ends] stores them into the device buffer (mv_final_obs_device) in stream order, and
+ * mv_fetch_obs then copies the whole device buffer into the host one.  mv_reset, mv_reset_envs and mv_states_load draw no terminal frame.
+ * Nothing else changes with the option: obs, depth, rewards, dones and true objectives are byte-identical with it on and off.
+ * Cost: a device and a pinned host buffer each as large as the observation tensor (+ depth), e.g. 151 MB each at Collect 1 024 x 4 and
+ * 128 x 72, and one more instance row per env in HBM: 552 + static_cap + decoration slots of 80 B, 103 KiB per env at the default
+ * static_cap (223 KiB in the hex mazes, whose decorations take 1 536 slots).  Time: one raster launch per step that draws only the ended
+ * envs' views, and the ending envs' warps write their terminal rows (DESIGN.md section 3 has the measured costs).
+ * MV_ERR_ARG when the option (or, for depth, option depth) is off; MV_ERR_STATE before mv_reset. */
+int mv_final_obs_host(mv_handle h, const uint8_t **out);
+int mv_final_depth_host(mv_handle h, const float **out);
+int mv_final_obs_device(mv_handle h, uint8_t **d_final_obs);
+int mv_final_depth_device(mv_handle h, float **d_final_depth);
 
 /* MegaverseGym::getRewardShaping / setRewardShaping (megaverse.cpp:214-222).  get: fills up to cap entries, returns the
  * number of keys in *n.  Key strings are owned by the engine. */
@@ -109,6 +137,7 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * objects, terrain slabs, the dense grid -- makes mv_step / mv_reset fail with MV_ERR_CAPACITY, and keeps failing: the env would
  * otherwise leave the reference's level sequence; with 1 the env takes the next level of its stream instead and mv_levels_skipped
  * counts it),
+ * "final_obs" (0/1, before the first reset, default 0: terminal frames of ended episodes, see mv_final_obs_host),
  * "overlap" (0/1, default 1: the raster kernel is a programmatic dependent launch of the step kernel and synchronises per env;
  * 0 serialises the kernels so that mv_last_kernel_ms can time them separately) */
 int mv_set_option(mv_handle h, const char *key, int value);
@@ -159,6 +188,9 @@ int mv_obs_device(mv_handle h, uint8_t **d_obs);
 int mv_depth_device(mv_handle h, float **d_depth);
 int mv_rewards_device(mv_handle h, float **d_rewards);
 int mv_dones_device(mv_handle h, uint8_t **d_dones);
+/* uint8[num_envs] MV_END_* and float[N] true objectives of the last step in HBM, written by the step kernel in stream order */
+int mv_done_reasons_device(mv_handle h, uint8_t **d_reasons);
+int mv_true_objectives_device(mv_handle h, float **d_true_objectives);
 /* the CUDA stream (cudaStream_t) all engine work is ordered on */
 int mv_stream(mv_handle h, void **stream);
 
@@ -196,6 +228,9 @@ int mv_fault_word(mv_handle h, int32_t *out);
 int mv_kernel_launches(mv_handle h, int64_t *out);
 /* device time of the last step's kernels in milliseconds: [0] step kernel, [1] raster kernel (CUDA events) */
 int mv_last_kernel_ms(mv_handle h, float *out2);
+/* device time of the last step's terminal-frame launch (option "final_obs") in milliseconds, CUDA events; 0 when the step had none or
+ * carried no timing events (mv_step_device with option overlap 1).  With it, mv_last_kernel_ms [1] is the step's own raster launch. */
+int mv_last_final_ms(mv_handle h, float *out);
 
 /* MegaverseGym::close (megaverse.cpp:224-243) */
 int mv_close(mv_handle h);

@@ -11,6 +11,7 @@ LIB_PATH = os.environ.get("MV_B200_LIB") or os.path.join(_PKG, "libmegaverse_b20
 _lib = None
 
 MV_OK, MV_ERR_ARG, MV_ERR_CUDA, MV_ERR_CAPACITY, MV_ERR_STATE = 0, -1, -2, -3, -4
+MV_END_NONE, MV_END_TIME, MV_END_SOLVED, MV_END_REQUESTED = 0, 1, 2, 3  # done_reasons(): why an episode ended
 
 
 class MegaverseError(RuntimeError):
@@ -40,7 +41,8 @@ def lib():
         L.mv_step_device_ends.argtypes = [vp, vp, vp]
         L.mv_reset_envs.argtypes = [vp, vp, vp, ci]
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
-                     "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream"):
+                     "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
+                     "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
         L.mv_get_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(ci)]
         L.mv_set_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci]
@@ -48,6 +50,7 @@ def lib():
         L.mv_faults.argtypes = [vp, C.POINTER(C.c_int32)]
         L.mv_kernel_launches.argtypes = [vp, C.POINTER(C.c_int64)]
         L.mv_last_kernel_ms.argtypes = [vp, C.POINTER(cf)]
+        L.mv_last_final_ms.argtypes = [vp, C.POINTER(cf)]
         for name in ("mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances"):
             getattr(L, name).argtypes = [vp, ci, vp, ci]
         L.mv_debug_get_view.argtypes = [vp, ci, ci, vp]
@@ -71,6 +74,8 @@ EXPORTS = [
     "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view", "mv_debug_warp_agent",
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
+    "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
+    "mv_final_depth_device", "mv_last_final_ms",
 ]
 
 
@@ -170,8 +175,12 @@ class Engine:
     def device_array(self, what="obs"):
         """zero-copy handle on an engine-owned device tensor for any consumer of the CUDA array interface
         (`torch.as_tensor(eng.device_array("obs"), device="cuda")`, CuPy, Numba): "obs" uint8[N,h,w,4], "depth" float32[N,h,w],
-        "rewards" float32[N], "dones" uint8[E].  Valid in the engine stream's order (mv_stream) until mv_close."""
-        shapes = {"obs": ((self.N, self.h, self.w, 4), "|u1"), "depth": ((self.N, self.h, self.w), "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1")}
+        "rewards" float32[N], "dones" uint8[E], "done_reasons" uint8[E] (MV_END_*), "true_objectives" float32[N], and with option final_obs
+        "final_obs" uint8[N,h,w,4] / "final_depth" float32[N,h,w] (terminal frames of mv_step_device steps).  Valid in the engine stream's
+        order (mv_stream) until mv_close."""
+        frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
+        shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
+                  "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4")}
         shape, typestr = shapes[what]
         ptr, stream = self.device_ptr(what), self.stream()
 
@@ -204,6 +213,17 @@ class Engine:
 
     def true_objectives(self):
         return self._host("mv_true_objectives", (self.N,), np.float32)
+
+    def done_reasons(self):
+        """uint8[E] MV_END_* of the last step: 0 not done, 1 time limit, 2 solved, 3 requested"""
+        return self._host("mv_done_reasons", (self.E,), np.uint8)
+
+    def final_obs(self):
+        """uint8[N,h,w,4] terminal frames (option final_obs): views of env e hold the frame its last episode ended on"""
+        return self._host("mv_final_obs_host", (self.N, self.h, self.w, 4), np.uint8)
+
+    def final_depth(self):
+        return self._host("mv_final_depth_host", (self.N, self.h, self.w), np.float32)
 
     def device_ptr(self, what):
         p = C.c_void_p()
@@ -297,6 +317,12 @@ class Engine:
         out = (C.c_float * 2)()
         self._ck(lib().mv_last_kernel_ms(self._h, out))
         return float(out[0]), float(out[1])
+
+    def last_final_ms(self):
+        """device time of the last step's terminal-frame launch (mv_last_final_ms)"""
+        out = C.c_float()
+        self._ck(lib().mv_last_final_ms(self._h, C.byref(out)))
+        return float(out.value)
 
     # ---- introspection (tests)
     def _dump(self, fn, env, dtype, cap=1 << 16):

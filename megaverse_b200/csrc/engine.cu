@@ -128,7 +128,7 @@ struct EnvSlab {
     size_t rowBytes() const { return size_t(units) * unitBytes; }
 };
 // indices into mv_engine::envSlabs() of the arrays that growStatics re-pitches
-enum { kSlabInst = 4, kSlabStatics = 8, kSlabStaticRot = 9, kSlabCount = 16 };
+enum { kSlabInst = 4, kSlabStatics = 8, kSlabStaticRot = 9, kSlabCount = 17 };
 
 // saved env states (mv_states_*): every per-env device row in arrays of `rows` rows with the engine's pitch, plus the host state
 struct StateStore {
@@ -216,6 +216,7 @@ struct mv_engine {
     DevBuf<float> d_rtable;
     DevBuf<float> d_rewards;
     DevBuf<uint8_t> d_dones;
+    DevBuf<uint8_t> d_doneReasons;  // [E] MV_END_* beside d_dones
     DevBuf<float> d_trueObj;
     DevBuf<uint8_t> d_obs;
     DevBuf<float> d_depth;
@@ -255,6 +256,7 @@ struct mv_engine {
     PinBuf<float> h_rtable;
     PinBuf<float> h_rewards;
     PinBuf<uint8_t> h_dones;
+    PinBuf<uint8_t> h_doneReasons;
     PinBuf<float> h_trueObj;
     PinBuf<uint8_t> h_obs;
     PinBuf<float> h_depth;
@@ -262,7 +264,7 @@ struct mv_engine {
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
     // mv_step_device pipeline: results of step k are consumed by the host while steps k+1, k+2 already run
-    struct Pending { bool valid = false; uint64_t step = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones; };
+    struct Pending { bool valid = false; uint64_t step = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; };
     std::vector<int64_t> lastAsyncDone;  // [E] asynchronous step index of the env's previous episode end
     bool asyncContractBroken = false;
     Pending ring[3];
@@ -284,6 +286,24 @@ struct mv_engine {
     DevBuf<int2> d_pairs;
     PinBuf<uint32_t> h_envList;                        // [E] the envs of the last mv_reset_envs
     DevBuf<uint32_t> d_envList;
+
+    // terminal frames (option "final_obs", allocated at the first reset): an env that ends in a step gets the frame that step would have
+    // drawn had the episode not ended.  The step kernel writes the ending envs' terminal rows (instances at the pitch of d_inst, counts,
+    // views); a masked raster launch over d_dones draws their views into the final-frame buffers: the pinned host ones for host-facing
+    // steps, HBM for mv_step_device.  Rows of envs that did not end are never written.
+    bool wantFinal = false;
+    bool finalOnDevice = false;     // the last terminal-frame launch stored into HBM (mv_fetch_obs copies the buffers down)
+    bool lastHadFinal = false;      // the last timed step ran a terminal-frame launch (ev[3] .. ev[2])
+    float lastFinalMs = 0.0f;
+    int finalGrid = 0;              // persistent grid of the masked raster variants
+    cudaEvent_t evFinal = nullptr;
+    DevBuf<MvInstance> d_termInst;  // [E][instCap]
+    DevBuf<int32_t> d_termCounts;   // [E][8]
+    DevBuf<float> d_termViews;      // [N][16]
+    DevBuf<uint8_t> d_finalObs;     // [N][H][W][4]
+    DevBuf<float> d_finalDepth;     // [N][H][W], with option depth
+    PinBuf<uint8_t> h_finalObs;
+    PinBuf<float> h_finalDepth;
 
     // ------------------------------------------------------------------ level generation scheduling
     // generate the level for episode `serial` of env e into staging slot s (worker thread)
@@ -379,6 +399,10 @@ struct mv_engine {
         d_statics.free(); d_staticRot.free(); d_inst.free(); h_statics.free(); h_staticRot.free();
         d_statics = nStat; d_staticRot = nRot; d_inst = nInst; h_statics = hStat; h_staticRot = hRot;
         staticCap = newCap; instCap = newInstCap;
+        if (d_termInst.p) {  // no copy: a terminal row is written whole before the launch that reads it
+            d_termInst.free();
+            if (d_termInst.alloc(size_t(E) * size_t(instCap)) != cudaSuccess) { setError("growing the terminal instance rows: allocation failed"); return MV_ERR_CUDA; }
+        }
         return MV_OK;
     }
     int flushUploads() {
@@ -439,6 +463,8 @@ struct mv_engine {
         sp.ready = d_ready.p; sp.readyStamp = ++readyStamp;
         sp.envOrder = rasterSched ? d_viewCost.p + costItems() : nullptr;  // a permutation at all times (identity until a cost-ordered raster launch has sorted it)
         sp.ends = dEnds;
+        sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
+        sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
         sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = gridWords; sp.forceReset = forceReset ? 1 : 0;
         sp.k = consts;
@@ -462,8 +488,31 @@ struct mv_engine {
         launches += 1;
         int rc = launchRaster();
         if (rc) return rc;
+        lastHadFinal = false;
+        if (wantFinal && !forceReset) {  // after the step's own frames: the terminal frames of the envs that ended (stream order, no stamps)
+            if (timing) MV_CUDA(cudaEventRecord(evFinal, stream));
+            rc = launchFinal(mirror == nullptr);
+            if (rc) return rc;
+            lastHadFinal = timing;
+        }
         if (timing) MV_CUDA(cudaEventRecord(ev[2], stream));
         return MV_OK;
+    }
+    // the masked raster launch over the terminal rows: every (view, band) item of an env whose d_dones byte is set, into the final-frame
+    // buffers -- pinned host memory (stored through UVA, like the zero-copy obs rows) or HBM
+    int launchFinal(bool toHost) {
+        mvr::ViewParams vp = {};
+        vp.instances = d_termInst.p; vp.instCounts = d_termCounts.p; vp.views = d_termViews.p; vp.instStride = instCap;
+        vp.obs = toHost ? h_finalObs.p : d_finalObs.p; vp.depth = wantDepth ? (toHost ? h_finalDepth.p : d_finalDepth.p) : nullptr;
+        vp.spill = d_spill.p; vp.spillStride = spillStride; vp.consumed = nullptr; vp.stats = nullptr;
+        vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4; vp.triCap = triCap;
+        vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
+        vp.ready = nullptr; vp.readyStamp = 0;
+        vp.viewBase = 0; vp.N = N;
+        vp.envMask = d_dones.p;
+        finalOnDevice = !toHost;
+        const int grid = std::min(rasterGridCap > 0 ? std::min(finalGrid, rasterGridCap) : finalGrid, N * rasterBands);
+        return launchView(vp, grid, false);
     }
     // One persistent launch over all (view, band) items.  Every CTA makes exactly one failing claim when the queue is empty, so the
     // work counter advances by items + grid per launch and the host keeps the base instead of resetting the counter (no memset node
@@ -477,7 +526,10 @@ struct mv_engine {
         attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr; cfg.numAttrs = dependent ? 1 : 0;
-        if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true>, vp));
+        if (vp.envMask) {
+            if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true, true>, vp));
+            else MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<false, true>, vp));
+        } else if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true>, vp));
         else MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<false>, vp));
         launches += 1;
         return MV_OK;
@@ -609,6 +661,15 @@ struct mv_engine {
             rasterCtasPerSM = fast ? std::min(rasterCtasPerSM, perSM) : perSM;
         }
         rasterGrid = numSMs * rasterCtasPerSM;
+        int finalPerSM = 0;
+        for (int fast = 0; fast < 2; ++fast) {  // the masked variants (terminal frames) size their own grid
+            const void *fn = fast ? reinterpret_cast<const void *>(mvr::viewKernel<true, true>) : reinterpret_cast<const void *>(mvr::viewKernel<false, true>);
+            MV_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, maxOptin));
+            int perSM = 0;
+            MV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, mvr::kThreads, rasterSmem));
+            finalPerSM = fast ? std::min(finalPerSM, perSM) : perSM;
+        }
+        finalGrid = numSMs * std::max(1, std::min(finalPerSM, rasterCtasPerSM));  // shares d_spill, sized by rasterGrid
         const int bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
         spillStride = W * bandRows;
         d_spill.free();
@@ -633,12 +694,15 @@ struct mv_engine {
     void readKernelTimes() {
         if (cudaEventQuery(ev[2]) != cudaSuccess) return;
         if (overlap) { lastMs[0] = -1.0f; cudaEventElapsedTime(&lastMs[1], ev[0], ev[2]); }
-        else { cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], ev[2]); }
+        else { cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], lastHadFinal ? evFinal : ev[2]); }
+        lastFinalMs = 0.0f;
+        if (lastHadFinal) cudaEventElapsedTime(&lastFinalMs, evFinal, ev[2]);
     }
 
     int finishStep(bool copyObs, bool wait = true) {
         MV_CUDA(cudaMemcpyAsync(h_rewards.p, d_rewards.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
+        MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
         if (copyObs && !rasterToHost && sliceCount <= 1 && progSlices <= 0) {
             MV_CUDA(cudaMemcpyAsync(h_obs.p, obsOut, size_t(N) * W * H * 4, cudaMemcpyDeviceToHost, stream));
@@ -657,6 +721,7 @@ struct mv_engine {
         MV_CUDA(cudaEventSynchronize(p.ev));
         std::memcpy(h_rewards.p, p.rewards.p, sizeof(float) * N);
         std::memcpy(h_dones.p, p.dones.p, E);
+        std::memcpy(h_doneReasons.p, p.reasons.p, E);
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
         p.valid = false;
         // the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes again sooner
@@ -748,7 +813,8 @@ struct mv_engine {
                  s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instCap), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
                  s(d_views.p, 1, sizeof(float) * 16 * A), s(d_levels.p, 2, sizeof(MvLevel)), s(d_statics.p, 2, sizeof(MvBox) * staticCap),
                  s(d_staticRot.p, 2, sizeof(float) * 2 * staticCap), s(d_deco.p, 2, sizeof(MvDeco) * decoCap), s(d_solid.p, 2, sizeof(uint32_t) * 3 * gridWords),
-                 s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t))}};
+                 s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t)),
+                 s(d_doneReasons.p, 1, 1)}};
     }
     size_t stateRowBytes() {
         size_t b = 0;
@@ -788,6 +854,7 @@ struct mv_engine {
             const size_t rb = sl[size_t(k)].rowBytes();
             table[k] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
         }
+        lastHadFinal = false;
         MV_CUDA(cudaEventRecord(ev[0], stream));
         MV_CUDA(mvs::copyRows(table, kSlabCount, d_pairs.p, n, stream));
         MV_CUDA(cudaEventRecord(ev[1], stream));
@@ -880,6 +947,7 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(d_envList.p, h_envList.p, sizeof(uint32_t) * size_t(n), cudaMemcpyHostToDevice, stream));
         mvk::StepParams sp = stepParams(d_actions.p, true, nullptr, nullptr);
         sp.envOrder = d_envList.p; sp.E = n;
+        lastHadFinal = false;
         MV_CUDA(cudaEventRecord(ev[0], stream));
         rc = launchStepKernel(sp);
         if (rc) return rc;
@@ -927,8 +995,11 @@ struct mv_engine {
         hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free(); d_sliceDone.free();
         h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free();
         h_faults.free(); h_faultWord.free();
+        d_doneReasons.free(); h_doneReasons.free();
+        d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
         for (auto &e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
-        for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); }
+        if (evFinal) { cudaEventDestroy(evFinal); evFinal = nullptr; }
+        for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); }
         for (auto &e2 : sliceEv) if (e2) cudaEventDestroy(e2);
         sliceEv.clear();
         if (copyStream) { cudaStreamDestroy(copyStream); copyStream = nullptr; }
@@ -1060,12 +1131,14 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     const size_t E = size_t(e->E), N = size_t(e->N), px = size_t(w) * h;
     bool ok = ck(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking), "stream") && ck(cudaStreamCreateWithFlags(&e->copyStream, cudaStreamNonBlocking), "copy stream");
     for (auto &evx : e->ev) ok = ok && ck(cudaEventCreate(&evx), "event");
+    ok = ok && ck(cudaEventCreate(&e->evFinal), "event");
     ok = ok && ck(e->d_levels.alloc(E * 2), "levels") && ck(e->d_statics.alloc(E * 2 * size_t(e->staticCap)), "statics") && ck(e->d_staticRot.alloc(E * 2 * size_t(e->staticCap) * 2), "staticRot") &&
          ck(e->h_statics.alloc(E * 2 * size_t(e->staticCap)), "h_statics") && ck(e->h_staticRot.alloc(E * 2 * size_t(e->staticCap) * 2), "h_staticRot") && ck(e->d_solid.alloc(E * 2 * 3 * e->gridWords), "solid") && ck(e->d_objGrid.alloc(E * e->gridCells), "objGrid") &&
          ck(e->d_envs.alloc(E), "envs") && ck(e->d_agents.alloc(N), "agents") && ck(e->d_objects.alloc(E * MV_MAX_OBJECTS), "objects") &&
          ck(e->d_inst.alloc(E * size_t(e->instCap)), "instances") && ck(e->d_deco.alloc(E * 2 * size_t(e->decoCap)), "deco") && ck(e->h_deco.alloc(E * 2 * size_t(e->decoCap)), "h_deco") && ck(e->d_instCounts.alloc(E * 8), "instCounts") && ck(e->d_views.alloc(N * 16), "views") &&
          ck(e->d_actions.alloc(N), "actions") && ck(e->d_rtable.alloc(N * MV_R_COUNT), "rtable") && ck(e->d_rewards.alloc(N), "rewards") &&
-         ck(e->d_dones.alloc(E), "dones") && ck(e->d_trueObj.alloc(N), "trueObj") && ck(e->d_obs.alloc(N * px * 4), "obs") && ck(e->d_faults.alloc(E), "faults") &&
+         ck(e->d_dones.alloc(E), "dones") && ck(e->d_doneReasons.alloc(E), "doneReasons") && ck(cudaMemset(e->d_doneReasons.p, 0, E), "doneReasons") &&
+         ck(e->d_trueObj.alloc(N), "trueObj") && ck(e->d_obs.alloc(N * px * 4), "obs") && ck(e->d_faults.alloc(E), "faults") &&
          ck(e->d_workCounter.alloc(4), "workCounter") && ck(cudaMemset(e->d_workCounter.p, 0, 16), "workCounter") &&
          ck(e->d_sliceDone.alloc(16), "sliceDone") && ck(cudaMemset(e->d_sliceDone.p, 0, 64), "sliceDone") &&
          ck(e->d_viewCost.alloc(e->costItems() + size_t(E) + 1), "viewCost") && ck(e->resetViewOrder(), "viewOrder") && ck(e->d_ready.alloc(E), "ready") &&
@@ -1087,15 +1160,16 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     while (e->rasterBands > 1 && (h / 4) % e->rasterBands) --e->rasterBands;
     if (ok && e->configureRaster() != MV_OK) return fail(MV_ERR_CUDA);
     ok = ok && ck(e->h_levels.alloc(E * 2), "h_levels") && ck(e->h_solid.alloc(E * 2 * 3 * e->gridWords), "h_solid") && ck(e->h_actions.alloc(N), "h_actions") &&
-         ck(e->h_rtable.alloc(N * MV_R_COUNT), "h_rtable") && ck(e->h_rewards.alloc(N), "h_rewards") && ck(e->h_dones.alloc(E), "h_dones") &&
+         ck(e->h_rtable.alloc(N * MV_R_COUNT), "h_rtable") && ck(e->h_rewards.alloc(N), "h_rewards") && ck(e->h_dones.alloc(E), "h_dones") && ck(e->h_doneReasons.alloc(E), "h_doneReasons") &&
          ck(e->h_trueObj.alloc(N), "h_trueObj") && ck(e->h_obs.alloc(N * px * 4), "h_obs") && ck(e->h_faults.alloc(E), "h_faults") && ck(e->h_faultWord.alloc(1), "h_faultWord") &&
          ck(e->h_envList.alloc(E), "h_envList") && ck(e->d_envList.alloc(E), "envList");
-    for (auto &p : e->ring) ok = ok && ck(cudaEventCreateWithFlags(&p.ev, cudaEventDisableTiming), "event") && ck(p.rewards.alloc(N), "ring") && ck(p.trueObj.alloc(N), "ring") && ck(p.dones.alloc(E), "ring");
+    for (auto &p : e->ring) ok = ok && ck(cudaEventCreateWithFlags(&p.ev, cudaEventDisableTiming), "event") && ck(p.rewards.alloc(N), "ring") && ck(p.trueObj.alloc(N), "ring") && ck(p.dones.alloc(E), "ring") && ck(p.reasons.alloc(E), "ring");
     if (!ok) return fail(MV_ERR_CUDA);
     std::memset(e->h_actions.p, 0, sizeof(int32_t) * N);
     e->h_faultWord.p[0] = 0;
     std::memset(e->h_rewards.p, 0, sizeof(float) * N);
     std::memset(e->h_dones.p, 0, E);
+    std::memset(e->h_doneReasons.p, 0, E);
     std::memset(e->h_trueObj.p, 0, sizeof(float) * N);
     std::memset(e->h_obs.p, 0, N * px * 4);
     for (size_t v = 0; v < N; ++v) e->fillRtableRow(int(v));
@@ -1121,6 +1195,11 @@ int mv_set_option(mv_handle h, const char *key, int value) {
             if (h->d_depth.alloc(cnt) != cudaSuccess || h->h_depth.alloc(cnt) != cudaSuccess) { h->setError("depth allocation failed"); return MV_ERR_CUDA; }
             if (!h->depthOut) h->depthOut = h->d_depth.p;
         }
+        return MV_OK;
+    }
+    if (k == "final_obs") {  // terminal frames of ended episodes; the buffers are allocated by the first reset (after "depth" / "static_cap")
+        if (h->didReset) { h->setError("option final_obs must be set before the first reset"); return MV_ERR_STATE; }
+        h->wantFinal = value != 0;
         return MV_OK;
     }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches
@@ -1223,6 +1302,19 @@ int mv_reset(mv_handle h) {
         std::memset(init.data(), 0, sizeof(MvEnvState) * init.size());
         for (auto &s : init) { s.slot = 1; s.episode_idx = -1; mvBzInit(s); }
         if (cudaMemcpy(h->d_envs.p, init.data(), sizeof(MvEnvState) * init.size(), cudaMemcpyHostToDevice) != cudaSuccess) { h->setError("env init upload failed"); return MV_ERR_CUDA; }
+        if (h->wantFinal) {
+            const size_t E = size_t(h->E), N = size_t(h->N), px = size_t(h->W) * h->H;
+            if (h->d_termInst.alloc(E * size_t(h->instCap)) != cudaSuccess || h->d_termCounts.alloc(E * 8) != cudaSuccess || h->d_termViews.alloc(N * 16) != cudaSuccess ||
+                h->d_finalObs.alloc(N * px * 4) != cudaSuccess || h->h_finalObs.alloc(N * px * 4) != cudaSuccess ||
+                (h->wantDepth && (h->d_finalDepth.alloc(N * px) != cudaSuccess || h->h_finalDepth.alloc(N * px) != cudaSuccess)) ||
+                cudaMemset(h->d_finalObs.p, 0, N * px * 4) != cudaSuccess || (h->wantDepth && cudaMemset(h->d_finalDepth.p, 0, sizeof(float) * N * px) != cudaSuccess)) {
+                h->d_termInst.free(); h->d_termCounts.free(); h->d_termViews.free(); h->d_finalObs.free(); h->h_finalObs.free(); h->d_finalDepth.free(); h->h_finalDepth.free();
+                h->setError("final_obs: allocation failed");
+                return MV_ERR_CUDA;
+            }
+            std::memset(h->h_finalObs.p, 0, N * px * 4);
+            if (h->wantDepth) std::memset(h->h_finalDepth.p, 0, sizeof(float) * N * px);
+        }
         regenerateNext(h);
         h->didReset = true;
     }
@@ -1465,10 +1557,16 @@ int mv_fetch_obs(mv_handle h) {
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     const int rc = h->drain();
     if (rc) return rc;
-    if (!h->deviceObsFresh) return MV_OK;  // the last step stored its frames straight into the host buffer: that copy is the newer one
     const size_t px = size_t(h->N) * h->W * h->H;
-    if (cudaMemcpyAsync(h->h_obs.p, h->obsOut, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("obs download failed"); return MV_ERR_CUDA; }
-    if (h->wantDepth && cudaMemcpyAsync(h->h_depth.p, h->depthOut, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("depth download failed"); return MV_ERR_CUDA; }
+    if (h->wantFinal && h->finalOnDevice) {  // terminal frames of mv_step_device steps (host-facing steps store theirs into the host buffer)
+        if (cudaMemcpyAsync(h->h_finalObs.p, h->d_finalObs.p, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("final obs download failed"); return MV_ERR_CUDA; }
+        if (h->wantDepth && cudaMemcpyAsync(h->h_finalDepth.p, h->d_finalDepth.p, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("final depth download failed"); return MV_ERR_CUDA; }
+    }
+    // after a zero-copy host-facing step the host buffer holds the newer frames: no copy
+    if (h->deviceObsFresh) {
+        if (cudaMemcpyAsync(h->h_obs.p, h->obsOut, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("obs download failed"); return MV_ERR_CUDA; }
+        if (h->wantDepth && cudaMemcpyAsync(h->h_depth.p, h->depthOut, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("depth download failed"); return MV_ERR_CUDA; }
+    }
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
     return MV_OK;
 }
@@ -1503,6 +1601,36 @@ int mv_depth_host(mv_handle h, const float **out) { if (!h || !out || !h->wantDe
 int mv_rewards(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_rewards.p; return MV_OK; }
 int mv_dones(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_dones.p; return MV_OK; }
 int mv_true_objectives(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_trueObj.p; return MV_OK; }
+int mv_done_reasons(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_doneReasons.p; return MV_OK; }
+static int finalBuffer(mv_handle h, bool depth, const char *fn) {
+    if (!h->wantFinal || (depth && !h->wantDepth)) { h->setError(std::string(fn) + ": option final_obs" + (depth ? " and option depth are" : " is") + " off"); return MV_ERR_ARG; }
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+int mv_final_obs_host(mv_handle h, const uint8_t **out) {
+    if (!h || !out) return MV_ERR_ARG;
+    const int rc = finalBuffer(h, false, "mv_final_obs_host");
+    if (rc == MV_OK) *out = h->h_finalObs.p;
+    return rc;
+}
+int mv_final_depth_host(mv_handle h, const float **out) {
+    if (!h || !out) return MV_ERR_ARG;
+    const int rc = finalBuffer(h, true, "mv_final_depth_host");
+    if (rc == MV_OK) *out = h->h_finalDepth.p;
+    return rc;
+}
+int mv_final_obs_device(mv_handle h, uint8_t **p) {
+    if (!h || !p) return MV_ERR_ARG;
+    const int rc = finalBuffer(h, false, "mv_final_obs_device");
+    if (rc == MV_OK) *p = h->d_finalObs.p;
+    return rc;
+}
+int mv_final_depth_device(mv_handle h, float **p) {
+    if (!h || !p) return MV_ERR_ARG;
+    const int rc = finalBuffer(h, true, "mv_final_depth_device");
+    if (rc == MV_OK) *p = h->d_finalDepth.p;
+    return rc;
+}
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth) {
     if (!h) return MV_ERR_ARG;
     DeviceGuard dg__(h->device);
@@ -1528,6 +1656,8 @@ int mv_depth_device(mv_handle h, float **p) {
 }
 int mv_rewards_device(mv_handle h, float **p) { if (!h || !p) return MV_ERR_ARG; *p = h->d_rewards.p; return MV_OK; }
 int mv_dones_device(mv_handle h, uint8_t **p) { if (!h || !p) return MV_ERR_ARG; *p = h->d_dones.p; return MV_OK; }
+int mv_done_reasons_device(mv_handle h, uint8_t **p) { if (!h || !p) return MV_ERR_ARG; *p = h->d_doneReasons.p; return MV_OK; }
+int mv_true_objectives_device(mv_handle h, float **p) { if (!h || !p) return MV_ERR_ARG; *p = h->d_trueObj.p; return MV_OK; }
 int mv_stream(mv_handle h, void **s) { if (!h || !s) return MV_ERR_ARG; *s = h->stream; return MV_OK; }
 
 int mv_get_reward_shaping(mv_handle h, int env, int agent, const char **keys, float *vals, int cap, int *n) {
@@ -1591,6 +1721,7 @@ int mv_fault_word(mv_handle h, int32_t *out) {  // no device round trip: the ste
 }
 int mv_kernel_launches(mv_handle h, int64_t *out) { if (!h || !out) return MV_ERR_ARG; *out = h->launches; return MV_OK; }
 int mv_last_kernel_ms(mv_handle h, float *out2) { if (!h || !out2) return MV_ERR_ARG; out2[0] = h->lastMs[0]; out2[1] = h->lastMs[1]; return MV_OK; }
+int mv_last_final_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_ARG; *out = h->lastFinalMs; return MV_OK; }
 
 int mv_close(mv_handle h) {
     if (!h) return MV_ERR_ARG;

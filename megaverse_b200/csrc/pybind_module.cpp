@@ -142,6 +142,20 @@ public:
         check(mv_dones(h__, &d));
         return py::array_t<uint8_t>({numEnvs_}, d, py::none{});
     }
+    // (extension) why each env's episode ended at the last step: MV_END_* (0 not done, 1 time limit, 2 solved, 3 requested)
+    py::array_t<uint8_t> getDoneReasons() {
+        alive();
+        const uint8_t *d;
+        check(mv_done_reasons(h__, &d));
+        return py::array_t<uint8_t>({numEnvs_}, d, py::none{});
+    }
+    // (extension) terminal frames, option "final_obs": [N,h,w,4], the views of env e hold the frame its last episode ended on
+    py::array_t<uint8_t> getFinalObservations() {
+        alive();
+        const uint8_t *o;
+        check(mv_final_obs_host(h__, &o));
+        return py::array_t<uint8_t>({int(masks_.size()), h_, w_, 4}, o, py::none{});
+    }
     py::array_t<float> getTrueObjectives() {
         alive();
         const float *t;
@@ -263,6 +277,8 @@ PYBIND11_MODULE(megaverse, m) {
         .def("get_rewards", &MegaverseGym::getRewardsArray)
         .def("get_dones", &MegaverseGym::getDones)
         .def("get_true_objectives", &MegaverseGym::getTrueObjectives)
+        .def("get_done_reasons", &MegaverseGym::getDoneReasons, "uint8[num_envs] why each episode ended at the last step: 0 not done, 1 time limit, 2 solved, 3 requested")
+        .def("get_final_observations", &MegaverseGym::getFinalObservations, "uint8[N,h,w,4] terminal frames (option final_obs): the frame each env's last episode ended on")
         .def("obs_device_ptr", &MegaverseGym::obsDevicePtr)
         .def("faults", &MegaverseGym::faults)
         .def("fault_word", &MegaverseGym::faultWord)

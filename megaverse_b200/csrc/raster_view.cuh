@@ -123,6 +123,8 @@ struct ViewParams {
     int bands, bandRows;         // bandRows: multiple of 4; bands * bandRows >= H
     int triCap;                  // triangle list capacity of a CTA (shared memory), <= kMaxTriCap
     float p00, p11, p22, p32;
+    // masked launches only (viewKernel<FAST, true>, natural order, viewBase == 0): [E] the items of an env whose byte is 0 are skipped
+    const uint8_t *envMask;
 };
 
 struct SmemLayout { uint32_t stage, cover, shade, xf, off, frag, small, meshV, meshI, clip, slow, sched, misc, total; };
@@ -789,8 +791,15 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
 
 // ---------------------------------------------------------------------------------------------------- work queue
 // Next work item of the CTA (called by one thread): an index into [0, total), or >= total when the queue is empty.  Natural order: the
-// claim itself; cost-ordered: the view the previous launch's sort put at that position.
-__device__ __forceinline__ uint32_t claimWork(const ViewParams &P, uint32_t total) {
+// claim itself; cost-ordered: the view the previous launch's sort put at that position.  Masked: claims of unmasked envs are passed over, so
+// every item is still claimed once and every CTA still ends on exactly one failing claim (the counter advances by items + grid).
+template <bool MASKED> __device__ __forceinline__ uint32_t claimWork(const ViewParams &P, uint32_t total) {
+    if (MASKED) {
+        const uint32_t perEnv = uint32_t(P.A) * uint32_t(P.bands);
+        uint32_t m = atomicAdd(P.workCounter, 1u) - P.counterBase;
+        while (m < total && !P.envMask[m / perEnv]) m = atomicAdd(P.workCounter, 1u) - P.counterBase;
+        return m;
+    }
     const uint32_t c = atomicAdd(P.workCounter, 1u) - P.counterBase;
     if (P.viewCost && c < total) {
         const uint32_t perEnv = uint32_t(P.A) * uint32_t(P.bands);
@@ -805,7 +814,8 @@ __device__ __forceinline__ uint32_t claimWork(const ViewParams &P, uint32_t tota
 #else
 #define MV_VIEW_BOUNDS __launch_bounds__(kThreads, MV_VIEW_MIN_CTAS)
 #endif
-template <bool FAST> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
+// MASKED: a terminal-frame launch (option "final_obs") that draws only the views of the envs P.envMask names
+template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
     unsigned char *smem = g_viewSmem;
     const SmemLayout L = smemLayout(P.triCap);
     MvInstance *stage = reinterpret_cast<MvInstance *>(smem + L.stage);
@@ -849,7 +859,7 @@ template <bool FAST> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_cons
     const int tilesX = P.W >> 5;
     unsigned long long *spill = P.spill + size_t(blockIdx.x) * size_t(P.spillStride);
 
-    if (tid == 0) { M.claim = claimWork(P, total); M.prefetched = 0; }
+    if (tid == 0) { M.claim = claimWork<MASKED>(P, total); M.prefetched = 0; }
     for (;;) {
         const long long tc0 = P.stats ? clock64() : 0;
         long long tcWait = 0, tcInst = 0, tcItem = 0;
@@ -1160,7 +1170,7 @@ template <bool FAST> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_cons
         // instance chunk while this item's tiles are drawn (the stage buffers, M.view and M.counts are idle during the tile pass): the
         // global round trips of the item head then cost nothing.  One thread; its warp joins the tile pass a little later.
         if (tid == 0) {
-            const uint32_t nc = claimWork(P, total);
+            const uint32_t nc = claimWork<MASKED>(P, total);
             int pre = 0;
             if (nc < total) {
                 const int nview = P.viewBase + int(nc / uint32_t(bands)), nenv = nview / P.A;

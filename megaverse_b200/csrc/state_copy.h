@@ -9,7 +9,7 @@
 
 namespace mvs {
 
-constexpr int kMaxSlabs = 16;
+constexpr int kMaxSlabs = 17;
 
 // one per-env array: row r of it starts at base + r * pitch and holds rowBytes bytes
 struct Slab {

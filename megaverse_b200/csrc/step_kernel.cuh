@@ -71,6 +71,13 @@ struct StepParams {
     const uint8_t *ends;         // optional [num_envs] (mv_step_device_ends): ends[env] != 0 ends the episode at this step, once it has run >= 3 steps
     int maxObj;                  // upper bound of n_obj over the live and staged levels (sizes the staging copy)
     uint32_t *prof;              // optional [E][16] per-phase cycle stamps (mv_debug_step_profile); nullptr in production
+    uint8_t *doneReasons;        // [E] MV_END_* of this step, written beside dones (MV_END_NONE where dones is 0)
+    uint8_t *hostDoneReasons;    // optional pinned host mirror (or nullptr)
+    // optional terminal rows (option "final_obs"; nullptr: off): an env that ends at this step gets here the instance list, counts and
+    // views this step would have drawn had the episode not ended.  Same layouts and instStride as instances / instCounts / views.
+    MvInstance *termInstances;
+    int32_t *termCounts;
+    float *termViews;
     MvConsts k;
 };
 
@@ -1408,6 +1415,29 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
         const uint8_t dn = (!P.forceReset && doneFlag) ? 1 : 0;
         P.dones[env] = dn;
         if (P.hostDones) P.hostDones[env] = dn;
+        // solved first: doneWithTimer ran (also when a request arrives during its grace), then the clock, else the caller's request
+        const uint8_t why = !dn ? uint8_t(MV_END_NONE) : (S.env.solved ? uint8_t(MV_END_SOLVED) : (S.env.episode_sec >= L->episode_len ? uint8_t(MV_END_TIME) : uint8_t(MV_END_REQUESTED)));
+        P.doneReasons[env] = why;
+        if (P.hostDoneReasons) P.hostDoneReasons[env] = why;
+    }
+
+    if (P.termInstances && !P.forceReset && doneFlag) {
+        // terminal row: the live row as the previous step left it, with this step's dynamic entries written on top from the still-live
+        // level slot.  writeInstances only reads S, so this is exactly what a step that does not end writes, and the live path below
+        // is untouched.
+        MvInstance *tInst = P.termInstances + size_t(env) * P.instStride;
+        int32_t *tCounts = P.termCounts + size_t(env) * 8;
+        float *tViews = P.termViews + size_t(env) * A * 16;
+        const int32_t *counts = P.instCounts + size_t(env) * 8;
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(P.instances + size_t(env) * P.instStride);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(tInst);
+        const int words = counts[1] * int(sizeof(MvInstance) / 4);
+        for (int i = lane; i < words; i += 32) dst[i] = src[i];
+        if (lane < 8) tCounts[lane] = counts[lane];
+        for (int i = lane; i < A * 16; i += 32) tViews[i] = P.views[size_t(env) * A * 16 + i];
+        __syncwarp();
+        writeInstances(S, *L, statics, P.deco + (size_t(env) * 2 + slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
+        __syncwarp();
     }
 
     if (resetNow) {

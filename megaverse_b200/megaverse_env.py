@@ -69,8 +69,10 @@ class MegaverseEnv(Env):
     # (`levels_skipped()`, also reported in the infos).
     SKIP_UNFIT_LEVELS = False
 
-    def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None):
+    def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
+        # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
+        # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -101,6 +103,9 @@ class MegaverseEnv(Env):
         self.env = MegaverseGym(self.scenario_name, self.img_w, self.img_h, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan, float_params)
         if self.SKIP_UNFIT_LEVELS:
             self.env.set_option("skip_unfit_levels", 1)
+        self.final_observation = bool(final_observation)
+        if self.final_observation:
+            self.env.set_option("final_obs", 1)
         self.default_shaping_scheme = self.env.get_reward_shaping(0, 0)
         # each scenario's default scheme, read from its first env before anyone could change it
         self._default_shaping = {}
@@ -144,12 +149,22 @@ class MegaverseEnv(Env):
         self.check_faults()
 
         env_dones = self.env.get_dones()
+        if self.final_observation:
+            reasons = self.env.get_done_reasons()
+            final = self.env.get_final_observations()
         dones, infos = [], []
         for env_i in range(self.num_envs):
             done = bool(env_dones[env_i])
             dones.extend([done for _ in range(self.num_agents_per_env)])
             if done:
                 infos.extend([dict(true_reward=float(self.env.true_objective(env_i, j))) for j in range(self.num_agents_per_env)])
+                if self.final_observation:
+                    for j in range(self.num_agents_per_env):
+                        view = env_i * self.num_agents_per_env + j
+                        # a copy: the engine's buffer row is rewritten at the env's next episode end
+                        infos[view]['final_observation'] = np.ascontiguousarray(np.transpose(final[view, :, :, :3], (2, 0, 1)))
+                        infos[view]['terminated'] = int(reasons[env_i]) == 2
+                        infos[view]['truncated'] = int(reasons[env_i]) in (1, 3)
             else:
                 infos.extend([{} for _ in range(self.num_agents_per_env)])
 
