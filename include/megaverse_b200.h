@@ -119,9 +119,6 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * memory; 1 by default), "zero_copy" (0/1, default 1: host-facing steps let the rasteriser store rows straight into the pinned host buffer, the
  * PCIe writes overlapping the drawing -- the HBM tensor is then stale and mv_obs_device refuses it until the next mv_step_device; 0:
  * rasterise into HBM in "host_slices" launches (0 = by size) whose downloads run on the copy engine while the next slice is drawn),
- * "host_progressive" (0..16, default 0: host-facing steps rasterise into HBM in ONE launch and the copy engine follows it slice by slice of
- * whole envs -- the rasteriser counts finished work items per slice, the copy stream waits on the counters; measured slower than the
- * zero-copy stores wherever single views are expensive, DESIGN.md section 7),
  * "fast_shading" (0/1, default 1: +-1 LSB fragment maths),
  * "tri_cap" (32..1022, default 368: the largest that leaves two CTAs per SM; triangles one raster CTA keeps in shared memory; a view with more is drawn in several batches,
  * results do not depend on it), "raster_bands" (row bands a view is cut into, one work item of the persistent raster grid each;

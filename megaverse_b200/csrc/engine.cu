@@ -182,14 +182,6 @@ struct mv_engine {
     bool rasterToHost = false;
     bool deviceObsFresh = false;   // the HBM obs tensor holds the last step's frames (false after a zero-copy host-facing step)
     int sliceCount = 1;            // this launch: > 1 = sliced download on copyStream
-    // progressive delivery (option "host_progressive" = slices): ONE raster launch into HBM; the rasteriser counts finished work items per slice
-    // of whole envs (d_sliceDone, never reset: the host keeps the running targets), the copy stream waits on each counter in turn
-    // (cuStreamWaitValue32) and downloads that slice with the copy engine while the rest of the batch is still being drawn
-    int progSlicesOpt = 0, progSlices = 0;
-    DevBuf<uint32_t> d_sliceDone;
-    uint32_t sliceTarget[16] = {};
-    typedef int (*WaitValue32Fn)(cudaStream_t, unsigned long long, unsigned int, unsigned int);
-    WaitValue32Fn waitValue32 = nullptr;
     cudaStream_t copyStream = nullptr;
     std::vector<cudaEvent_t> sliceEv;
     int numSMs = 132;              // H100 SXM; replaced by the device's count in mv_create
@@ -232,7 +224,7 @@ struct mv_engine {
     size_t costItems() const { return size_t(N) * size_t(H / 4); }
     int rasterGridCap = 0;             // option "raster_grid": upper bound of the raster grid (0: all CTAs the GPU holds) -- for several engines sharing one GPU
     int rasterSched = 1;               // option "raster_sched": 0 natural order, 1 cost-ordered when the launch has several items per CTA, 2 always
-    int rasterGrid = 0, rasterCtasPerSM = 0, spillStride = 0, rasterBands = 1;
+    int rasterGrid = 0, rasterCtasPerSM = 0, spillStride = 0, rasterBands = 1, bandRows = 0;
     size_t rasterSmem = 0;
     // hi-res pass (draw_hires): its own output buffers, allocated on first use
     struct Hires {
@@ -501,18 +493,23 @@ struct mv_engine {
     // the masked raster launch over the terminal rows: every (view, band) item of an env whose d_dones byte is set, into the final-frame
     // buffers -- pinned host memory (stored through UVA, like the zero-copy obs rows) or HBM
     int launchFinal(bool toHost) {
-        mvr::ViewParams vp = {};
-        vp.instances = d_termInst.p; vp.instCounts = d_termCounts.p; vp.views = d_termViews.p; vp.instStride = instCap;
+        mvr::ViewParams vp = rasterParams();
+        vp.instances = d_termInst.p; vp.instCounts = d_termCounts.p; vp.views = d_termViews.p;
         vp.obs = toHost ? h_finalObs.p : d_finalObs.p; vp.depth = wantDepth ? (toHost ? h_finalDepth.p : d_finalDepth.p) : nullptr;
-        vp.spill = d_spill.p; vp.spillStride = spillStride; vp.consumed = nullptr; vp.stats = nullptr;
-        vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4; vp.triCap = triCap;
-        vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
-        vp.ready = nullptr; vp.readyStamp = 0;
         vp.viewBase = 0; vp.N = N;
         vp.envMask = d_dones.p;
         finalOnDevice = !toHost;
         const int grid = std::min(rasterGridCap > 0 ? std::min(finalGrid, rasterGridCap) : finalGrid, N * rasterBands);
         return launchView(vp, grid, false);
+    }
+    // what every raster launch at the engine's frame size shares (the step's frames and the terminal frames): instance stride, spill
+    // slab, frame and band geometry, projection; the rest is zero (no stats, no ready stamps, no mask, natural order)
+    mvr::ViewParams rasterParams() const {
+        mvr::ViewParams vp = {};
+        vp.instStride = instCap; vp.spill = d_spill.p; vp.spillStride = spillStride;
+        vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = bandRows; vp.triCap = triCap;
+        vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
+        return vp;
     }
     // One persistent launch over all (view, band) items.  Every CTA makes exactly one failing claim when the queue is empty, so the
     // work counter advances by items + grid per launch and the host keeps the base instead of resetting the counter (no memset node
@@ -543,13 +540,11 @@ struct mv_engine {
     // dependent = false: a launch that follows no step kernel (the re-render after mv_states_load)
     int launchRaster(bool dependent = true) {
         const bool dep = overlap && dependent;
-        mvr::ViewParams vp = {};
-        vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p; vp.instStride = instCap;
+        mvr::ViewParams vp = rasterParams();
+        vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         // pinned allocations are mapped into the device address space (UVA), so the kernel can store through the host pointer
         vp.obs = rasterToHost ? h_obs.p : obsOut; vp.depth = wantDepth ? (rasterToHost ? h_depth.p : depthOut) : nullptr;
-        vp.spill = d_spill.p; vp.spillStride = spillStride; vp.consumed = nullptr; vp.stats = d_rasterStats.p;
-        vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4; vp.triCap = triCap;
-        vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
+        vp.stats = d_rasterStats.p;
         // programmatic dependent launch: the grid may start before the step kernel has drained; a CTA waits for its env's stamp
         vp.ready = dep ? d_ready.p : nullptr; vp.readyStamp = dep ? readyStamp : 0;
         deviceObsFresh = !rasterToHost;
@@ -559,23 +554,7 @@ struct mv_engine {
             if (rasterSched == 2 || (rasterSched == 1 && N * rasterBands > grid)) {  // more work items than CTAs: their order matters
                 vp.viewCost = d_viewCost.p; vp.order = d_viewCost.p + costItems(); vp.exitCounter = d_viewCost.p + costItems() + size_t(E);
             }
-            if (progSlices > 0) { vp.sliceDone = d_sliceDone.p; vp.envsPerSlice = (E + progSlices - 1) / progSlices; }
-            const int rcl = launchView(vp, grid, dep);
-            if (rcl || progSlices <= 0) return rcl;
-            // downloads: slice k as soon as all of its work items are drawn (cyclic >= comparison on the device counter)
-            const size_t px = size_t(W) * H;
-            for (int k = 0, e0 = 0; e0 < E; ++k, e0 += vp.envsPerSlice) {
-                const int envs = std::min(vp.envsPerSlice, E - e0);
-                sliceTarget[k] += uint32_t(envs) * uint32_t(A) * uint32_t(rasterBands);
-                if (waitValue32(copyStream, (unsigned long long)(uintptr_t)(d_sliceDone.p + k), sliceTarget[k], 1u /* CU_STREAM_WAIT_VALUE_GEQ */) != 0) {
-                    setError("cuStreamWaitValue32 failed");
-                    return MV_ERR_CUDA;
-                }
-                const size_t v0 = size_t(e0) * A, cnt = size_t(envs) * A;
-                MV_CUDA(cudaMemcpyAsync(h_obs.p + v0 * px * 4, obsOut + v0 * px * 4, cnt * px * 4, cudaMemcpyDeviceToHost, copyStream));
-                if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p + v0 * px, depthOut + v0 * px, sizeof(float) * cnt * px, cudaMemcpyDeviceToHost, copyStream));
-            }
-            return MV_OK;
+            return launchView(vp, grid, dep);
         }
         // sliced download: whole envs per slice; slice s is copied down by the copy engine while slice s+1 is rasterised
         const size_t px = size_t(W) * H;
@@ -593,20 +572,16 @@ struct mv_engine {
         }
         return MV_OK;
     }
-    // decide how this host-facing launch delivers its frames
+    // decide how this host-facing launch delivers its frames: zero-copy stores, or into HBM and then one copy (sliceCount 1) or a
+    // download per slice of whole envs (sliceCount > 1)
     void chooseDelivery(bool copyObs) {
-        progSlices = 0;
-        if (copyObs && progSlicesOpt > 0 && waitValue32 && d_sliceDone.p) { rasterToHost = false; sliceCount = 1; progSlices = std::min({progSlicesOpt, E, 16}); return; }
-        const int d = copyObs ? hostDelivery() : 1;
-        rasterToHost = copyObs && d == 0; sliceCount = std::max(1, d);
-    }
-    // how a host-facing step delivers its obs: returns the slice count (0 = zero-copy stores, 1 = one copy after the raster)
-    int hostDelivery() const {
-        const size_t bytes = size_t(N) * W * H * (wantDepth ? 8 : 4);
-        const bool zc = zeroCopyOpt != 0;
-        if (zc) return 0;
-        if (hostSlicesOpt > 0) return std::min(hostSlicesOpt, E);
-        return int(std::max<size_t>(1, std::min<size_t>({size_t(4), size_t(E), bytes / (size_t(32) << 20)})));  // four slices: the best copy-engine form at 151 MB (H100)
+        rasterToHost = copyObs && zeroCopyOpt != 0;
+        if (!copyObs || rasterToHost) sliceCount = 1;
+        else if (hostSlicesOpt > 0) sliceCount = std::min(hostSlicesOpt, E);
+        else {  // four slices: the best copy-engine form at 151 MB (H100)
+            const size_t bytes = size_t(N) * W * H * (wantDepth ? 8 : 4);
+            sliceCount = int(std::max<size_t>(1, std::min<size_t>({size_t(4), size_t(E), bytes / (size_t(32) << 20)})));
+        }
     }
     // draw_hires (megaverse.cpp:154-177): every agent view once more, at (w, h), from the instance lists and camera matrices of
     // the last step -- the same kernel over row bands of the large frame.  Result in hires.h_obs, uint8[N][h][w][4].
@@ -635,7 +610,7 @@ struct mv_engine {
         fillConstsFor(k, w, hgt);
         mvr::ViewParams vp = {};
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p; vp.instStride = instCap;
-        vp.obs = hires.d_obs.p; vp.depth = nullptr; vp.spill = hires.spill.p; vp.spillStride = stride; vp.consumed = nullptr;
+        vp.obs = hires.d_obs.p; vp.depth = nullptr; vp.spill = hires.spill.p; vp.spillStride = stride;
         vp.viewBase = 0; vp.N = N; vp.A = A; vp.W = w; vp.H = hgt; vp.bands = bands; vp.bandRows = rowsPerBand; vp.triCap = triCap;
         vp.p00 = k.p00; vp.p11 = k.p11; vp.p22 = k.p22; vp.p32 = k.p32;
         vp.ready = nullptr; vp.readyStamp = 0;
@@ -670,7 +645,7 @@ struct mv_engine {
             finalPerSM = fast ? std::min(finalPerSM, perSM) : perSM;
         }
         finalGrid = numSMs * std::max(1, std::min(finalPerSM, rasterCtasPerSM));  // shares d_spill, sized by rasterGrid
-        const int bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
+        bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
         spillStride = W * bandRows;
         d_spill.free();
         if (d_spill.alloc(size_t(rasterGrid) * size_t(spillStride)) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
@@ -704,13 +679,13 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
-        if (copyObs && !rasterToHost && sliceCount <= 1 && progSlices <= 0) {
+        if (copyObs && !rasterToHost && sliceCount <= 1) {
             MV_CUDA(cudaMemcpyAsync(h_obs.p, obsOut, size_t(N) * W * H * 4, cudaMemcpyDeviceToHost, stream));
             if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p, depthOut, sizeof(float) * size_t(N) * W * H, cudaMemcpyDeviceToHost, stream));
         }
         if (!wait) return MV_OK;
         MV_CUDA(cudaStreamSynchronize(stream));
-        if (sliceCount > 1 || progSlices > 0) MV_CUDA(cudaStreamSynchronize(copyStream));
+        if (sliceCount > 1) MV_CUDA(cudaStreamSynchronize(copyStream));
         readKernelTimes();
         return MV_OK;
     }
@@ -763,7 +738,7 @@ struct mv_engine {
             MV_CUDA(cudaMemcpyAsync(d_rtable.p, h_rtable.p, sizeof(float) * N * MV_R_COUNT, cudaMemcpyHostToDevice, stream));
             rtableDirty = false;
         }
-        rasterToHost = false; sliceCount = 1; progSlices = 0;
+        rasterToHost = false; sliceCount = 1;
         rc = launchStep(dActions, false, &slotP, dEnds);  // rewards / dones / true objectives land in the ring slot straight from the kernel
         if (rc) return rc;
         MV_CUDA(cudaEventRecord(slotP.ev, stream));
@@ -797,7 +772,7 @@ struct mv_engine {
     int stepEnd() {
         if (!hostStepPending) { setError("mv_step_end without mv_step_begin"); return MV_ERR_STATE; }
         MV_CUDA(cudaStreamSynchronize(stream));
-        if (sliceCount > 1 || progSlices > 0) MV_CUDA(cudaStreamSynchronize(copyStream));
+        if (sliceCount > 1) MV_CUDA(cudaStreamSynchronize(copyStream));
         readKernelTimes();
         hostStepPending = false;
         std::memset(h_actions.p, 0, sizeof(int32_t) * N);  // env.cpp:140-142: actions are cleared after every step
@@ -992,7 +967,7 @@ struct mv_engine {
         h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
         d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_faults.free();
-        hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free(); d_sliceDone.free();
+        hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free();
         h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free();
         h_faults.free(); h_faultWord.free();
         d_doneReasons.free(); h_doneReasons.free();
@@ -1140,18 +1115,9 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
          ck(e->d_dones.alloc(E), "dones") && ck(e->d_doneReasons.alloc(E), "doneReasons") && ck(cudaMemset(e->d_doneReasons.p, 0, E), "doneReasons") &&
          ck(e->d_trueObj.alloc(N), "trueObj") && ck(e->d_obs.alloc(N * px * 4), "obs") && ck(e->d_faults.alloc(E), "faults") &&
          ck(e->d_workCounter.alloc(4), "workCounter") && ck(cudaMemset(e->d_workCounter.p, 0, 16), "workCounter") &&
-         ck(e->d_sliceDone.alloc(16), "sliceDone") && ck(cudaMemset(e->d_sliceDone.p, 0, 64), "sliceDone") &&
          ck(e->d_viewCost.alloc(e->costItems() + size_t(E) + 1), "viewCost") && ck(e->resetViewOrder(), "viewOrder") && ck(e->d_ready.alloc(E), "ready") &&
          ck(cudaMemset(e->d_ready.p, 0, sizeof(uint32_t) * size_t(E)), "ready");
     { cudaDeviceProp prop; if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) e->numSMs = prop.multiProcessorCount; }
-    {   // stream memory operation of the driver API (no link dependency on libcuda): the copy stream of the progressive delivery waits on it
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuStreamWaitValue32", &fn, cudaEnableDefault, &qr) == cudaSuccess && qr == cudaDriverEntryPointSuccess && fn)
-            e->waitValue32 = reinterpret_cast<mv_engine::WaitValue32Fn>(fn);
-        else
-            (void)cudaGetLastError();
-    }
     if (e->instCap > mvr::kMaxInstancesPerEnv) { e->setError("instance capacity exceeds the draw-order key range"); return fail(MV_ERR_CAPACITY); }
     // few views: split every view into row bands so that the persistent grid (2 CTAs per SM) has something to balance; every band repeats
     // the view's geometry.  Measured on an H100 (ms per step, 1 / 2 / 3 bands): TowerBuilding 64 views 0.106 / 0.091 / 0.085, 256 views
@@ -1239,12 +1205,6 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         if (value < 0) return MV_ERR_ARG;
         cudaStreamSynchronize(h->stream);
         h->rasterGridCap = value;
-        return MV_OK;
-    }
-    if (k == "host_progressive") {  // slices of the progressive host delivery (0 = off): one raster launch, the copy engine follows it slice by slice
-        if (value < 0 || value > 16) return MV_ERR_ARG;
-        if (value > 0 && !h->waitValue32) { h->setError("host_progressive: cuStreamWaitValue32 is not available"); return MV_ERR_STATE; }
-        h->progSlicesOpt = value;
         return MV_OK;
     }
     if (k == "obs_to_host") { h->obsToHost = value != 0; return MV_OK; }
@@ -1952,7 +1912,7 @@ int mv_debug_render_instances(const float *view16, const float *inst18, int n, i
         cudaMemset(dCtr, 0, 16);
         mvr::ViewParams vp = {};
         vp.instances = dInst; vp.instCounts = dCnt; vp.views = dView; vp.instStride = int(inst.size()); vp.obs = dObs; vp.depth = depth ? dDepth : nullptr;
-        vp.workCounter = dCtr; vp.counterBase = 0; vp.ready = nullptr; vp.readyStamp = 0; vp.consumed = nullptr; vp.spill = dSpill; vp.spillStride = w * bandRows;
+        vp.workCounter = dCtr; vp.counterBase = 0; vp.ready = nullptr; vp.readyStamp = 0; vp.spill = dSpill; vp.spillStride = w * bandRows;
         vp.viewBase = 0; vp.N = 1; vp.A = 1; vp.W = w; vp.H = h; vp.bands = bands; vp.bandRows = bandRows; vp.triCap = triCap;
         vp.p00 = k.p00; vp.p11 = k.p11; vp.p22 = k.p22; vp.p32 = k.p32;
         mvr::viewKernel<false><<<bands, mvr::kThreads, smem>>>(vp);

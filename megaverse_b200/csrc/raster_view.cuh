@@ -100,11 +100,8 @@ struct ViewParams {
     uint32_t counterBase;
     const uint32_t *ready;       // [E] step-kernel completion stamps (nullptr: plain stream order)
     uint32_t readyStamp;         // value ready[env] holds once this step's state, instances and views of env are written
-    uint32_t *consumed;          // optional [E]: += 1 when a work item of env has read the env's instance list and view (step/raster overlap)
     unsigned long long *stats;   // optional [16]: work items, instances, visible instances, items, clipped items, triangles, batches, -, then
                                  // thread-0 cycles: head (claim, stamp, view), TMA waits, instance passes, item passes, final tile pass, whole item
-    unsigned long long *spill;   // [gridDim.x][spillStride] per-CTA fragment slab for views drawn in several batches
-    int spillStride;             // >= W * bandRows
     // cost-ordered work queue (optional; viewBase == 0, N = E * A): claim c draws item c % (A * bands) of env order[c / (A * bands)].  Every
     // CTA writes the SM cycles a work item took into viewCost; the last CTA to leave sorts the ENVS by the cost of their items, descending
     // (counting sort over 256 cost classes), into `order` for the next launch -- so the persistent CTAs do not run dry at very different
@@ -113,11 +110,10 @@ struct ViewParams {
     uint32_t *viewCost;          // [N * bands] (indexed like the work items: view * bands + band) or nullptr
     uint32_t *order;             // [E] a permutation of the envs
     uint32_t *exitCounter;       // CTAs that have left (the last one sorts)
-    // progressive host delivery (optional): sliceDone[env / envsPerSlice] += 1 when a work item is completely drawn (frames visible device-wide),
-    // so that a copy stream blocked on the counter can start downloading a slice of whole envs while the rest of the batch is still being
-    // drawn; the cost order is then slice-major (slices complete one after the other)
-    uint32_t *sliceDone;
-    int envsPerSlice;
+    unsigned long long *spill;   // [gridDim.x][spillStride] per-CTA fragment slab for views drawn in several batches
+    // field order: with the int fields from spillStride on starting 4 bytes past an 8-byte boundary, ptxas gives viewKernel 96-104 B of
+    // stack instead of 112 B (sm_90a, CUDA 12.9)
+    int spillStride;             // >= W * bandRows
     int viewBase, N;             // this launch draws views [viewBase, viewBase + N)
     int A, W, H;
     int bands, bandRows;         // bandRows: multiple of 4; bands * bandRows >= H
@@ -1161,10 +1157,6 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
             __syncthreads();  // the transform table and the stage buffer are rewritten by the next chunk
             if (P.stats) tcItem += clock64() - tw2;
         }
-        if (P.consumed && tid == 0) {  // this item no longer needs the env's instance list or view matrix
-            __threadfence();
-            atomicAdd(P.consumed + env, 1u);
-        }
         const long long tc2 = P.stats ? clock64() : 0;
         // Claim the next work item now and, if its env's state is already published, fetch its view matrix, its counts and its first
         // instance chunk while this item's tiles are drawn (the stage buffers, M.view and M.counts are idle during the tile pass): the
@@ -1204,7 +1196,6 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
         }
         tilePass<FAST>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, true);
         __syncthreads();
-        if (P.sliceDone && tid == 0) { __threadfence(); atomicAdd(P.sliceDone + env / P.envsPerSlice, 1u); }
         if (P.viewCost && tid == 0) P.viewCost[claim] = uint32_t(min((unsigned long long)clock64() - M.itemStart, 0xffffffffull * 16ull) >> 4);
         if (P.stats && tid < 8) {
             unsigned long long v = M.stat[tid];
@@ -1263,24 +1254,18 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
 #pragma unroll
             for (int d = 16; d; d >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, d));
             if (lane == 0) M.wsum[warp] = int32_t(mx);
-            // sort key: (slice of the progressive host delivery, if any) major, cost class descending minor
-            int nSlices = P.sliceDone ? (E + P.envsPerSlice - 1) / P.envsPerSlice : 1;
-            if (!inSmem || E + nSlices * 256 > capS) nSlices = 1;  // no room for the classes of every slice: plain cost order
-            const int envsPerSlice = nSlices > 1 ? P.envsPerSlice : E;
-            const int nBins = nSlices * 256;
-            uint32_t *kbins = nSlices > 1 ? costS + E : bins;
-            for (int b = tid; b < nBins; b += kThreads) kbins[b] = 0u;
+            for (int b = tid; b < 256; b += kThreads) bins[b] = 0u;
             __syncthreads();
 #pragma unroll
             for (int w = 0; w < kWarps; ++w) mx = max(mx, uint32_t(M.wsum[w]));
             const float scale = 255.0f / float(mx);
-            auto keyOf = [&](int e) { return (e / envsPerSlice) * 256 + 255 - min(255, int(float(envCost(e)) * scale)); };
-            for (int e = tid; e < E; e += kThreads) atomicAdd(&kbins[keyOf(e)], 1u);
+            auto keyOf = [&](int e) { return 255 - min(255, int(float(envCost(e)) * scale)); };  // cost class, most expensive first
+            for (int e = tid; e < E; e += kThreads) atomicAdd(&bins[keyOf(e)], 1u);
             __syncthreads();
             {   // exclusive scan of the class counts: a run of consecutive classes per thread, then a scan over the threads
-                const int per = (nBins + kThreads - 1) / kThreads, b0 = min(nBins, tid * per), b1 = min(nBins, b0 + per);
+                const int per = (256 + kThreads - 1) / kThreads, b0 = min(256, tid * per), b1 = min(256, b0 + per);
                 uint32_t sum = 0u;
-                for (int b = b0; b < b1; ++b) sum += kbins[b];
+                for (int b = b0; b < b1; ++b) sum += bins[b];
                 uint32_t incl = sum;
 #pragma unroll
                 for (int d = 1; d < 32; d <<= 1) { const uint32_t up = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += up; }
@@ -1290,11 +1275,11 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
                 uint32_t run = incl - sum;
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) if (w < warp) run += uint32_t(M.wsum[w]);
-                for (int b = b0; b < b1; ++b) { const uint32_t c = kbins[b]; kbins[b] = run; run += c; }
+                for (int b = b0; b < b1; ++b) { const uint32_t c = bins[b]; bins[b] = run; run += c; }
             }
             __syncthreads();
             for (int e = tid; e < E; e += kThreads) {
-                const uint32_t at = atomicAdd(&kbins[keyOf(e)], 1u);
+                const uint32_t at = atomicAdd(&bins[keyOf(e)], 1u);
                 P.order[at] = uint32_t(e);
             }
             if (tid == 0) *P.exitCounter = 0u;

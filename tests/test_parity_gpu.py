@@ -732,21 +732,25 @@ def test_cost_ordered_work_queue_keeps_frames_identical(built):
 
 @pytest.mark.timeout(180)
 @pytest.mark.parametrize("scenario,E,A,depth,slices", [("Collect", 300, 2, False, 8), ("ObstaclesHard", 100, 1, True, 16), ("TowerBuilding", 7, 3, False, 4)])
-def test_progressive_host_delivery_matches_zero_copy(built, scenario, E, A, depth, slices):
-    """host delivery by the copy engine following ONE raster launch slice by slice (option host_progressive: the rasteriser counts finished
-    work items per slice of envs, the copy stream waits on the counters) against the default zero-copy stores: frames, depth, rewards and
-    dones identical every step, also when the number of envs is not a multiple of the slice count and when bands and the cost order are on"""
+def test_sliced_host_delivery_matches_zero_copy(built, scenario, E, A, depth, slices):
+    """host delivery into HBM in one raster launch per slice of envs, each slice downloaded by the copy engine while the next is drawn
+    (zero_copy 0, host_slices), against the default zero-copy stores: frames, depth, rewards and dones identical every step, also when
+    the number of envs is not a multiple of the slice count and when bands and the cost order are on"""
     from megaverse_b200 import capi
 
     gs = []
-    for prog in (0, slices):
+    for sliced in (False, True):
         g = capi.Engine(scenario, E, A, 128, 72, num_threads=4, depth=depth)
-        g.set_option("host_progressive", prog)
-        g.set_option("raster_sched", 2 if prog else 1)
+        if sliced:
+            g.set_option("zero_copy", 0)
+            g.set_option("host_slices", slices)
+        g.set_option("raster_sched", 2 if sliced else 1)
         for e in range(E):
             g.seed_env(e, 900 + e)
         g.reset()
         gs.append(g)
+    with pytest.raises(capi.MegaverseError):
+        gs[1].set_option("host_progressive", 4)  # not an option: host delivery is zero-copy, one copy or sliced
     assert np.array_equal(np.array(gs[0].obs()), np.array(gs[1].obs())), "first frame"
     rng = np.random.default_rng(8)
     for t in range(30):

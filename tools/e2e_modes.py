@@ -21,8 +21,7 @@ acts = (1 << rng.integers(0, 11, size=(K + 10, E * A))).astype(np.int32)
 mb = E * A * 128 * 72 * (8 if depth else 4) / 1e6
 for name, opts in [("zero-copy stores", {"zero_copy": 1}), ("one copy after the raster", {"zero_copy": 0, "host_slices": 1}), ("2 slices", {"zero_copy": 0, "host_slices": 2}),
                    ("4 slices", {"zero_copy": 0, "host_slices": 4}), ("8 slices", {"zero_copy": 0, "host_slices": 8}), ("16 slices", {"zero_copy": 0, "host_slices": 16}),
-                   ("progressive, 4 slices", {"host_progressive": 4}), ("progressive, 8 slices", {"host_progressive": 8}), ("progressive, 16 slices", {"host_progressive": 16}),
-                   ("by size (default)", {"zero_copy": -1, "host_slices": 0, "host_progressive": 0}), ("no delivery (obs_to_host 0)", {"obs_to_host": 0})]:
+                   ("by size (default)", {"zero_copy": -1, "host_slices": 0}), ("no delivery (obs_to_host 0)", {"obs_to_host": 0})]:
     for k, v in opts.items():
         g.set_option(k, v)
     for t in range(5):
