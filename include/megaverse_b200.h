@@ -135,6 +135,15 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * otherwise leave the reference's level sequence; with 1 the env takes the next level of its stream instead and mv_levels_skipped
  * counts it),
  * "final_obs" (0/1, before the first reset, default 0: terminal frames of ended episodes, see mv_final_obs_host),
+ * "action_repeat" (1..4, before the first reset (MV_ERR_STATE after it, MV_ERR_ARG outside the range), default 1: action repeat, or
+ * frame skip, inside the engine.  Every step call (mv_step, mv_step_begin/end, mv_step_device[_ends]) runs up to k physics ticks of
+ * 1/15 s per env with the same action masks, then draws once.  Interact acts on the first tick only (it toggles carrying, so one call
+ * is one press); movement, look and jump repeat.  An episode end at tick j < k stops that env's ticks: it flips to its next level as
+ * at any end, and the frame drawn is the new episode's first.  The reward of an agent is the float sum, in tick order from 0, of what
+ * each tick paid; the tick that ends the episode pays 0, as a step that ends does.  Done, reason, true objective and terminal frame
+ * are those of the ending tick.  Requested ends: see mv_step_device_ends.  k = 1 is the reference's step.  mv_reset, mv_reset_envs,
+ * mv_states_load, mv_draw_hires and mv_debug_warp_agent run no ticks and are unchanged; state-store rows do not carry k.  The
+ * cap: with k ticks per call the asynchronous path needs episodes of 3k ticks, 0.8 s at k = 4 (DESIGN.md section 2),
  * "overlap" (0/1, default 1: the raster kernel is a programmatic dependent launch of the step kernel and synchronises per env;
  * 0 serialises the kernels so that mv_last_kernel_ms can time them separately) */
 int mv_set_option(mv_handle h, const char *key, int value);
@@ -148,7 +157,10 @@ int mv_step_device(mv_handle h, const int32_t *d_masks);
  * step's actions and scenario rules ran, exactly as a timer end: done = 1, reward 0, the true objective reported, flip to the pre-staged
  * next level, and the frame of this step is the new episode's first.  A request for an env whose current episode has run fewer than 3
  * steps (its step counter is below 3 after this step) is ignored: this call retires step k-2 at call k, so the next level of an env that
- * ended one or two steps ago is not staged yet.  The rule depends on the step count only, never on host timing. */
+ * ended one or two steps ago is not staged yet.  The rule depends on the step count only, never on host timing.
+ * With option "action_repeat" k the request applies after the call's last tick, and the rule reads "fewer than 3k ticks" (the tick
+ * counter counts ticks, so it is still three calls).  A request for an env whose episode already ended at an earlier tick of the same
+ * call is ignored: that end stands, with its own reason.  A call's reward is the sum of its ticks before the end. */
 int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends);
 /* Restart chosen envs now: envs[i] start a new episode.  seeds == NULL: each continues its own level stream (it takes its pre-staged
  * next level, as at a natural episode end); else env envs[i] is first reseeded with seeds[i] and plays the first level of that stream --
@@ -255,7 +267,9 @@ int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, 
 /* libstdc++ unordered_set iteration-order emulation (bzset.h): ops[i] = {op(0 insert,1 erase,2 clear), x, y, z};
  * writes the final iteration order as xyz triples, returns the element count */
 /* per-env cycle stamps of the step kernel's phases: out = uint32[E][16] (0 staged, 1 actions, 2 candidate list, 3 controllers,
- * 4 transforms, 5 scenario, 6 outputs/reset, 7 instance list, 8 commit, 12 candidate count); enable=1 arms it, 0 frees it */
+ * 4 transforms, 5 scenario, 6 outputs/reset, 7 instance list, 8 commit, 12 candidate count); enable=1 arms it, 0 frees it.  Stamps count
+ * from the start of the call and cover the whole call: with option "action_repeat" 1..4 and 12 are those of the last tick it ran, 5 ends
+ * the tick loop */
 int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable);
 /* rasteriser launch shape: out4 = {persistent grid size, CTAs per SM, dynamic shared memory per CTA in bytes, row bands per view} */
 int mv_debug_raster_config(mv_handle h, int32_t *out4);

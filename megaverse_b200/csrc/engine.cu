@@ -284,7 +284,8 @@ struct mv_engine {
     // views); a masked raster launch over d_dones draws their views into the final-frame buffers: the pinned host ones for host-facing
     // steps, HBM for mv_step_device.  Rows of envs that did not end are never written.
     bool wantFinal = false;
-    bool finalOnDevice = false;     // the last terminal-frame launch stored into HBM (mv_fetch_obs copies the buffers down)
+    int actionRepeat = 1;           // option "action_repeat": physics ticks per step call (the step kernel's tick loop), drawn once
+    bool finalOnDevice = false;    // the last terminal-frame launch stored into HBM (mv_fetch_obs copies the buffers down)
     bool lastHadFinal = false;      // the last timed step ran a terminal-frame launch (ev[3] .. ev[2])
     float lastFinalMs = 0.0f;
     int finalGrid = 0;              // persistent grid of the masked raster variants
@@ -455,6 +456,7 @@ struct mv_engine {
         sp.ready = d_ready.p; sp.readyStamp = ++readyStamp;
         sp.envOrder = rasterSched ? d_viewCost.p + costItems() : nullptr;  // a permutation at all times (identity until a cost-ordered raster launch has sorted it)
         sp.ends = dEnds;
+        sp.repeat = actionRepeat;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
@@ -700,7 +702,9 @@ struct mv_engine {
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
         p.valid = false;
         // the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes again sooner
-        // flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on
+        // flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on.  Counted in calls
+        // whatever option "action_repeat" is: retiring, regenerating and uploading happen once per call, so the level pipeline is three
+        // calls deep (the kernel's request rule, num_frames >= 3 * repeat ticks, is the same three calls counted on the device)
         if (lastAsyncDone.empty()) lastAsyncDone.assign(size_t(E), -1000);
         for (int e = 0; e < E; ++e)
             if (h_dones.p[e]) {
@@ -719,7 +723,8 @@ struct mv_engine {
         return MV_OK;
     }
     // asynchronous device-resident step: returns after enqueueing.  Episode bookkeeping lags two steps, which is safe
-    // because an env cannot finish twice within four steps (doneWithTimer leaves 0.3 s = 4.5 steps, scenario.hpp:114-117)
+    // because an env cannot finish twice within four steps (doneWithTimer leaves 0.3 s = 4.5 steps, scenario.hpp:114-117); with option
+    // "action_repeat" k a call runs k ticks, and DESIGN.md section 2 gives the shortest natural episodes that bound k
     int stepAsync(const int32_t *dActions, const uint8_t *dEnds) {
         if (!didReset) { setError("mv_step_device before mv_reset"); return MV_ERR_STATE; }
         if (hostStepPending) { const int rcp = stepEnd(); if (rcp) return rcp; }
@@ -1166,6 +1171,12 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     if (k == "final_obs") {  // terminal frames of ended episodes; the buffers are allocated by the first reset (after "depth" / "static_cap")
         if (h->didReset) { h->setError("option final_obs must be set before the first reset"); return MV_ERR_STATE; }
         h->wantFinal = value != 0;
+        return MV_OK;
+    }
+    if (k == "action_repeat") {  // physics ticks per step call (see the header); the state store keeps no copy: it belongs to the engine
+        if (h->didReset) { h->setError("option action_repeat must be set before the first reset"); return MV_ERR_STATE; }
+        if (value < 1 || value > 4) { h->setError("action_repeat out of range [1,4]"); return MV_ERR_ARG; }
+        h->actionRepeat = value;
         return MV_OK;
     }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches

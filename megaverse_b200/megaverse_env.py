@@ -69,10 +69,13 @@ class MegaverseEnv(Env):
     # (`levels_skipped()`, also reported in the infos).
     SKIP_UNFIT_LEVELS = False
 
-    def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False):
+    def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
+                 action_repeat=1):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
+        # (extension) action_repeat=k (1..4): every step() runs k physics ticks with the same actions (Interact on the first only) and draws
+        # once; an episode end stops the ticks, and the rewards returned are each agent's sum over the ticks run (option "action_repeat")
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -106,6 +109,8 @@ class MegaverseEnv(Env):
         self.final_observation = bool(final_observation)
         if self.final_observation:
             self.env.set_option("final_obs", 1)
+        self.action_repeat = int(action_repeat)
+        self.env.set_option("action_repeat", self.action_repeat)
         self.default_shaping_scheme = self.env.get_reward_shaping(0, 0)
         # each scenario's default scheme, read from its first env before anyone could change it
         self._default_shaping = {}
