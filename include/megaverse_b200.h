@@ -143,14 +143,26 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * each tick paid; the tick that ends the episode pays 0, as a step that ends does.  Done, reason, true objective and terminal frame
  * are those of the ending tick.  Requested ends: see mv_step_device_ends.  k = 1 is the reference's step.  mv_reset, mv_reset_envs,
  * mv_states_load, mv_draw_hires and mv_debug_warp_agent run no ticks and are unchanged; state-store rows do not carry k.  The
- * cap: with k ticks per call the asynchronous path needs episodes of 3k ticks, 0.8 s at k = 4 (DESIGN.md section 2),
+ * cap: with k ticks per call and two level slots the asynchronous path needs episodes of 3k ticks, 0.8 s at k = 4 (DESIGN.md section 2);
+ * option "level_slots" 4 lifts it),
+ * "level_slots" (2 or 4, before the first reset (MV_ERR_STATE after it, MV_ERR_ARG for any other value), default 2: level slots per
+ * env, one live and the rest holding the env's next levels in episode order.  With 2, mv_step_device[_ends] needs episodes of at least
+ * three calls (see there).  With 4 it takes every episode length at every action_repeat k and honours every end request: an env ends
+ * at most once per call, and the level replacing an end is on the device three calls later, when three ends have used the three staged
+ * levels at most.  Outputs do not depend on it.  Cost of the two extra slots, in HBM and again in pinned host memory, per env: two
+ * levels of 33 248 B, their static boxes (32 B each, static_cap of them) and rotations (8 B each), decorations (80 B each) and three
+ * bit planes of the dense grid -- 374 KiB per Collect env (392 MB at 1 024 envs), 139 KiB per TowerBuilding env, 509 KiB per env of a
+ * batch with an Obstacles env, plus 240 KiB per env for the hex mazes' decorations; state-store rows grow by the same.  The first
+ * mv_reset generates three levels per env instead of one),
  * "overlap" (0/1, default 1: the raster kernel is a programmatic dependent launch of the step kernel and synchronises per env;
  * 0 serialises the kernels so that mv_last_kernel_ms can time them separately) */
 int mv_set_option(mv_handle h, const char *key, int value);
 
 /* Device-resident path (SURVEY.md 8f rank 1): the caller's consumer reads the tensors in HBM.
  * mv_step_device: like mv_step but takes the action masks from DEVICE memory (NULL = the engine's own buffer, see
- * mv_actions_device) and leaves the observation tensor on the device; rewards/dones still land on the host. */
+ * mv_actions_device) and leaves the observation tensor on the device; rewards/dones still land on the host.  Contract: with two level
+ * slots (the default) an env may end at most once in any three consecutive calls, else the call returns MV_ERR_STATE (see mv_sync); with
+ * option "level_slots" 4 episodes of any length are accepted. */
 int mv_step_device(mv_handle h, const int32_t *d_masks);
 /* mv_step_device with per-env episode ends requested from the device: d_ends = uint8[num_envs] in DEVICE memory (NULL = none, which is
  * mv_step_device), read in the engine stream's order (mv_stream).  An env with d_ends[e] != 0 ends its episode at this step, after this
@@ -160,7 +172,8 @@ int mv_step_device(mv_handle h, const int32_t *d_masks);
  * ended one or two steps ago is not staged yet.  The rule depends on the step count only, never on host timing.
  * With option "action_repeat" k the request applies after the call's last tick, and the rule reads "fewer than 3k ticks" (the tick
  * counter counts ticks, so it is still three calls).  A request for an env whose episode already ended at an earlier tick of the same
- * call is ignored: that end stands, with its own reason.  A call's reward is the sum of its ticks before the end. */
+ * call is ignored: that end stands, with its own reason.  A call's reward is the sum of its ticks before the end.
+ * With option "level_slots" 4 every request is honoured, including one in a new episode's first call: the next level is always staged. */
 int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends);
 /* Restart chosen envs now: envs[i] start a new episode.  seeds == NULL: each continues its own level stream (it takes its pre-staged
  * next level, as at a natural episode end); else env envs[i] is first reseeded with seeds[i] and plays the first level of that stream --
@@ -182,8 +195,9 @@ int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n)
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth);
 /* mv_step_device is ASYNCHRONOUS: it returns after enqueueing the step on the engine stream (device tensors are valid in
  * stream order).  mv_sync waits for everything enqueued and publishes the last step's rewards/dones/true objectives to the
- * host pointers.  Episode bookkeeping lags the device by two steps on this path, so it needs episodes of >= 4 steps
- * (always true with the scenarios' own parameters); a violation raises MV_FAULT_LEVEL_NOT_READY in mv_faults. */
+ * host pointers.  Episode bookkeeping lags the device by two steps on this path, so with two level slots it needs episodes of at least
+ * three steps (true with the scenarios' own parameters at action_repeat 1); a violation raises MV_FAULT_LEVEL_NOT_READY in mv_faults and
+ * the next call returns MV_ERR_STATE.  Option "level_slots" 4 removes the limit. */
 /* MegaverseGym::drawHires + getHiresObservation (megaverse.cpp:154-177,199-203): renders every agent view once more at w x h
  * (multiples of 32 x 4, e.g. the reference's 768 x 432) from the state of the last step; *out = uint8[N][h][w][4], engine-owned,
  * valid until the next mv_draw_hires / mv_close */

@@ -19,6 +19,7 @@
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
+#include <deque>
 #include <functional>
 #include <map>
 #include <memory>
@@ -120,7 +121,7 @@ template <typename T> struct PinBuf {
     void free() { if (p) cudaFreeHost(p); p = nullptr; }
 };
 
-// one per-env device array as the state store sees it: `units` rows per env (2 for the arrays that hold both level slots) of unitBytes
+// one per-env device array as the state store sees it: `units` rows per env (the slot count for the arrays that hold the level slots) of unitBytes
 struct EnvSlab {
     uint8_t *base;
     int units;
@@ -137,13 +138,14 @@ struct StateStore {
     struct HostRow {
         std::optional<mv::LevelGenerator> gen;  // empty: the row was never saved
         std::string scenario;                   // the saved env's scenario name: only an env of the same name may load the row
-        int slot = 0, episode = 0, words[2] = {0, 0};
-        // the host mirrors of both level slots that the debug dumps and the uploads read
-        MvLevel level[2];
-        std::vector<MvBox> statics[2];
-        std::vector<float> staticRot[2];
-        std::vector<MvDeco> deco[2];
-        std::vector<uint32_t> solid[2];  // the three bit planes, levelWords words each
+        int slot = 0, episode = 0;
+        // the host mirrors of every level slot that the debug dumps and the uploads read, one entry per slot (option "level_slots")
+        std::vector<int> words;
+        std::vector<MvLevel> level;
+        std::vector<std::vector<MvBox>> statics;
+        std::vector<std::vector<float>> staticRot;
+        std::vector<std::vector<MvDeco>> deco;
+        std::vector<std::vector<uint32_t>> solid;  // the three bit planes, levelWords words each
     };
     std::vector<HostRow> host;
     void free() { for (auto &s : slabs) s.free(); }
@@ -192,9 +194,12 @@ struct mv_engine {
     float lastMs[2] = {0, 0};
     int64_t launches = 0;
 
-    DevBuf<MvLevel> d_levels;
-    DevBuf<MvBox> d_statics;       // [E][2][staticCap]
-    DevBuf<float> d_staticRot;     // [E][2][staticCap][2]
+    // Level slots (option "level_slots" D, 2 or 4): each env has one live slot and D - 1 staged ones that hold its next episodes' levels in
+    // order; the step kernel moves to the next slot of the ring at an episode end.  Every [E][D] array below is laid out by it.
+    int levelSlots = 2;
+    DevBuf<MvLevel> d_levels;      // [E][D]
+    DevBuf<MvBox> d_statics;       // [E][D][staticCap]
+    DevBuf<float> d_staticRot;     // [E][D][staticCap][2]
     int staticCap = MV_INITIAL_STATIC_CAP;  // grows when a generated level has more static boxes (growStatics)
     DevBuf<uint32_t> d_solid;
     DevBuf<uint8_t> d_objGrid;
@@ -233,17 +238,17 @@ struct mv_engine {
         DevBuf<unsigned long long> spill;
         void free() { d_obs.free(); h_obs.free(); spill.free(); W = H = 0; }
     } hires;
-    DevBuf<MvDeco> d_deco;
+    DevBuf<MvDeco> d_deco;         // [E][D][decoCap]
     PinBuf<MvDeco> h_deco;
     int decoCap = 1, instCap = MV_DYN_INSTANCES + MV_INITIAL_STATIC_CAP + 1;
 
-    PinBuf<MvLevel> h_levels;      // [E][2] staging mirror
-    PinBuf<MvBox> h_statics;       // [E][2][staticCap]
+    PinBuf<MvLevel> h_levels;      // [E][D] staging mirror
+    PinBuf<MvBox> h_statics;       // [E][D][staticCap]
     PinBuf<float> h_staticRot;
     // levels with more static boxes than the arrays hold: parked here by the workers until flushUploads has grown the arrays
     std::vector<std::pair<int, mv::LevelOut>> oversize;
     int wantStaticCap = 0;
-    PinBuf<uint32_t> h_solid;      // [E][2][gridWords]
+    PinBuf<uint32_t> h_solid;      // [E][D][3][gridWords]
     PinBuf<int32_t> h_actions;
     PinBuf<float> h_rtable;
     PinBuf<float> h_rewards;
@@ -267,8 +272,12 @@ struct mv_engine {
     uint64_t asyncSteps = 0;
 
     std::vector<int> hostSlot, hostEpisode;   // mirrors of the device's live slot / episode index
-    std::vector<int> levelWords;              // [E*2] words of the bit planes a staged level uses
-    std::vector<int> pendingUpload;           // env ids whose freshly generated next level waits for H2D
+    std::vector<int> levelWords;              // [E*D] words of the bit planes a staged level uses
+    std::vector<int> pendingUpload;           // level ids (env * D + slot) whose freshly generated level waits for H2D
+    // an env's levels come from one stateful generator (RNG stream, Sokoban's unplayed levels): its jobs run one after another, in the order
+    // they were scheduled, on whichever worker drains the env's queue
+    std::vector<std::deque<std::pair<int, int>>> genQueue;  // [E] (slot, serial) waiting for the env's generator
+    std::vector<uint8_t> genBusy;                           // [E] a worker is draining the env's queue
     std::vector<std::string> genErrors;
     std::mutex genMutex;
     bool rtableDirty = true;
@@ -299,9 +308,30 @@ struct mv_engine {
     PinBuf<float> h_finalDepth;
 
     // ------------------------------------------------------------------ level generation scheduling
-    // generate the level for episode `serial` of env e into staging slot s (worker thread)
+    // generate the level for episode `serial` of env e into staging slot s, after every job scheduled for the env before
     void scheduleGen(int e, int s, int serial) {
-        pool->submit([this, e, s, serial] {
+        {
+            std::lock_guard<std::mutex> lk(genMutex);
+            genQueue[size_t(e)].emplace_back(s, serial);
+            if (genBusy[size_t(e)]) return;  // the worker draining the env's queue takes it next
+            genBusy[size_t(e)] = 1;
+        }
+        pool->submit([this, e] {
+            for (;;) {
+                std::pair<int, int> job;
+                {
+                    std::lock_guard<std::mutex> lk(genMutex);
+                    if (genQueue[size_t(e)].empty()) { genBusy[size_t(e)] = 0; return; }
+                    job = genQueue[size_t(e)].front();
+                    genQueue[size_t(e)].pop_front();
+                }
+                generateLevel(e, job.first, job.second);
+            }
+        });
+    }
+    // worker thread: one level of env e's stream into slot s
+    void generateLevel(int e, int s, int serial) {
+        {
             mv::LevelOut out;
             // the env's own scenario's capacity, not the engine's pitch: a level is accepted exactly as in a single-scenario engine
             const int cap = mv::gridCapacity(envScenario[size_t(e)]);
@@ -324,11 +354,11 @@ struct mv_engine {
             if (int(out.statics.size()) > staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
                 std::lock_guard<std::mutex> lk(genMutex);
                 wantStaticCap = std::max(wantStaticCap, int(out.statics.size()));
-                oversize.emplace_back(e * 2 + s, std::move(out));
+                oversize.emplace_back(e * levelSlots + s, std::move(out));
                 return;
             }
-            stageLevel(e * 2 + s, out);
-        });
+            stageLevel(e * levelSlots + s, out);
+        }
     }
     // worker thread (or flushUploads for parked levels): copy a generated level into the pinned staging mirrors and queue its upload
     void stageLevel(int id, const mv::LevelOut &out) {
@@ -338,16 +368,15 @@ struct mv_engine {
                 std::memcpy(h_statics.p + size_t(id) * size_t(staticCap), out.statics.data(), sizeof(MvBox) * out.statics.size());
                 std::memcpy(h_staticRot.p + size_t(id) * size_t(staticCap) * 2, out.staticRot.data(), sizeof(float) * out.staticRot.size());
             }
-            const int e = id >> 1, s = id & 1;
-            if (!out.deco.empty()) std::memcpy(&h_deco.p[(size_t(e) * 2 + s) * size_t(decoCap)], out.deco.data(), sizeof(MvDeco) * out.deco.size());
-            uint32_t *dst = h_solid.p + (size_t(e) * 2 + s) * 3 * gridWords;  // planes: solid, exit, lava
+            if (!out.deco.empty()) std::memcpy(&h_deco.p[size_t(id) * size_t(decoCap)], out.deco.data(), sizeof(MvDeco) * out.deco.size());
+            uint32_t *dst = h_solid.p + size_t(id) * 3 * gridWords;  // planes: solid, exit, lava
             const size_t nw = std::min(out.solid.size(), size_t(gridWords));
             std::memcpy(dst, out.solid.data(), sizeof(uint32_t) * nw);
             std::memcpy(dst + gridWords, out.exitBits.data(), sizeof(uint32_t) * nw);
             std::memcpy(dst + 2 * size_t(gridWords), out.lavaBits.data(), sizeof(uint32_t) * nw);
-            levelWords[size_t(e) * 2 + s] = int(nw);
+            levelWords[size_t(id)] = int(nw);
             std::lock_guard<std::mutex> lk(genMutex);
-            pendingUpload.push_back(e * 2 + s);
+            pendingUpload.push_back(id);
         }
     }
     // more static boxes per level: re-pitch every array that is laid out by staticCap (level statics, instance lists), device and host
@@ -357,15 +386,15 @@ struct mv_engine {
         if (newInstCap > mvr::kMaxInstancesPerEnv) { setError("a level needs more drawables than the draw-order key can number"); return MV_ERR_CAPACITY; }
         MV_CUDA(cudaStreamSynchronize(stream));
         DevBuf<MvBox> nStat; DevBuf<float> nRot; DevBuf<MvInstance> nInst; PinBuf<MvBox> hStat; PinBuf<float> hRot;
-        const size_t rows = size_t(E) * 2;
+        const size_t rows = size_t(E) * levelSlots;
         // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside
         struct Repitch { DevBuf<uint8_t> *buf; DevBuf<uint8_t> next; size_t rows, oldPitch, newPitch; };
         std::vector<Repitch> storeGrow;
         for (auto &st : stores) {
             if (!st) continue;
             const size_t r = size_t(st->rows);
-            storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * 2, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
-            storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * 2, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
+            storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * levelSlots, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
+            storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * levelSlots, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
             storeGrow.push_back({&st->slabs[kSlabInst], {}, r, sizeof(MvInstance) * instCap, sizeof(MvInstance) * newInstCap});
         }
         bool storesOk = true;
@@ -457,6 +486,7 @@ struct mv_engine {
         sp.envOrder = rasterSched ? d_viewCost.p + costItems() : nullptr;  // a permutation at all times (identity until a cost-ordered raster launch has sorted it)
         sp.ends = dEnds;
         sp.repeat = actionRepeat;
+        sp.slots = levelSlots;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
@@ -655,15 +685,21 @@ struct mv_engine {
         return MV_OK;
     }
 
-    // after a step (or forced reset): flip host mirrors for finished envs and start generating the level after next
+    // after a step (or forced reset): move the host mirrors of finished envs to the next slot of the ring and start generating the level
+    // D - 1 episodes ahead into the slot just freed
     void afterFlip(const uint8_t *flipped) {
+        const int D = levelSlots;
         for (int e = 0; e < E; ++e) {
             if (!flipped || flipped[e]) {
-                hostSlot[size_t(e)] ^= 1;
+                hostSlot[size_t(e)] = (hostSlot[size_t(e)] + 1) % D;
                 hostEpisode[size_t(e)] += 1;
-                scheduleGen(e, hostSlot[size_t(e)] ^ 1, hostEpisode[size_t(e)] + 1);
+                scheduleGen(e, (hostSlot[size_t(e)] + D - 1) % D, hostEpisode[size_t(e)] + D - 1);
             }
         }
+    }
+    // (re)build env e's staged levels, episodes after the live one in order, from its generator's current state
+    void restage(int e) {
+        for (int i = 1; i < levelSlots; ++i) scheduleGen(e, (hostSlot[size_t(e)] + i) % levelSlots, hostEpisode[size_t(e)] + i);
     }
 
     // per-kernel times exist only when the kernels run back to back (overlap off); with the dependent launch the step and
@@ -701,14 +737,16 @@ struct mv_engine {
         std::memcpy(h_doneReasons.p, p.reasons.p, E);
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
         p.valid = false;
-        // the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes again sooner
-        // flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on.  Counted in calls
-        // whatever option "action_repeat" is: retiring, regenerating and uploading happen once per call, so the level pipeline is three
-        // calls deep (the kernel's request rule, num_frames >= 3 * repeat ticks, is the same three calls counted on the device)
+        // with two level slots the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes
+        // again sooner flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on.  Counted
+        // in calls whatever option "action_repeat" is: retiring, regenerating and uploading happen once per call, so the level pipeline is
+        // three calls deep (the kernel's request rule, num_frames >= 3 * repeat ticks, is the same three calls counted on the device).  With
+        // four slots an env ends at most once per call, and the level replacing the end of call j is uploaded before kernel j + 3, when the
+        // ends of calls j, j + 1 and j + 2 have used the three staged levels at most: there is nothing to check
         if (lastAsyncDone.empty()) lastAsyncDone.assign(size_t(E), -1000);
         for (int e = 0; e < E; ++e)
             if (h_dones.p[e]) {
-                if (int64_t(p.step) - lastAsyncDone[size_t(e)] < 3) asyncContractBroken = true;
+                if (levelSlots == 2 && int64_t(p.step) - lastAsyncDone[size_t(e)] < 3) asyncContractBroken = true;
                 lastAsyncDone[size_t(e)] = int64_t(p.step);
             }
         afterFlip(h_dones.p);
@@ -722,9 +760,10 @@ struct mv_engine {
         }
         return MV_OK;
     }
-    // asynchronous device-resident step: returns after enqueueing.  Episode bookkeeping lags two steps, which is safe
+    // asynchronous device-resident step: returns after enqueueing.  Episode bookkeeping lags two steps, which is safe with two level slots
     // because an env cannot finish twice within four steps (doneWithTimer leaves 0.3 s = 4.5 steps, scenario.hpp:114-117); with option
-    // "action_repeat" k a call runs k ticks, and DESIGN.md section 2 gives the shortest natural episodes that bound k
+    // "action_repeat" k a call runs k ticks, and DESIGN.md section 2 gives the shortest natural episodes that bound k.  Option
+    // "level_slots" 4 lifts the bound (see retire)
     int stepAsync(const int32_t *dActions, const uint8_t *dEnds) {
         if (!didReset) { setError("mv_step_device before mv_reset"); return MV_ERR_STATE; }
         if (hostStepPending) { const int rcp = stepEnd(); if (rcp) return rcp; }
@@ -789,10 +828,11 @@ struct mv_engine {
     // every per-env device row, in the order of StateStore::slabs
     std::array<EnvSlab, kSlabCount> envSlabs() {
         auto s = [](void *p, int units, size_t bytes) { return EnvSlab{static_cast<uint8_t *>(p), units, bytes}; };
+        const int D = levelSlots;
         return {{s(d_envs.p, 1, sizeof(MvEnvState)), s(d_agents.p, 1, sizeof(MvAgent) * A), s(d_objects.p, 1, sizeof(MvObject) * MV_MAX_OBJECTS),
                  s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instCap), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
-                 s(d_views.p, 1, sizeof(float) * 16 * A), s(d_levels.p, 2, sizeof(MvLevel)), s(d_statics.p, 2, sizeof(MvBox) * staticCap),
-                 s(d_staticRot.p, 2, sizeof(float) * 2 * staticCap), s(d_deco.p, 2, sizeof(MvDeco) * decoCap), s(d_solid.p, 2, sizeof(uint32_t) * 3 * gridWords),
+                 s(d_views.p, 1, sizeof(float) * 16 * A), s(d_levels.p, D, sizeof(MvLevel)), s(d_statics.p, D, sizeof(MvBox) * staticCap),
+                 s(d_staticRot.p, D, sizeof(float) * 2 * staticCap), s(d_deco.p, D, sizeof(MvDeco) * decoCap), s(d_solid.p, D, sizeof(uint32_t) * 3 * gridWords),
                  s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t)),
                  s(d_doneReasons.p, 1, 1)}};
     }
@@ -852,8 +892,10 @@ struct mv_engine {
             r.gen = gens[size_t(e)];
             r.scenario = envScenarioName[size_t(e)];
             r.slot = hostSlot[size_t(e)]; r.episode = hostEpisode[size_t(e)];
-            for (int s = 0; s < 2; ++s) {
-                const size_t id = size_t(e) * 2 + s;
+            const size_t D = size_t(levelSlots);
+            r.words.resize(D); r.level.resize(D); r.statics.resize(D); r.staticRot.resize(D); r.deco.resize(D); r.solid.resize(D);
+            for (size_t s = 0; s < D; ++s) {
+                const size_t id = size_t(e) * D + s;
                 const MvLevel &L = h_levels.p[id];
                 r.level[s] = L;
                 r.words[s] = levelWords[id];
@@ -888,8 +930,8 @@ struct mv_engine {
             const StateStore::HostRow &r = st.host[size_t(rows[i])];
             gens[size_t(e)] = *r.gen;
             hostSlot[size_t(e)] = r.slot; hostEpisode[size_t(e)] = r.episode;
-            for (int s = 0; s < 2; ++s) {
-                const size_t id = size_t(e) * 2 + s;
+            for (size_t s = 0; s < r.level.size(); ++s) {  // the store's slot count is the engine's
+                const size_t id = size_t(e) * size_t(levelSlots) + s;
                 h_levels.p[id] = r.level[s];
                 levelWords[id] = r.words[s];
                 std::copy(r.statics[s].begin(), r.statics[s].end(), h_statics.p + id * staticCap);
@@ -914,11 +956,11 @@ struct mv_engine {
     int resetEnvs(const int32_t *envs, const int32_t *seeds, int n) {
         int rc = quiesce();
         if (rc) return rc;
-        if (seeds) {  // the staged slot takes the first level of the new stream, as in a fresh engine; the workers are idle after quiesce
+        if (seeds) {  // the staged slots take the first levels of the new stream, in order, as in a fresh engine; the workers are idle after quiesce
             for (int i = 0; i < n; ++i) {
                 const int e = envs[i];
                 gens[size_t(e)].restart((unsigned long)seeds[i]);
-                scheduleGen(e, hostSlot[size_t(e)] ^ 1, hostEpisode[size_t(e)] + 1);
+                restage(e);
             }
             rc = flushUploads();
             if (rc) return rc;
@@ -1099,6 +1141,8 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
         return fail(MV_ERR_ARG);
     }
     e->levelWords.assign(size_t(e->E) * 2, 0);
+    e->genQueue.resize(size_t(e->E));
+    e->genBusy.assign(size_t(e->E), 0);
     e->pool.reset(new WorkerPool(e->threads));
     // one pitch for all envs: the largest capacity among the engine's scenarios
     e->gridCells = 0; e->decoCap = 0;
@@ -1179,6 +1223,23 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         h->actionRepeat = value;
         return MV_OK;
     }
+    if (k == "level_slots") {  // level slots per env (see the header): every [E][D] array is allocated again, on the device and pinned
+        if (h->didReset) { h->setError("option level_slots must be set before the first reset"); return MV_ERR_STATE; }
+        if (value != 2 && value != 4) { h->setError("level_slots must be 2 or 4"); return MV_ERR_ARG; }
+        const size_t rows = size_t(h->E) * size_t(value), cap = size_t(h->staticCap), deco = size_t(h->decoCap), words = size_t(h->gridWords) * 3;
+        h->d_levels.free(); h->d_statics.free(); h->d_staticRot.free(); h->d_deco.free(); h->d_solid.free();
+        h->h_levels.free(); h->h_statics.free(); h->h_staticRot.free(); h->h_deco.free(); h->h_solid.free();
+        h->levelSlots = value;
+        h->levelWords.assign(rows, 0);
+        if (h->d_levels.alloc(rows) != cudaSuccess || h->d_statics.alloc(rows * cap) != cudaSuccess || h->d_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
+            h->d_deco.alloc(rows * deco) != cudaSuccess || h->d_solid.alloc(rows * words) != cudaSuccess || h->h_levels.alloc(rows) != cudaSuccess ||
+            h->h_statics.alloc(rows * cap) != cudaSuccess || h->h_staticRot.alloc(rows * cap * 2) != cudaSuccess || h->h_deco.alloc(rows * deco) != cudaSuccess ||
+            h->h_solid.alloc(rows * words) != cudaSuccess) {
+            h->setError("level_slots: allocation failed");
+            return MV_ERR_CUDA;
+        }
+        return MV_OK;
+    }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches
         if (value < 32 || value > mvr::kMaxTriCap) { h->setError("tri_cap out of range [32,1022]"); return MV_ERR_ARG; }
         const int old = h->triCap;
@@ -1190,7 +1251,7 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     if (k == "static_cap") {  // initial size of the per-level static-box arrays (they grow on demand; tests start small to exercise that)
         if (h->didReset) { h->setError("option static_cap must be set before the first reset"); return MV_ERR_STATE; }
         if (value < 1 || value > (1 << 20)) return MV_ERR_ARG;
-        const size_t rows = size_t(h->E) * 2;
+        const size_t rows = size_t(h->E) * h->levelSlots;
         h->d_statics.free(); h->d_staticRot.free(); h->h_statics.free(); h->h_staticRot.free(); h->d_inst.free();
         h->staticCap = value;
         h->instCap = MV_DYN_INSTANCES + h->staticCap + h->decoCap;
@@ -1229,13 +1290,13 @@ int mv_set_option(mv_handle h, const char *key, int value) {
 }
 
 static void regenerateNext(mv_handle h) {
-    // (re)build every env's pre-staged next level from its current RNG state
-    for (int e = 0; e < h->E; ++e) h->scheduleGen(e, h->hostSlot[size_t(e)] ^ 1, h->hostEpisode[size_t(e)] + 1);
+    // (re)build every env's pre-staged levels from its current RNG state
+    for (int e = 0; e < h->E; ++e) h->restage(e);
 }
 
 static void ensureMirrors(mv_handle h) {
     if (h->hostSlot.empty()) {
-        h->hostSlot.assign(size_t(h->E), 1);      // first flip lands on slot 0
+        h->hostSlot.assign(size_t(h->E), h->levelSlots - 1);  // first flip lands on slot 0
         h->hostEpisode.assign(size_t(h->E), -1);  // ... as episode 0
     }
 }
@@ -1256,7 +1317,7 @@ int mv_seed_env(mv_handle h, int env, int seed) {
     if (!h || env < 0 || env >= h->E) return MV_ERR_ARG;
     h->pool->waitAll();
     h->gens[size_t(env)].seed((unsigned long)seed);
-    if (h->didReset) h->scheduleGen(env, h->hostSlot[size_t(env)] ^ 1, h->hostEpisode[size_t(env)] + 1);
+    if (h->didReset) h->restage(env);  // every staged level, from the new stream in order
     return MV_OK;
 }
 
@@ -1268,10 +1329,11 @@ int mv_reset(mv_handle h) {
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     if (h->didReset) { const int rcd = h->drain(); if (rcd) return rcd; }
     if (!h->didReset) {
-        // initial device state: slot 1 / episode -1 so that the forced flip lands on (slot 0, episode 0)
+        // initial device state: the last slot / episode -1 so that the forced flip lands on (slot 0, episode 0); the first levels go to
+        // slots 0 .. D - 2 as episodes 0 .. D - 2
         std::vector<MvEnvState> init(size_t(h->E));
         std::memset(init.data(), 0, sizeof(MvEnvState) * init.size());
-        for (auto &s : init) { s.slot = 1; s.episode_idx = -1; mvBzInit(s); }
+        for (auto &s : init) { s.slot = h->levelSlots - 1; s.episode_idx = -1; mvBzInit(s); }
         if (cudaMemcpy(h->d_envs.p, init.data(), sizeof(MvEnvState) * init.size(), cudaMemcpyHostToDevice) != cudaSuccess) { h->setError("env init upload failed"); return MV_ERR_CUDA; }
         if (h->wantFinal) {
             const size_t E = size_t(h->E), N = size_t(h->N), px = size_t(h->W) * h->H;
@@ -1722,7 +1784,7 @@ static void dumpLevelExtras(const MvLevel &L, const MvBox *statics, const float 
 
 int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
-    const size_t lid = size_t(env) * 2 + h->hostSlot[size_t(env)];
+    const size_t lid = size_t(env) * h->levelSlots + h->hostSlot[size_t(env)];
     const MvLevel &L = h->h_levels.p[lid];
     const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
     const float *staticRot = h->h_staticRot.p + lid * size_t(h->staticCap) * 2;
@@ -1764,10 +1826,11 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cudaMemcpy(ag.data(), &h->d_agents.p[size_t(env) * h->A], sizeof(MvAgent) * h->A, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cudaMemcpy(ob.data(), &h->d_objects.p[size_t(env) * MV_MAX_OBJECTS], sizeof(MvObject) * MV_MAX_OBJECTS, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
-    const MvLevel &L = h->h_levels.p[size_t(env) * 2 + es.slot];
+    const size_t lid = size_t(env) * h->levelSlots + es.slot;
+    const MvLevel &L = h->h_levels.p[lid];
     std::vector<float> o;
     int ncol = h->A + L.n_obj;
-    const MvBox *statics = h->h_statics.p + (size_t(env) * 2 + es.slot) * size_t(h->staticCap);
+    const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
     for (int i = 0; i < L.n_static; ++i) ncol += (statics[i].flags & MV_SOLID) ? 1 : 0;
     const float len = L.episode_len;
     o.push_back(es.episode_sec); o.push_back(len); o.push_back(float(es.num_frames)); o.push_back(float(es.highest_tower));
@@ -1809,9 +1872,10 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     MvEnvState es;
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
-    const MvLevel &L = h->h_levels.p[size_t(env) * 2 + es.slot];
-    const uint32_t *sol = h->h_solid.p + (size_t(env) * 2 + es.slot) * 3 * h->gridWords;
-    const MvBox *statics = h->h_statics.p + (size_t(env) * 2 + es.slot) * size_t(h->staticCap);
+    const size_t lid = size_t(env) * h->levelSlots + es.slot;
+    const MvLevel &L = h->h_levels.p[lid];
+    const uint32_t *sol = h->h_solid.p + lid * 3 * h->gridWords;
+    const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
     std::vector<uint8_t> og(size_t(h->gridCells));
     if (cudaMemcpy(og.data(), h->d_objGrid.p + size_t(env) * h->gridCells, og.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     // opacity is a property of the box a solid voxel belongs to

@@ -39,17 +39,17 @@ constexpr float kMaxAcceleration = 35.0f + 15.0f, kMaxAirAcceleration = 3.0f, kE
 constexpr unsigned FULL = 0xffffffffu;
 
 struct StepParams {
-    const MvLevel *levels;       // [E][2]
-    const MvBox *statics;        // [E][2][staticCap] static layout boxes of the two level slots (collider order == draw order)
-    const float *staticRot;      // [E][2][staticCap][2] MV_ROTATED boxes: local x axis in world space (ax, az)
+    const MvLevel *levels;       // [E][slots]
+    const MvBox *statics;        // [E][slots][staticCap] static layout boxes of the level slots (collider order == draw order)
+    const float *staticRot;      // [E][slots][staticCap][2] MV_ROTATED boxes: local x axis in world space (ax, az)
     int staticCap;
-    const uint32_t *solid;       // [E][2][3][gridWords] planes: solid, exit terrain, lava terrain
+    const uint32_t *solid;       // [E][slots][3][gridWords] planes: solid, exit terrain, lava terrain
     uint8_t *objGrid;            // [E][gridCells]
     MvEnvState *envs;            // [E]
     MvAgent *agents;             // [E*A]
     MvObject *objects;           // [E][MV_MAX_OBJECTS]
     MvInstance *instances;       // [E][instStride]
-    const MvDeco *deco;          // [E][2][decoCap] decorations of the two level slots
+    const MvDeco *deco;          // [E][slots][decoCap] decorations of the level slots
     int decoCap, instStride;
     int32_t *instCounts;         // [E][8]
     float *views;                // [E*A][16]
@@ -68,8 +68,9 @@ struct StepParams {
     uint32_t *ready;             // [E] completion stamps polled by the geometry kernel (programmatic dependent launch)
     uint32_t readyStamp;
     const uint32_t *envOrder;  // optional [E]: warp w of the grid steps env envOrder[w] (the order in which the rasteriser will ask for the envs)
-    const uint8_t *ends;         // optional [num_envs] (mv_step_device_ends): ends[env] != 0 ends the episode after this call's last tick, once it has run >= 3 * repeat ticks
+    const uint8_t *ends;         // optional [num_envs] (mv_step_device_ends): ends[env] != 0 ends the episode after this call's last tick (with 2 slots: once it has run >= 3 * repeat ticks)
     int repeat;                  // option "action_repeat": physics ticks per call (1..4), the episode stops them early
+    int slots;                   // option "level_slots": level slots per env (2 or 4), one live and the rest staged in episode order
     int maxObj;                  // upper bound of n_obj over the live and staged levels (sizes the staging copy)
     uint32_t *prof;              // optional [E][16] per-phase cycle stamps (mv_debug_step_profile); nullptr in production
     uint8_t *doneReasons;        // [E] MV_END_* of this step, written beside dones (MV_END_NONE where dones is 0)
@@ -909,9 +910,9 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     }
     __syncwarp();
     int slot = S.env.slot;
-    const MvLevel *L = &P.levels[size_t(env) * 2 + slot];
-    const MvBox *statics = P.statics + (size_t(env) * 2 + slot) * size_t(P.staticCap);
-    const float *staticRot = P.staticRot + (size_t(env) * 2 + slot) * size_t(P.staticCap) * 2;
+    const MvLevel *L = &P.levels[size_t(env) * P.slots + slot];
+    const MvBox *statics = P.statics + (size_t(env) * P.slots + slot) * size_t(P.staticCap);
+    const float *staticRot = P.staticRot + (size_t(env) * P.slots + slot) * size_t(P.staticCap) * 2;
     int ns = L->n_static, no = L->n_obj;
     if (!P.forceReset) mbarWait(&S.mbar, 0);
 
@@ -1141,7 +1142,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                             toVoxel(v3(S.agents[j].object_t[12], S.agents[j].object_t[13], S.agents[j].object_t[14]), cx, cy, cz);
                             if (cx == vx && cy == vy && cz == vz) { collidesWithAgent = true; break; }
                         }
-                        const uint32_t *sol = P.solid + (size_t(env) * 2 + slot) * 3 * P.gridWords;
+                        const uint32_t *sol = P.solid + (size_t(env) * P.slots + slot) * 3 * P.gridWords;
                         auto solidAt = [&](int g) { return g >= 0 && ((sol[g >> 5] >> (g & 31)) & 1u); };
                         auto objAt = [&](int g) { return g >= 0 ? int(objGrid[g]) : int(MV_NO_OBJECT); };
                         const bool empty = !solidAt(gi) && objAt(gi) == MV_NO_OBJECT;
@@ -1208,7 +1209,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                         }
                     }
                 }
-                const uint32_t *planes = P.solid + (size_t(env) * 2 + slot) * 3 * P.gridWords;
+                const uint32_t *planes = P.solid + (size_t(env) * P.slots + slot) * 3 * P.gridWords;
                 auto planeBit = [&](int plane, int g) { return g >= 0 && ((planes[size_t(plane) * P.gridWords + (g >> 5)] >> (g & 31)) & 1u); };
                 // FallDetectionComponent::resetAgent (component_fall_detection.hpp:44-56) -> KinematicCharacterController::warp
                 auto resetAgent = [&](int i) {
@@ -1411,9 +1412,10 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                 }
                 for (int i = 0; i < A; ++i) S.agents[i].total_reward += S.lastReward[i];
                 e.num_frames += 1;
-                // a requested end (mv_step_device_ends) is a timer end after the call's last tick; before the episode's third call the env's next
-                // level may not be staged yet (every call of an episode but one that ends runs all its ticks, so that is 3 * repeat ticks)
-                const bool requested = P.ends && P.ends[env] && tick == P.repeat - 1 && e.num_frames >= 3 * P.repeat;
+                // a requested end (mv_step_device_ends) is a timer end after the call's last tick; with two level slots, before the episode's
+                // third call the env's next level may not be staged yet (every call of an episode but one that ends runs all its ticks, so that
+                // is 3 * repeat ticks).  Four slots always hold the next level
+                const bool requested = P.ends && P.ends[env] && tick == P.repeat - 1 && (P.slots != 2 || e.num_frames >= 3 * P.repeat);
                 S.doneFlag = (e.episode_sec >= len || requested) ? 1 : 0;
             }
             __syncwarp();
@@ -1461,16 +1463,16 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
         if (lane < 8) tCounts[lane] = counts[lane];
         for (int i = lane; i < A * 16; i += 32) tViews[i] = P.views[size_t(env) * A * 16 + i];
         __syncwarp();
-        writeInstances(S, *L, statics, P.deco + (size_t(env) * 2 + slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
+        writeInstances(S, *L, statics, P.deco + (size_t(env) * P.slots + slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
         __syncwarp();
     }
 
     if (resetNow) {
-        // flip to the pre-staged next level (episode end, or mv_reset forcing a new episode everywhere)
-        slot ^= 1;
-        L = &P.levels[size_t(env) * 2 + slot];
-        statics = P.statics + (size_t(env) * 2 + slot) * size_t(P.staticCap);
-        staticRot = P.staticRot + (size_t(env) * 2 + slot) * size_t(P.staticCap) * 2;
+        // flip to the pre-staged next level (episode end, or mv_reset forcing a new episode everywhere): the slots form a ring
+        slot = slot + 1 == P.slots ? 0 : slot + 1;
+        L = &P.levels[size_t(env) * P.slots + slot];
+        statics = P.statics + (size_t(env) * P.slots + slot) * size_t(P.staticCap);
+        staticRot = P.staticRot + (size_t(env) * P.slots + slot) * size_t(P.staticCap) * 2;
         if (lane == 0) {
             S.env.slot = slot;
             S.env.episode_idx += 1;
@@ -1498,7 +1500,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     __syncwarp();
     MV_PROBE(6);  // outputs, flip/reset, object write-back
 
-    writeInstances(S, *L, statics, P.deco + (size_t(env) * 2 + slot) * P.decoCap, P.instances + size_t(env) * P.instStride, P.instCounts + size_t(env) * 8, P.views + size_t(env) * A * 16, A, resetNow, lane);
+    writeInstances(S, *L, statics, P.deco + (size_t(env) * P.slots + slot) * P.decoCap, P.instances + size_t(env) * P.instStride, P.instCounts + size_t(env) * 8, P.views + size_t(env) * A * 16, A, resetNow, lane);
 
     MV_PROBE(7);  // instance list + views
 
