@@ -34,6 +34,14 @@ typedef struct mv_engine *mv_handle;
                                 * 0.3 s grace that follows: terminal */
 #define MV_END_REQUESTED 3     /* the caller's end mask (mv_step_device_ends): truncated */
 
+/* segmentation classes (option "segmentation"): a pixel's value is class << 8 | index, 0 where nothing was drawn */
+#define MV_SEG_NONE 0          /* background: nothing drawn (depth 0) */
+#define MV_SEG_STATIC 1        /* static layout boxes and static decorations (hex-maze walls, Rearrange's target arrangement, ...); index 0 */
+#define MV_SEG_TERRAIN 2       /* terrain slabs; index = the slab's TerrainType bit number (0 exit, 1 lava, 2 building zone) */
+#define MV_SEG_OBJECT 3        /* movable objects, carried or not; index = the object's index in the level's object list */
+#define MV_SEG_AGENT 4         /* an agent's body, eyes and HUD bar; index = agent index within the env */
+#define MV_SEG_REWARD 5        /* reward objects (diamonds, Collect's objects, hex-maze objects, pillars); index = reward-object index */
+
 /* MegaverseGym::MegaverseGym (megaverse.cpp:38-58).  num_threads = host level-generation workers (the reference's
  * numSimulationThreads drove Bullet on the CPU, vector_env.cpp:6-40).  device = CUDA ordinal. */
 int mv_create(const char *scenario, int w, int h, int num_envs, int num_agents_per_env, int num_threads, int device,
@@ -109,6 +117,21 @@ int mv_final_obs_host(mv_handle h, const uint8_t **out);
 int mv_final_depth_host(mv_handle h, const float **out);
 int mv_final_obs_device(mv_handle h, uint8_t **d_final_obs);
 int mv_final_depth_device(mv_handle h, float **d_final_depth);
+/* Segmentation, option "segmentation" (0/1, before the first reset: MV_ERR_STATE after it, MV_ERR_ARG for any other value; default 0).
+ * uint16[N][h][w], view index env*A + agent, rows as in the observation tensor: the MV_SEG_* class of the drawable behind each pixel << 8 |
+ * its index, 0 exactly where nothing was drawn (exactly where depth is 0).  The rasteriser names the drawable whose fragment won the pixel,
+ * so the tensor shows coverage and the depth-tie order exactly, in both shading modes.  Every call that draws the batch writes it beside
+ * the observations and is delivered the same way: mv_step and mv_step_begin/end into the host buffer (mv_segmentation_host), on return
+ * like the observations; mv_step_device[_ends] into the device buffer (mv_segmentation_device) in stream order, copied down by
+ * mv_fetch_obs; mv_reset, mv_reset_envs and mv_states_load draw it again.  Nothing else changes with the option: obs, depth, rewards,
+ * dones, done reasons, true objectives and terminal frames are byte-identical with it on and off.
+ * Memory: 2 B per pixel in HBM and again pinned (18 432 B per view at 128 x 72: 75.5 MB each at Collect 1 024 x 4); nothing is
+ * allocated while the option is off.
+ * Limits: mv_draw_hires and mv_debug_render_instances draw no segmentation; mv_set_obs_buffer does not redirect it (it stays in the
+ * engine's own buffer); terminal frames (option final_obs) carry none; the multi-GPU gather does not gather it.
+ * Both calls return MV_ERR_ARG when the option is off; the device pointer is refused (MV_ERR_STATE) exactly when mv_depth_device's is. */
+int mv_segmentation_host(mv_handle h, const uint16_t **out);
+int mv_segmentation_device(mv_handle h, uint16_t **d_seg);
 
 /* MegaverseGym::getRewardShaping / setRewardShaping (megaverse.cpp:214-222).  get: fills up to cap entries, returns the
  * number of keys in *n.  Key strings are owned by the engine. */
@@ -135,6 +158,8 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * otherwise leave the reference's level sequence; with 1 the env takes the next level of its stream instead and mv_levels_skipped
  * counts it),
  * "final_obs" (0/1, before the first reset, default 0: terminal frames of ended episodes, see mv_final_obs_host),
+ * "segmentation" (0/1, before the first reset, default 0: the class and index of the drawable behind every pixel, see
+ * mv_segmentation_host),
  * "action_repeat" (1..4, before the first reset (MV_ERR_STATE after it, MV_ERR_ARG outside the range), default 1: action repeat, or
  * frame skip, inside the engine.  Every step call (mv_step, mv_step_begin/end, mv_step_device[_ends]) runs up to k physics ticks of
  * 1/15 s per env with the same action masks, then draws once.  Interact acts on the first tick only (it toggles carrying, so one call
@@ -203,8 +228,8 @@ int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth);
  * valid until the next mv_draw_hires / mv_close */
 int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out);
 int mv_sync(mv_handle h);
-/* after mv_step_device steps: waits, then copies the device obs (and depth, when enabled) into the host buffers that
- * mv_obs_host / mv_depth_host return */
+/* after mv_step_device steps: waits, then copies the device obs (and depth and segmentation, when enabled) into the host buffers that
+ * mv_obs_host / mv_depth_host / mv_segmentation_host return */
 int mv_fetch_obs(mv_handle h);
 int mv_actions_device(mv_handle h, int32_t **d_masks);
 int mv_obs_device(mv_handle h, uint8_t **d_obs);

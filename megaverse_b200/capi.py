@@ -12,6 +12,8 @@ _lib = None
 
 MV_OK, MV_ERR_ARG, MV_ERR_CUDA, MV_ERR_CAPACITY, MV_ERR_STATE = 0, -1, -2, -3, -4
 MV_END_NONE, MV_END_TIME, MV_END_SOLVED, MV_END_REQUESTED = 0, 1, 2, 3  # done_reasons(): why an episode ended
+# segmentation(): a pixel is class << 8 | index of the drawable behind it, 0 where nothing was drawn
+MV_SEG_NONE, MV_SEG_STATIC, MV_SEG_TERRAIN, MV_SEG_OBJECT, MV_SEG_AGENT, MV_SEG_REWARD = 0, 1, 2, 3, 4, 5
 
 
 class MegaverseError(RuntimeError):
@@ -42,7 +44,8 @@ def lib():
         L.mv_reset_envs.argtypes = [vp, vp, vp, ci]
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
-                     "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device"):
+                     "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device",
+                     "mv_segmentation_host", "mv_segmentation_device"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
         L.mv_get_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(ci)]
         L.mv_set_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci]
@@ -75,14 +78,14 @@ EXPORTS = [
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
-    "mv_final_depth_device", "mv_last_final_ms",
+    "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device",
 ]
 
 
 class Engine:
     """Thin object wrapper: one method per C entry point, numpy views over engine-owned host memory."""
 
-    def __init__(self, scenario, num_envs, num_agents, w=128, h=72, num_threads=1, device=0, params=None, depth=False):
+    def __init__(self, scenario, num_envs, num_agents, w=128, h=72, num_threads=1, device=0, params=None, depth=False, segmentation=False):
         """scenario: one name for every env, or a list of num_envs names (env e runs scenario[e]: mv_create_mixed)"""
         L = lib()
         params = params or {}
@@ -102,6 +105,8 @@ class Engine:
         self.E, self.A, self.N, self.w, self.h = num_envs, num_agents, num_envs * num_agents, w, h
         if depth:
             self._ck(L.mv_set_option(self._h, b"depth", 1))
+        if segmentation:
+            self._ck(L.mv_set_option(self._h, b"segmentation", 1))
 
     def _ck(self, rc):
         if rc != MV_OK:
@@ -175,12 +180,13 @@ class Engine:
     def device_array(self, what="obs"):
         """zero-copy handle on an engine-owned device tensor for any consumer of the CUDA array interface
         (`torch.as_tensor(eng.device_array("obs"), device="cuda")`, CuPy, Numba): "obs" uint8[N,h,w,4], "depth" float32[N,h,w],
-        "rewards" float32[N], "dones" uint8[E], "done_reasons" uint8[E] (MV_END_*), "true_objectives" float32[N], and with option final_obs
-        "final_obs" uint8[N,h,w,4] / "final_depth" float32[N,h,w] (terminal frames of mv_step_device steps).  Valid in the engine stream's
-        order (mv_stream) until mv_close."""
+        "rewards" float32[N], "dones" uint8[E], "done_reasons" uint8[E] (MV_END_*), "true_objectives" float32[N], with option final_obs
+        "final_obs" uint8[N,h,w,4] / "final_depth" float32[N,h,w] (terminal frames of mv_step_device steps), and with option segmentation
+        "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index).  Valid in the engine stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
-                  "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4")}
+                  "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
+                  "segmentation": (px, "<u2")}
         shape, typestr = shapes[what]
         ptr, stream = self.device_ptr(what), self.stream()
 
@@ -204,6 +210,10 @@ class Engine:
 
     def depth(self):
         return self._host("mv_depth_host", (self.N, self.h, self.w), np.float32)
+
+    def segmentation(self):
+        """uint16[N,h,w] (option segmentation): MV_SEG_* class << 8 | index of the drawable behind each pixel, 0 where nothing was drawn"""
+        return self._host("mv_segmentation_host", (self.N, self.h, self.w), np.uint16)
 
     def rewards(self):
         return self._host("mv_rewards", (self.N,), np.float32)

@@ -174,6 +174,7 @@ struct mv_engine {
     int triCap = 368;              // triangle-list capacity of one raster CTA (shared memory); larger views are drawn in several batches
     std::atomic<int> maxObjSeen{0};
     bool wantDepth = false, obsToHost = true, didReset = false, fastShading = true;
+    bool wantSeg = false;          // option "segmentation": the rasteriser also writes each pixel's drawable tag (d_seg / h_seg)
     bool hostStepPending = false;  // between mv_step_begin and mv_step_end
     bool skipUnfitLevels = false;  // option "skip_unfit_levels": replace a level that exceeds a fixed capacity by the stream's next one
     std::atomic<int> levelsSkipped{0};
@@ -217,6 +218,7 @@ struct mv_engine {
     DevBuf<float> d_trueObj;
     DevBuf<uint8_t> d_obs;
     DevBuf<float> d_depth;
+    DevBuf<uint16_t> d_seg;        // [N][H][W], with option segmentation (never redirected by mv_set_obs_buffer)
     uint8_t *obsOut = nullptr;     // where the rasteriser writes in HBM: d_obs, or the caller's tensor slice (mv_set_obs_buffer)
     float *depthOut = nullptr;
     DevBuf<int32_t> d_faults;
@@ -257,6 +259,7 @@ struct mv_engine {
     PinBuf<float> h_trueObj;
     PinBuf<uint8_t> h_obs;
     PinBuf<float> h_depth;
+    PinBuf<uint16_t> h_seg;
     PinBuf<int32_t> h_faults;
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
@@ -558,6 +561,9 @@ struct mv_engine {
         if (vp.envMask) {
             if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true, true>, vp));
             else MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<false, true>, vp));
+        } else if (vp.seg) {
+            if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true, false, true>, vp));
+            else MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<false, false, true>, vp));
         } else if (fastShading) MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<true>, vp));
         else MV_CUDA(cudaLaunchKernelEx(&cfg, mvr::viewKernel<false>, vp));
         launches += 1;
@@ -576,6 +582,7 @@ struct mv_engine {
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         // pinned allocations are mapped into the device address space (UVA), so the kernel can store through the host pointer
         vp.obs = rasterToHost ? h_obs.p : obsOut; vp.depth = wantDepth ? (rasterToHost ? h_depth.p : depthOut) : nullptr;
+        vp.seg = wantSeg ? (rasterToHost ? h_seg.p : d_seg.p) : nullptr;
         vp.stats = d_rasterStats.p;
         // programmatic dependent launch: the grid may start before the step kernel has drained; a CTA waits for its env's stamp
         vp.ready = dep ? d_ready.p : nullptr; vp.readyStamp = dep ? readyStamp : 0;
@@ -601,6 +608,7 @@ struct mv_engine {
             MV_CUDA(cudaStreamWaitEvent(copyStream, sliceEv[size_t(si)], 0));
             MV_CUDA(cudaMemcpyAsync(h_obs.p + size_t(base) * px * 4, obsOut + size_t(base) * px * 4, size_t(cnt) * px * 4, cudaMemcpyDeviceToHost, copyStream));
             if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p + size_t(base) * px, depthOut + size_t(base) * px, sizeof(float) * size_t(cnt) * px, cudaMemcpyDeviceToHost, copyStream));
+            if (wantSeg) MV_CUDA(cudaMemcpyAsync(h_seg.p + size_t(base) * px, d_seg.p + size_t(base) * px, sizeof(uint16_t) * size_t(cnt) * px, cudaMemcpyDeviceToHost, copyStream));
         }
         return MV_OK;
     }
@@ -611,7 +619,7 @@ struct mv_engine {
         if (!copyObs || rasterToHost) sliceCount = 1;
         else if (hostSlicesOpt > 0) sliceCount = std::min(hostSlicesOpt, E);
         else {  // four slices: the best copy-engine form at 151 MB (H100)
-            const size_t bytes = size_t(N) * W * H * (wantDepth ? 8 : 4);
+            const size_t bytes = size_t(N) * W * H * ((wantDepth ? 8 : 4) + (wantSeg ? 2 : 0));
             sliceCount = int(std::max<size_t>(1, std::min<size_t>({size_t(4), size_t(E), bytes / (size_t(32) << 20)})));
         }
     }
@@ -659,13 +667,15 @@ struct mv_engine {
         int maxOptin = 0;
         MV_CUDA(cudaDeviceGetAttribute(&maxOptin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         if (int(rasterSmem) > maxOptin) { setError("tri_cap needs more shared memory than an SM has"); return MV_ERR_ARG; }
-        for (int fast = 0; fast < 2; ++fast) {
-            const void *fn = fast ? reinterpret_cast<const void *>(mvr::viewKernel<true>) : reinterpret_cast<const void *>(mvr::viewKernel<false>);
+        const void *plain[4] = {reinterpret_cast<const void *>(mvr::viewKernel<false>), reinterpret_cast<const void *>(mvr::viewKernel<true>),
+                                reinterpret_cast<const void *>(mvr::viewKernel<false, false, true>), reinterpret_cast<const void *>(mvr::viewKernel<true, false, true>)};
+        for (int v = 0; v < 4; ++v) {  // the grid fits every variant a step may launch (with and without segmentation)
+            const void *fn = plain[v];
             MV_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, maxOptin));  // per function, not per engine: allow the device maximum
             int perSM = 0;
             MV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, mvr::kThreads, rasterSmem));
             if (perSM < 1) { setError("raster kernel does not fit on an SM with this tri_cap"); return MV_ERR_CUDA; }
-            rasterCtasPerSM = fast ? std::min(rasterCtasPerSM, perSM) : perSM;
+            rasterCtasPerSM = v ? std::min(rasterCtasPerSM, perSM) : perSM;
         }
         rasterGrid = numSMs * rasterCtasPerSM;
         int finalPerSM = 0;
@@ -720,6 +730,7 @@ struct mv_engine {
         if (copyObs && !rasterToHost && sliceCount <= 1) {
             MV_CUDA(cudaMemcpyAsync(h_obs.p, obsOut, size_t(N) * W * H * 4, cudaMemcpyDeviceToHost, stream));
             if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p, depthOut, sizeof(float) * size_t(N) * W * H, cudaMemcpyDeviceToHost, stream));
+            if (wantSeg) MV_CUDA(cudaMemcpyAsync(h_seg.p, d_seg.p, sizeof(uint16_t) * size_t(N) * W * H, cudaMemcpyDeviceToHost, stream));
         }
         if (!wait) return MV_OK;
         MV_CUDA(cudaStreamSynchronize(stream));
@@ -1013,9 +1024,9 @@ struct mv_engine {
         stores.clear();
         h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
-        d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_faults.free();
+        d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_seg.free(); d_faults.free();
         hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free();
-        h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free();
+        h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free(); h_seg.free();
         h_faults.free(); h_faultWord.free();
         d_doneReasons.free(); h_doneReasons.free();
         d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
@@ -1209,6 +1220,20 @@ int mv_set_option(mv_handle h, const char *key, int value) {
             const size_t cnt = size_t(h->N) * h->W * h->H;
             if (h->d_depth.alloc(cnt) != cudaSuccess || h->h_depth.alloc(cnt) != cudaSuccess) { h->setError("depth allocation failed"); return MV_ERR_CUDA; }
             if (!h->depthOut) h->depthOut = h->d_depth.p;
+        }
+        return MV_OK;
+    }
+    if (k == "segmentation") {  // the drawable behind every pixel (see the header); the buffers are allocated here, only when it is on
+        if (h->didReset) { h->setError("option segmentation must be set before the first reset"); return MV_ERR_STATE; }
+        if (value != 0 && value != 1) { h->setError("segmentation must be 0 or 1"); return MV_ERR_ARG; }
+        h->wantSeg = value != 0;
+        if (h->wantSeg && !h->d_seg.p) {
+            const size_t cnt = size_t(h->N) * h->W * h->H;
+            if (h->d_seg.alloc(cnt) != cudaSuccess || h->h_seg.alloc(cnt) != cudaSuccess) {
+                h->d_seg.free(); h->h_seg.free(); h->wantSeg = false;
+                h->setError("segmentation allocation failed");
+                return MV_ERR_CUDA;
+            }
         }
         return MV_OK;
     }
@@ -1599,6 +1624,7 @@ int mv_fetch_obs(mv_handle h) {
     if (h->deviceObsFresh) {
         if (cudaMemcpyAsync(h->h_obs.p, h->obsOut, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("obs download failed"); return MV_ERR_CUDA; }
         if (h->wantDepth && cudaMemcpyAsync(h->h_depth.p, h->depthOut, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("depth download failed"); return MV_ERR_CUDA; }
+        if (h->wantSeg && cudaMemcpyAsync(h->h_seg.p, h->d_seg.p, px * sizeof(uint16_t), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("segmentation download failed"); return MV_ERR_CUDA; }
     }
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
     return MV_OK;
@@ -1631,6 +1657,12 @@ int mv_sync(mv_handle h) {
 
 int mv_obs_host(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_obs.p; return MV_OK; }
 int mv_depth_host(mv_handle h, const float **out) { if (!h || !out || !h->wantDepth) return MV_ERR_ARG; *out = h->h_depth.p; return MV_OK; }
+int mv_segmentation_host(mv_handle h, const uint16_t **out) {
+    if (!h || !out) return MV_ERR_ARG;
+    if (!h->wantSeg) { h->setError("mv_segmentation_host: option segmentation is off"); return MV_ERR_ARG; }
+    *out = h->h_seg.p;
+    return MV_OK;
+}
 int mv_rewards(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_rewards.p; return MV_OK; }
 int mv_dones(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_dones.p; return MV_OK; }
 int mv_true_objectives(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_trueObj.p; return MV_OK; }
@@ -1685,6 +1717,13 @@ int mv_depth_device(mv_handle h, float **p) {
     if (!h || !p || !h->wantDepth) return MV_ERR_ARG;
     if (h->didReset && !h->deviceObsFresh) { h->setError("the last step delivered its frames to the host buffer only (zero-copy): the HBM tensor is stale"); return MV_ERR_STATE; }
     *p = h->depthOut;
+    return MV_OK;
+}
+int mv_segmentation_device(mv_handle h, uint16_t **p) {
+    if (!h || !p) return MV_ERR_ARG;
+    if (!h->wantSeg) { h->setError("mv_segmentation_device: option segmentation is off"); return MV_ERR_ARG; }
+    if (h->didReset && !h->deviceObsFresh) { h->setError("the last step delivered its frames to the host buffer only (zero-copy): the HBM tensor is stale"); return MV_ERR_STATE; }
+    *p = h->d_seg.p;
     return MV_OK;
 }
 int mv_rewards_device(mv_handle h, float **p) { if (!h || !p) return MV_ERR_ARG; *p = h->d_rewards.p; return MV_OK; }

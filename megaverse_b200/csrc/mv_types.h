@@ -214,7 +214,7 @@ struct MvInstance {
     float model[16];  // column-major absoluteTransformationMatrix()
     int32_t mesh;     // 0 box, 1 capsule, 2 sphere, 3 cone, 4 cylinder (DrawableType, env.hpp:57-67)
     int32_t color;    // palette index
-    int32_t pad[2];
+    int32_t pad[2];   // pad[0]: segmentation tag MV_SEG_* << 8 | index (written by the step kernel, read by the rasteriser); pad[1]: 0
 };
 // instance slots besides the static boxes and decorations: the engine allocates staticCap + MV_DYN_INSTANCES + the scenario's decoration
 // capacity per env; the rasteriser's draw-order key bounds the total at MV_HARD_MAX_INSTANCES

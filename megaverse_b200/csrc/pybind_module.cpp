@@ -156,6 +156,13 @@ public:
         check(mv_final_obs_host(h__, &o));
         return py::array_t<uint8_t>({int(masks_.size()), h_, w_, 4}, o, py::none{});
     }
+    // (extension) option "segmentation": uint16 [N,h,w], MV_SEG_* class << 8 | index of the drawable behind each pixel, 0 where nothing was drawn
+    py::array_t<uint16_t> getSegmentation() {
+        alive();
+        const uint16_t *o;
+        check(mv_segmentation_host(h__, &o));
+        return py::array_t<uint16_t>({int(masks_.size()), h_, w_}, o, py::none{});
+    }
     py::array_t<float> getTrueObjectives() {
         alive();
         const float *t;
@@ -279,6 +286,7 @@ PYBIND11_MODULE(megaverse, m) {
         .def("get_true_objectives", &MegaverseGym::getTrueObjectives)
         .def("get_done_reasons", &MegaverseGym::getDoneReasons, "uint8[num_envs] why each episode ended at the last step: 0 not done, 1 time limit, 2 solved, 3 requested")
         .def("get_final_observations", &MegaverseGym::getFinalObservations, "uint8[N,h,w,4] terminal frames (option final_obs): the frame each env's last episode ended on")
+        .def("get_segmentation", &MegaverseGym::getSegmentation, "uint16[N,h,w] segmentation (option segmentation): class << 8 | index of the drawable behind each pixel, 0 where nothing was drawn")
         .def("obs_device_ptr", &MegaverseGym::obsDevicePtr)
         .def("faults", &MegaverseGym::faults)
         .def("fault_word", &MegaverseGym::faultWord)

@@ -44,7 +44,8 @@ struct __align__(16) TriCover {  // what the coverage / depth loop reads (broadc
     float invArea;
     uint32_t key;       // draw order + 1 (later wins depth ties: LESS_OR_EQUAL)
     int32_t flags;      // bits 0..2: edge e is top-left (no bias was applied); bit 3: every edge function fits int32 in the viewport;
-                        // bit 4: the three vertex normals are identical (box faces, cone and cylinder caps)
+                        // bit 4: the three vertex normals are identical (box faces, cone and cylinder caps); bits 16..31: the
+                        // instance's segmentation tag (MvInstance::pad[0])
     uint32_t bx, by;    // pixel box, inclusive: x0 | x1 << 16, y0 | y1 << 16
 };
 struct __align__(16) TriShade {  // what deferred shading reads for the winning fragment
@@ -68,7 +69,8 @@ constexpr int kWarps = kThreads / 32;
 #endif
 constexpr int kInstChunk = MV_VIEW_INST_CHUNK;   // instances per TMA chunk (one thread each in the instance pass)
 static_assert(kInstChunk <= kThreads && kInstChunk <= 128, "one thread per instance of a chunk; slow-list entries keep 7 bits of it");
-constexpr int kXfWords = 23;      // per instance: model-view (12: three rows of each column), normal matrix (9), colour, mesh | face mask << 8
+constexpr int kXfWords = 23;      // per instance: model-view (12: three rows of each column), normal matrix (9), colour | segmentation tag << 16,
+                                  // mesh | face mask << 8
 constexpr int kClipVerts = 6;     // a triangle clipped by two planes has at most 5 vertices
 constexpr int kSmallList = 128;   // small triangles of a tile collected before they are evaluated (32 at a time, one lane each)
 #ifndef MV_SMALL_AREA
@@ -96,6 +98,7 @@ struct ViewParams {
     int instStride;
     uint8_t *obs;                // [N][H][W][4]
     float *depth;                // [N][H][W] or nullptr
+    uint16_t *seg;               // [N][H][W] segmentation tag of each pixel's winner (0: nothing drawn) or nullptr
     uint32_t *workCounter;       // persistent work queue: claim = atomicAdd(counter, 1) - counterBase (never reset: the host advances the base)
     uint32_t counterBase;
     const uint32_t *ready;       // [E] step-kernel completion stamps (nullptr: plain stream order)
@@ -263,7 +266,8 @@ __device__ __forceinline__ bool triBox(const SetupCtx &cx, const ScreenVert &a, 
 // edge / plane set-up of one visible triangle into list slot `slot`
 template <bool FAST>
 __device__ __forceinline__ void writeTri(const SetupCtx &cx, int slot, const ClipVert &va, const ClipVert &vb, const ClipVert &vc, const ScreenVert &a,
-                                         const ScreenVert &b, const ScreenVert &c, const TriBox &tb, int color, uint32_t key) {
+                                         const ScreenVert &b, const ScreenVert &c, const TriBox &tb, int colorTag, uint32_t key) {
+    const int color = colorTag & 0xffff;  // palette index | segmentation tag << 16
     TriCover cv;
     TriShade s;
     const int32_t sxs[3] = {a.sx, b.sx, c.sx}, sys[3] = {a.sy, b.sy, c.sy};
@@ -293,7 +297,7 @@ __device__ __forceinline__ void writeTri(const SetupCtx &cx, int slot, const Cli
     }
     cv.invArea = 1.0f / float(-tb.area2);
     cv.key = key;
-    cv.flags = tl | (worst < (1ll << 30) ? 8 : 0) | (flat ? 16 : 0);
+    cv.flags = tl | (worst < (1ll << 30) ? 8 : 0) | (flat ? 16 : 0) | (colorTag & int(0xffff0000u));
     cv.bx = tb.bx;
     cv.by = tb.by;
     s.diffuse[0] = c_palette[color][0]; s.diffuse[1] = c_palette[color][1]; s.diffuse[2] = c_palette[color][2];
@@ -579,7 +583,9 @@ __device__ __forceinline__ unsigned long long packFrag(float z, uint32_t key, in
 #endif
 extern __shared__ __align__(128) unsigned char g_viewSmem[];  // the CTA's dynamic shared memory (carved up by smemLayout)
 
-template <bool FAST>
+// SEG: the launch writes segmentation (P.seg); a template parameter so that the launches without it keep the tile pass as it was
+// (register pressure at the 128-register cap: a run-time test on P.seg made launches without it 1-2 % slower, H100 80GB HBM3 at 700 W)
+template <bool FAST, bool SEG>
 __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned long long *spill, int view, int rowLo, int bandTiles, int batch, bool final) {
     // addresses derived from the shared-memory symbol itself, so that this out-of-line function keeps shared-space loads and atomics
     const SmemLayout L = smemLayout(P.triCap);
@@ -781,6 +787,22 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
             *reinterpret_cast<ulonglong2 *>(sp) = make_ulonglong2(f4[0], f4[1]);
             *reinterpret_cast<ulonglong2 *>(sp + 2) = make_ulonglong2(f4[2], f4[3]);
         }
+        // segmentation: the fresh winners' tags, read back from their list records after everything else is stored (nothing extra stays
+        // live across the shading loop).  The colour's rules: batch 0 writes every pixel (0 where nothing was drawn), later batches the
+        // pixels they win
+        if (SEG && (batch == 0 || fr0 || fr1 || fr2 || fr3)) {
+            uint16_t *segPix = P.seg + (size_t(view) * P.H + size_t(py)) * P.W + px;
+            uint2 sg = batch == 0 ? make_uint2(0u, 0u) : *reinterpret_cast<const uint2 *>(segPix);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint32_t ti = uint32_t(winners >> (16 * k)) & 0xffffu;
+                if (ti == 0xffffu) continue;  // background of batch 0, or a pixel an earlier batch won
+                const uint32_t g = uint32_t(cover[ti].flags) >> 16;
+                uint32_t &word = k < 2 ? sg.x : sg.y;
+                word = (k & 1) ? ((word & 0xffffu) | (g << 16)) : ((word & 0xffff0000u) | g);
+            }
+            *reinterpret_cast<uint2 *>(segPix) = sg;
+        }
         __syncwarp();  // the warp's fragment buffer is cleared by the next tile
     }
 }
@@ -811,7 +833,8 @@ template <bool MASKED> __device__ __forceinline__ uint32_t claimWork(const ViewP
 #define MV_VIEW_BOUNDS __launch_bounds__(kThreads, MV_VIEW_MIN_CTAS)
 #endif
 // MASKED: a terminal-frame launch (option "final_obs") that draws only the views of the envs P.envMask names
-template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
+// SEG: P.seg is set (option "segmentation"); never with MASKED
+template <bool FAST, bool MASKED = false, bool SEG = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
     unsigned char *smem = g_viewSmem;
     const SmemLayout L = smemLayout(P.triCap);
     MvInstance *stage = reinterpret_cast<MvInstance *>(smem + L.stage);
@@ -972,7 +995,7 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
                             for (int row = 0; row < 3; ++row) xf[(col * 3 + row) * kInstChunk + tid] = mv.c[col * 4 + row];
 #pragma unroll
                         for (int q = 0; q < 9; ++q) xf[(12 + q) * kInstChunk + tid] = nm[q];
-                        xf[21 * kInstChunk + tid] = __int_as_float(color);
+                        xf[21 * kInstChunk + tid] = __int_as_float(color | (__float_as_int(c4.z) << 16));  // pad[0]: the segmentation tag
                     }
                 }
                 xf[22 * kInstChunk + tid] = __int_as_float(meta);
@@ -1145,7 +1168,7 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
                     }
                     if (!__syncthreads_or((pending || slowFull) ? 1 : 0)) break;
                     // the list is full: draw what it holds, then retry what did not fit
-                    tilePass<FAST>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, false);
+                    tilePass<FAST, SEG>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, false);
                     if (P.stats && tid == 0) M.stat[5] += uint32_t(min(M.nTris, M.nValid));
                     ++batch;
                     again = true;
@@ -1194,7 +1217,7 @@ template <bool FAST, bool MASKED = false> __global__ void MV_VIEW_BOUNDS viewKer
             }
             M.claim = nc; M.prefetched = pre;
         }
-        tilePass<FAST>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, true);
+        tilePass<FAST, SEG>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, true);
         __syncthreads();
         if (P.viewCost && tid == 0) P.viewCost[claim] = uint32_t(min((unsigned long long)clock64() - M.itemStart, 0xffffffffull * 16ull) >> 4);
         if (P.stats && tid < 8) {

@@ -22,6 +22,7 @@
 #include "bzset.h"
 #include "dev_math.cuh"
 #include "mv_types.h"
+#include "../../include/megaverse_b200.h"  // MV_SEG_*
 
 namespace mvk {
 using namespace dm;
@@ -765,9 +766,11 @@ __device__ __forceinline__ float tsElem(float tx, float ty, float tz, float sx, 
 // ---------------------------------------------------------------- render inputs (K3): instance list + view matrices
 // Model matrices are the drawables' absoluteTransformationMatrix() (v4r_env_renderer.cpp:52-55), which Magnum evaluates as
 // compose(parent.absoluteTransformation(), transformation()) -- left to right from the scene root (SceneGraph/Object.hpp:114-117).
-__device__ __forceinline__ void putInstance(MvInstance &d, const M4 &m, int mesh, int color) {
+// tag: the drawable's segmentation class and index, MV_SEG_* << 8 | index (the rasteriser's option "segmentation" draws it)
+__device__ __forceinline__ int segTag(int cls, int index) { return cls << 8 | index; }
+__device__ __forceinline__ void putInstance(MvInstance &d, const M4 &m, int mesh, int color, int tag) {
     storeM4(d.model, m);
-    d.mesh = mesh; d.color = color; d.pad[0] = 0; d.pad[1] = 0;
+    d.mesh = mesh; d.color = color; d.pad[0] = tag; d.pad[1] = 0;
 }
 // T(t) * (S(s) * I) built directly: every product in the generic 4x4 chain is x*1 or x*0 and every partial sum adds +0, so
 // this is bit-identical to the multiplied-out matrix (scale and translation components are positive or zero terms)
@@ -785,10 +788,11 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
         for (int i = lane; i < L.n_static; i += 32) {
             const MvBox &b = statics[i];
             if (!(b.flags & MV_OPAQUE)) continue;
-            putInstance(inst[b.flags >> 8], tsMatrix(v3(b.c[0], b.c[1], b.c[2]), v3(b.h[0], b.h[1], b.h[2])), 0, b.color);
+            putInstance(inst[b.flags >> 8], tsMatrix(v3(b.c[0], b.c[1], b.c[2]), v3(b.h[0], b.h[1], b.h[2])), 0, b.color, segTag(MV_SEG_STATIC, 0));
         }
-        for (int i = lane; i < L.n_terrain; i += 32) putInstance(inst[L.slot_terrain + i], loadM4(L.terrain[i].model), 0, L.terrain[i].color);
-        for (int i = lane; i < L.n_deco; i += 32) putInstance(inst[deco[i].slot], loadM4(deco[i].model), deco[i].mesh, deco[i].color);
+        for (int i = lane; i < L.n_terrain; i += 32)  // type is one TerrainType bit
+            putInstance(inst[L.slot_terrain + i], loadM4(L.terrain[i].model), 0, L.terrain[i].color, segTag(MV_SEG_TERRAIN, __ffs(L.terrain[i].type) - 1));
+        for (int i = lane; i < L.n_deco; i += 32) putInstance(inst[deco[i].slot], loadM4(deco[i].model), deco[i].mesh, deco[i].color, segTag(MV_SEG_STATIC, 0));
     }
     const int no = L.n_obj;
     // movable objects: everything at reset, afterwards only what can have moved -- carried objects (they follow their
@@ -803,7 +807,7 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
             const MvAgent &a = S.agents[o.parent];
             m = mul4(mul4(mul4(loadM4(a.object_t), loadM4(a.cam_local)), pickupLocal()), m);  // left to right, as absoluteTransformation()
         }
-        putInstance(inst[MV_OBJ_SLOT(o.meta)], m, MV_OBJ_MESH(o.meta), o.color);
+        putInstance(inst[MV_OBJ_SLOT(o.meta)], m, MV_OBJ_MESH(o.meta), o.color, segTag(MV_SEG_OBJECT, i));
     }
     // per agent: view matrix, eyes, HUD bar, body.  Every chain is associated the way Magnum's absoluteTransformation()
     // recursion does it (SceneGraph/Object.hpp:114-117): from the root, left to right -- ((objT * cam) * ui) * anchor) * bar.
@@ -840,12 +844,12 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
             }
             __syncwarp();
             if (half == 1) inst[L.slot_bars + i].model[e] = mul4Elem(T[2], T[4], e);  // r4
-            if (lane >= 16 && lane < 28) {  // mesh / colour / padding words of the three instances
+            if (lane >= 16 && lane < 28) {  // mesh / colour / segmentation tag / padding words of the three instances
                 const int which = (lane - 16) >> 2, w = (lane - 16) & 3;
                 const int agentColors[7] = {0, 1, 3, 7, 14, 10, 12};  // const.hpp:85 as palette indices
                 MvInstance &d = inst[(which == 0 ? L.slot_eyes : (which == 1 ? L.slot_bars : L.slot_body)) + i];
                 const int mesh = which == 2 ? 1 : 0, color = which == 0 ? 6 : (which == 1 ? 3 : agentColors[i % 7]);  // AGENT_EYES = DARK_NAVY, bar BLUE
-                if (w == 0) d.mesh = mesh; else if (w == 1) d.color = color; else d.pad[w - 2] = 0;
+                if (w == 0) d.mesh = mesh; else if (w == 1) d.color = color; else d.pad[w - 2] = w == 2 ? segTag(MV_SEG_AGENT, i) : 0;
             }
             __syncwarp();
         }
@@ -861,9 +865,10 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
             root = mul4(translation4(v3(far, far, far)), root);
         }
         const int slot0 = L.reward_slot[i], mesh = L.reward_mesh[i], cnt = L.reward_cnt[i];
-        putInstance(inst[slot0], root, mesh, L.reward_voxel[i][3]);
+        putInstance(inst[slot0], root, mesh, L.reward_voxel[i][3], segTag(MV_SEG_REWARD, i));
         for (int k = 1; k < cnt; ++k)
-            putInstance(inst[slot0 + k], mul4(root, mesh == 3 ? loadM4(L.cone_bottom_local) : loadM4(L.reward_child[i][k - 1])), mesh, L.reward_voxel[i][3]);
+            putInstance(inst[slot0 + k], mul4(root, mesh == 3 ? loadM4(L.cone_bottom_local) : loadM4(L.reward_child[i][k - 1])), mesh, L.reward_voxel[i][3],
+                        segTag(MV_SEG_REWARD, i));
     }
     if (lane == 0) {
         counts[0] = L.mesh_counts[0]; counts[1] = L.mesh_counts[0] + L.mesh_counts[1] + L.mesh_counts[2] + L.mesh_counts[3] + L.mesh_counts[4];

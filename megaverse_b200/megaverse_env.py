@@ -70,12 +70,14 @@ class MegaverseEnv(Env):
     SKIP_UNFIT_LEVELS = False
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
-                 action_repeat=1):
+                 action_repeat=1, segmentation=False):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
         # (extension) action_repeat=k (1..4): every step() runs k physics ticks with the same actions (Interact on the first only) and draws
         # once; an episode end stops the ticks, and the rewards returned are each agent's sum over the ticks run (option "action_repeat")
+        # (extension) segmentation=True: segmentation() gives, per agent, the class and index of the drawable behind every pixel of its
+        # current observation (option "segmentation"); step()'s return values do not change
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -109,6 +111,9 @@ class MegaverseEnv(Env):
         self.final_observation = bool(final_observation)
         if self.final_observation:
             self.env.set_option("final_obs", 1)
+        self.segmentation_enabled = bool(segmentation)
+        if self.segmentation_enabled:
+            self.env.set_option("segmentation", 1)
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
         self.default_shaping_scheme = self.env.get_reward_shaping(0, 0)
@@ -135,6 +140,12 @@ class MegaverseEnv(Env):
         obs = self.env.get_observations()
         chw = np.transpose(obs[:, :, :, :3], (0, 3, 1, 2))
         return [chw[i] for i in range(self.num_agents)]
+
+    def segmentation(self):
+        """(extension, segmentation=True) per-agent uint16 [h, w] views, in the order of observations(): MV_SEG_* class << 8 | index of the
+        drawable behind each pixel of the current frame, 0 where nothing was drawn.  Views of engine memory, valid until the next step."""
+        seg = self.env.get_segmentation()
+        return [seg[i] for i in range(self.num_agents)]
 
     def check_faults(self):
         """raise if the engine latched a fault bit (one pinned-memory read, no device round trip)"""
