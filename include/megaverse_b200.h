@@ -146,8 +146,10 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * "tri_cap" (32..1022, default 368: the largest that leaves two CTAs per SM; triangles one raster CTA keeps in shared memory; a view with more is drawn in several batches,
  * results do not depend on it), "raster_bands" (row bands a view is cut into, one work item of the persistent raster grid each;
  * chosen from the number of views by default, results do not depend on it),
- * "raster_grid" (CTAs of the persistent raster grid, 0 = as many as the GPU holds (default): engines that share one GPU -- one per scenario
- * of a mixed batch -- take a share each so that their grids run side by side instead of queueing behind each other),
+ * "raster_grid" (CTAs of the persistent raster grid, 0 = as many as the GPU holds (default): every raster launch of the engine -- the
+ * step's frames, each slice of the sliced download, terminal frames, mv_draw_hires -- takes at most this many; engines that share one GPU
+ * -- one per scenario of a mixed batch -- take a share each so that their grids run side by side instead of queueing behind each other;
+ * results do not depend on it),
  * "raster_sched" (0/1/2, default 1: launches with more work items than raster CTAs draw the envs in the order of what their views cost in
  * the previous step, most expensive first, and the step kernel steps them in that order; 0 natural order, 2 always; results do not depend
  * on it),

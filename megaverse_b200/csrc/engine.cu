@@ -51,6 +51,13 @@ struct DeviceGuard {
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+// the head of an entry point that takes a handle and touches the device: MV_ERR_ARG for a null handle, MV_ERR_CUDA when the switch to
+// the engine's device fails, else the rest of the body runs on that device
+#define MV_ON_DEVICE(h)                                                                                           \
+    if (!(h)) return MV_ERR_ARG;                                                                                  \
+    DeviceGuard dg__((h)->device);                                                                                \
+    if (!dg__.ok) { (h)->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+
 thread_local std::string g_createError;
 
 #define MV_CUDA(call)                                                                                             \
@@ -153,8 +160,16 @@ struct StateStore {
 
 }  // namespace
 
-struct MvConsts;
-static void fillConstsFor(MvConsts &k, int W, int H);
+static void fillConsts(MvConsts &k, int W, int H);
+
+// the frame part of a raster launch: frame size, row bands of bandRows rows, the per-CTA spill slab (one band of the frame per CTA), the
+// triangle-list capacity and the projection of k; the rest is zero (no stats, no ready stamps, no mask, natural order)
+static mvr::ViewParams frameParams(int W, int H, int bands, int bandRows, unsigned long long *spill, int triCap, const MvConsts &k) {
+    mvr::ViewParams vp = {};
+    vp.W = W; vp.H = H; vp.bands = bands; vp.bandRows = bandRows; vp.spill = spill; vp.spillStride = W * bandRows; vp.triCap = triCap;
+    vp.p00 = k.p00; vp.p11 = k.p11; vp.p22 = k.p22; vp.p32 = k.p32;
+    return vp;
+}
 
 struct mv_engine {
     std::string error;
@@ -191,8 +206,14 @@ struct mv_engine {
     MvConsts consts{};
 
     cudaStream_t stream = nullptr;
+    // kernel times of the last timed call, read by readKernelTimes only.  The call records ev[0] before its first kernel, ev[1] after it
+    // when its raster launch is serialised behind it, evFinal before a terminal-frame launch and ev[2] at the end
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t evFinal = nullptr;
+    enum class Timed { Union, Split, FirstOnly } timedAs = Timed::Union;  // no ev[1] (overlapping kernels), ev[1], no raster launch (a save)
+    bool lastHadFinal = false;
     float lastMs[2] = {0, 0};
+    float lastFinalMs = 0.0f;
     int64_t launches = 0;
 
     // Level slots (option "level_slots" D, 2 or 4): each env has one live slot and D - 1 staged ones that hold its next episodes' levels in
@@ -231,7 +252,7 @@ struct mv_engine {
     size_t costItems() const { return size_t(N) * size_t(H / 4); }
     int rasterGridCap = 0;             // option "raster_grid": upper bound of the raster grid (0: all CTAs the GPU holds) -- for several engines sharing one GPU
     int rasterSched = 1;               // option "raster_sched": 0 natural order, 1 cost-ordered when the launch has several items per CTA, 2 always
-    int rasterGrid = 0, rasterCtasPerSM = 0, spillStride = 0, rasterBands = 1, bandRows = 0;
+    int rasterGrid = 0, rasterCtasPerSM = 0, rasterBands = 1, bandRows = 0;
     size_t rasterSmem = 0;
     // hi-res pass (draw_hires): its own output buffers, allocated on first use
     struct Hires {
@@ -298,10 +319,7 @@ struct mv_engine {
     bool wantFinal = false;
     int actionRepeat = 1;           // option "action_repeat": physics ticks per step call (the step kernel's tick loop), drawn once
     bool finalOnDevice = false;    // the last terminal-frame launch stored into HBM (mv_fetch_obs copies the buffers down)
-    bool lastHadFinal = false;      // the last timed step ran a terminal-frame launch (ev[3] .. ev[2])
-    float lastFinalMs = 0.0f;
     int finalGrid = 0;              // persistent grid of the masked raster variants
-    cudaEvent_t evFinal = nullptr;
     DevBuf<MvInstance> d_termInst;  // [E][instCap]
     DevBuf<int32_t> d_termCounts;   // [E][8]
     DevBuf<float> d_termViews;      // [N][16]
@@ -381,6 +399,23 @@ struct mv_engine {
             std::lock_guard<std::mutex> lk(genMutex);
             pendingUpload.push_back(id);
         }
+    }
+    // (re)allocate the [E][D] level-slot arrays, on the device and pinned: levels, static boxes and their rotations (staticCap per level),
+    // decorations and the three bit planes; and the instance rows, whose pitch staticCap sets as well
+    int allocLevelSlots(const char *what) {
+        const size_t rows = size_t(E) * size_t(levelSlots), cap = size_t(staticCap), deco = size_t(decoCap), words = size_t(gridWords) * 3;
+        d_levels.free(); d_statics.free(); d_staticRot.free(); d_deco.free(); d_solid.free(); d_inst.free();
+        h_levels.free(); h_statics.free(); h_staticRot.free(); h_deco.free(); h_solid.free();
+        levelWords.assign(rows, 0);
+        instCap = MV_DYN_INSTANCES + staticCap + decoCap;
+        if (d_levels.alloc(rows) != cudaSuccess || d_statics.alloc(rows * cap) != cudaSuccess || d_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
+            d_deco.alloc(rows * deco) != cudaSuccess || d_solid.alloc(rows * words) != cudaSuccess || d_inst.alloc(size_t(E) * size_t(instCap)) != cudaSuccess ||
+            h_levels.alloc(rows) != cudaSuccess || h_statics.alloc(rows * cap) != cudaSuccess || h_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
+            h_deco.alloc(rows * deco) != cudaSuccess || h_solid.alloc(rows * words) != cudaSuccess) {
+            setError(std::string(what) + ": allocation failed");
+            return MV_ERR_CUDA;
+        }
+        return MV_OK;
     }
     // more static boxes per level: re-pitch every array that is laid out by staticCap (level statics, instance lists), device and host
     int growStatics(int need) {
@@ -504,52 +539,54 @@ struct mv_engine {
         const size_t smem = sizeof(mvk::WarpShared) * warpsPerBlock;
         mvk::stepKernel<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
+        launches += 1;
         return MV_OK;
     }
-    int launchStep(const int32_t *dActions, bool forceReset, Pending *mirror = nullptr, const uint8_t *dEnds = nullptr) {
-        const mvk::StepParams sp = stepParams(dActions, forceReset, mirror, dEnds);
-        const bool timing = !(mirror && overlap);  // the asynchronous fast path carries no timing events
-        if (timing) MV_CUDA(cudaEventRecord(ev[0], stream));
-        if (const int rck = launchStepKernel(sp)) return rck;
-        if (!overlap) MV_CUDA(cudaEventRecord(ev[1], stream));  // an event between the two kernels would serialise them
-        launches += 1;
-        int rc = launchRaster();
-        if (rc) return rc;
-        lastHadFinal = false;
-        if (wantFinal && !forceReset) {  // after the step's own frames: the terminal frames of the envs that ended (stream order, no stamps)
-            if (timing) MV_CUDA(cudaEventRecord(evFinal, stream));
-            rc = launchFinal(mirror == nullptr);
-            if (rc) return rc;
-            lastHadFinal = timing;
+    // One step (or forced flip) of sp.E envs: the step kernel, the raster launch of every view -- a programmatic dependent of the step
+    // kernel when `dependent` and option overlap are on, else in stream order behind it -- and, unless the step is a forced reset, the
+    // terminal frames of the envs that ended.  Every call but the asynchronous one with option overlap records kernel times.
+    int launchStep(const mvk::StepParams &sp, bool dependent) {
+        const bool async = sp.hostRewards != nullptr;  // mv_step_device: results land in its ring slot, terminal frames in HBM
+        const bool dep = dependent && overlap, timed = !(async && overlap), final = wantFinal && !sp.forceReset;
+        if (timed) MV_CUDA(cudaEventRecord(ev[0], stream));
+        if (const int rc = launchStepKernel(sp)) return rc;
+        if (timed && !dep) MV_CUDA(cudaEventRecord(ev[1], stream));  // an event between the two kernels would serialise them
+        if (const int rc = launchRaster(dep)) return rc;
+        if (final) {  // after the step's own frames: the terminal frames of the envs that ended (stream order, no stamps)
+            if (timed) MV_CUDA(cudaEventRecord(evFinal, stream));
+            if (const int rc = launchFinal(!async)) return rc;
         }
-        if (timing) MV_CUDA(cudaEventRecord(ev[2], stream));
+        return endTimes(dep ? Timed::Union : Timed::Split, timed, final);
+    }
+    // the last event of a call (ev[2], only when `timed`) and what its events bracket, for readKernelTimes
+    int endTimes(Timed kind, bool timed = true, bool hadFinal = false) {
+        if (timed) MV_CUDA(cudaEventRecord(ev[2], stream));
+        timedAs = kind;
+        lastHadFinal = timed && hadFinal;
         return MV_OK;
     }
     // the masked raster launch over the terminal rows: every (view, band) item of an env whose d_dones byte is set, into the final-frame
     // buffers -- pinned host memory (stored through UVA, like the zero-copy obs rows) or HBM
     int launchFinal(bool toHost) {
-        mvr::ViewParams vp = rasterParams();
+        mvr::ViewParams vp = frameParams(W, H, rasterBands, bandRows, d_spill.p, triCap, consts);
         vp.instances = d_termInst.p; vp.instCounts = d_termCounts.p; vp.views = d_termViews.p;
         vp.obs = toHost ? h_finalObs.p : d_finalObs.p; vp.depth = wantDepth ? (toHost ? h_finalDepth.p : d_finalDepth.p) : nullptr;
         vp.viewBase = 0; vp.N = N;
         vp.envMask = d_dones.p;
         finalOnDevice = !toHost;
-        const int grid = std::min(rasterGridCap > 0 ? std::min(finalGrid, rasterGridCap) : finalGrid, N * rasterBands);
-        return launchView(vp, grid, false);
+        return launchView(vp, false);
     }
-    // what every raster launch at the engine's frame size shares (the step's frames and the terminal frames): instance stride, spill
-    // slab, frame and band geometry, projection; the rest is zero (no stats, no ready stamps, no mask, natural order)
-    mvr::ViewParams rasterParams() const {
-        mvr::ViewParams vp = {};
-        vp.instStride = instCap; vp.spill = d_spill.p; vp.spillStride = spillStride;
-        vp.A = A; vp.W = W; vp.H = H; vp.bands = rasterBands; vp.bandRows = bandRows; vp.triCap = triCap;
-        vp.p00 = consts.p00; vp.p11 = consts.p11; vp.p22 = consts.p22; vp.p32 = consts.p32;
-        return vp;
+    // CTAs of a launch: the persistent grid of the kernel variant, at most option raster_grid, at most one per work item
+    int rasterGridFor(const mvr::ViewParams &vp) const {
+        const int full = vp.envMask ? finalGrid : rasterGrid;
+        return std::min(rasterGridCap > 0 ? std::min(full, rasterGridCap) : full, vp.N * vp.bands);
     }
     // One persistent launch over all (view, band) items.  Every CTA makes exactly one failing claim when the queue is empty, so the
     // work counter advances by items + grid per launch and the host keeps the base instead of resetting the counter (no memset node
-    // between the step kernel and its programmatic dependent).
-    int launchView(mvr::ViewParams &vp, int grid, bool dependent) {
+    // between the step kernel and its programmatic dependent).  Every engine launch reads instance lists at the engine's pitch.
+    int launchView(mvr::ViewParams &vp, bool dependent) {
+        const int grid = rasterGridFor(vp);
+        vp.A = A; vp.instStride = instCap;
         vp.workCounter = d_workCounter.p; vp.counterBase = counterBase;
         counterBase += uint32_t(vp.N) * uint32_t(vp.bands) + uint32_t(grid);
         cudaLaunchConfig_t cfg = {};
@@ -575,10 +612,9 @@ struct mv_engine {
         for (int e = 0; e < E; ++e) init[costItems() + size_t(e)] = uint32_t(e);
         return cudaMemcpy(d_viewCost.p, init.data(), sizeof(uint32_t) * init.size(), cudaMemcpyHostToDevice);
     }
-    // dependent = false: a launch that follows no step kernel (the re-render after mv_states_load)
-    int launchRaster(bool dependent = true) {
-        const bool dep = overlap && dependent;
-        mvr::ViewParams vp = rasterParams();
+    // dep: a programmatic dependent launch of the step kernel just enqueued
+    int launchRaster(bool dep) {
+        mvr::ViewParams vp = frameParams(W, H, rasterBands, bandRows, d_spill.p, triCap, consts);
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         // pinned allocations are mapped into the device address space (UVA), so the kernel can store through the host pointer
         vp.obs = rasterToHost ? h_obs.p : obsOut; vp.depth = wantDepth ? (rasterToHost ? h_depth.p : depthOut) : nullptr;
@@ -589,27 +625,31 @@ struct mv_engine {
         deviceObsFresh = !rasterToHost;
         if (sliceCount <= 1) {
             vp.viewBase = 0; vp.N = N;
-            const int grid = std::min(rasterGridCap > 0 ? std::min(rasterGrid, rasterGridCap) : rasterGrid, N * rasterBands);
-            if (rasterSched == 2 || (rasterSched == 1 && N * rasterBands > grid)) {  // more work items than CTAs: their order matters
+            if (rasterSched == 2 || (rasterSched == 1 && N * rasterBands > rasterGridFor(vp))) {  // more work items than CTAs: their order matters
                 vp.viewCost = d_viewCost.p; vp.order = d_viewCost.p + costItems(); vp.exitCounter = d_viewCost.p + costItems() + size_t(E);
             }
-            return launchView(vp, grid, dep);
+            return launchView(vp, dep);
         }
         // sliced download: whole envs per slice; slice s is copied down by the copy engine while slice s+1 is rasterised
-        const size_t px = size_t(W) * H;
         const int perSlice = ((E + sliceCount - 1) / sliceCount) * A;
         for (int base = 0, si = 0; base < N; base += perSlice, ++si) {
             const int cnt = std::min(perSlice, N - base);
             vp.viewBase = base; vp.N = cnt;
-            const int rc = launchView(vp, std::min(rasterGrid, cnt * rasterBands), dep && si == 0);
+            const int rc = launchView(vp, dep && si == 0);
             if (rc) return rc;
             while (int(sliceEv.size()) <= si) { cudaEvent_t e2; MV_CUDA(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming)); sliceEv.push_back(e2); }
             MV_CUDA(cudaEventRecord(sliceEv[size_t(si)], stream));
             MV_CUDA(cudaStreamWaitEvent(copyStream, sliceEv[size_t(si)], 0));
-            MV_CUDA(cudaMemcpyAsync(h_obs.p + size_t(base) * px * 4, obsOut + size_t(base) * px * 4, size_t(cnt) * px * 4, cudaMemcpyDeviceToHost, copyStream));
-            if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p + size_t(base) * px, depthOut + size_t(base) * px, sizeof(float) * size_t(cnt) * px, cudaMemcpyDeviceToHost, copyStream));
-            if (wantSeg) MV_CUDA(cudaMemcpyAsync(h_seg.p + size_t(base) * px, d_seg.p + size_t(base) * px, sizeof(uint16_t) * size_t(cnt) * px, cudaMemcpyDeviceToHost, copyStream));
+            if (const int rcd = downloadViews(base, cnt, copyStream)) return rcd;
         }
+        return MV_OK;
+    }
+    // views [base, base + cnt) of the HBM frames -- obs, and depth and segmentation when they are on -- into the host buffers
+    int downloadViews(int base, int cnt, cudaStream_t s) {
+        const size_t px = size_t(W) * H, off = size_t(base) * px, n = size_t(cnt) * px;
+        MV_CUDA(cudaMemcpyAsync(h_obs.p + off * 4, obsOut + off * 4, n * 4, cudaMemcpyDeviceToHost, s));
+        if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p + off, depthOut + off, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
+        if (wantSeg) MV_CUDA(cudaMemcpyAsync(h_seg.p + off, d_seg.p + off, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost, s));
         return MV_OK;
     }
     // decide how this host-facing launch delivers its frames: zero-copy stores, or into HBM and then one copy (sliceCount 1) or a
@@ -631,15 +671,12 @@ struct mv_engine {
         int rc = drain();
         if (rc) return rc;
         // bands of about a hundred 32x4 tiles each
-        const int tilesX = w / 32, tileRows = hgt / 4;
-        const int rowsPerBand = std::max(1, 96 / tilesX) * 4;
+        const int rowsPerBand = std::max(1, 96 / (w / 32)) * 4;
         const int bands = (hgt + rowsPerBand - 1) / rowsPerBand;
-        const int stride = w * rowsPerBand;
-        (void)tileRows;
         if (hires.W != w || hires.H != hgt) {
             hires.free();
             const size_t px = size_t(N) * w * hgt * 4;
-            if (hires.d_obs.alloc(px) != cudaSuccess || hires.h_obs.alloc(px) != cudaSuccess || hires.spill.alloc(size_t(rasterGrid) * size_t(stride)) != cudaSuccess) {
+            if (hires.d_obs.alloc(px) != cudaSuccess || hires.h_obs.alloc(px) != cudaSuccess || hires.spill.alloc(size_t(rasterGrid) * w * rowsPerBand) != cudaSuccess) {
                 hires.free();
                 setError("hi-res buffers: allocation failed");
                 return MV_ERR_CUDA;
@@ -647,14 +684,12 @@ struct mv_engine {
             hires.W = w; hires.H = hgt;
         }
         MvConsts k;
-        fillConstsFor(k, w, hgt);
-        mvr::ViewParams vp = {};
-        vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p; vp.instStride = instCap;
-        vp.obs = hires.d_obs.p; vp.depth = nullptr; vp.spill = hires.spill.p; vp.spillStride = stride;
-        vp.viewBase = 0; vp.N = N; vp.A = A; vp.W = w; vp.H = hgt; vp.bands = bands; vp.bandRows = rowsPerBand; vp.triCap = triCap;
-        vp.p00 = k.p00; vp.p11 = k.p11; vp.p22 = k.p22; vp.p32 = k.p32;
-        vp.ready = nullptr; vp.readyStamp = 0;
-        rc = launchView(vp, std::min(rasterGrid, N * bands), false);
+        fillConsts(k, w, hgt);
+        mvr::ViewParams vp = frameParams(w, hgt, bands, rowsPerBand, hires.spill.p, triCap, k);
+        vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
+        vp.obs = hires.d_obs.p;
+        vp.viewBase = 0; vp.N = N;
+        rc = launchView(vp, false);
         if (rc) return rc;
         MV_CUDA(cudaMemcpyAsync(hires.h_obs.p, hires.d_obs.p, size_t(N) * w * hgt * 4, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaStreamSynchronize(stream));
@@ -688,9 +723,8 @@ struct mv_engine {
         }
         finalGrid = numSMs * std::max(1, std::min(finalPerSM, rasterCtasPerSM));  // shares d_spill, sized by rasterGrid
         bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
-        spillStride = W * bandRows;
         d_spill.free();
-        if (d_spill.alloc(size_t(rasterGrid) * size_t(spillStride)) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
+        if (d_spill.alloc(size_t(rasterGrid) * W * bandRows) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
         hires.free();  // its spill slab is sized by the grid
         return MV_OK;
     }
@@ -712,13 +746,16 @@ struct mv_engine {
         for (int i = 1; i < levelSlots; ++i) scheduleGen(e, (hostSlot[size_t(e)] + i) % levelSlots, hostEpisode[size_t(e)] + i);
     }
 
-    // per-kernel times exist only when the kernels run back to back (overlap off); with the dependent launch the step and
-    // geometry kernels overlap and only their union is meaningful: {-1, whole step}
+    // per-kernel times exist only when the raster launch runs behind the first kernel (ev[1]); when the step and raster kernels overlap
+    // (the dependent launch) only their union is meaningful: {-1, whole call}
     void readKernelTimes() {
         if (cudaEventQuery(ev[2]) != cudaSuccess) return;
-        if (overlap) { lastMs[0] = -1.0f; cudaEventElapsedTime(&lastMs[1], ev[0], ev[2]); }
-        else { cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], lastHadFinal ? evFinal : ev[2]); }
-        lastFinalMs = 0.0f;
+        lastMs[0] = -1.0f; lastMs[1] = 0.0f; lastFinalMs = 0.0f;
+        switch (timedAs) {
+        case Timed::Union: cudaEventElapsedTime(&lastMs[1], ev[0], ev[2]); break;
+        case Timed::Split: cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], lastHadFinal ? evFinal : ev[2]); break;
+        case Timed::FirstOnly: cudaEventElapsedTime(&lastMs[0], ev[0], ev[2]); break;
+        }
         if (lastHadFinal) cudaEventElapsedTime(&lastFinalMs, evFinal, ev[2]);
     }
 
@@ -728,14 +765,23 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
         if (copyObs && !rasterToHost && sliceCount <= 1) {
-            MV_CUDA(cudaMemcpyAsync(h_obs.p, obsOut, size_t(N) * W * H * 4, cudaMemcpyDeviceToHost, stream));
-            if (wantDepth) MV_CUDA(cudaMemcpyAsync(h_depth.p, depthOut, sizeof(float) * size_t(N) * W * H, cudaMemcpyDeviceToHost, stream));
-            if (wantSeg) MV_CUDA(cudaMemcpyAsync(h_seg.p, d_seg.p, sizeof(uint16_t) * size_t(N) * W * H, cudaMemcpyDeviceToHost, stream));
+            const int rc = downloadViews(0, N, stream);
+            if (rc) return rc;
         }
-        if (!wait) return MV_OK;
+        return wait ? waitHostStep() : MV_OK;
+    }
+    // the end of a host-facing call: its stream and the slice downloads drained, then its kernel times
+    int waitHostStep() {
         MV_CUDA(cudaStreamSynchronize(stream));
         if (sliceCount > 1) MV_CUDA(cudaStreamSynchronize(copyStream));
         readKernelTimes();
+        return MV_OK;
+    }
+    // the reward table, when mv_set_reward_shaping has changed it since the last upload
+    int uploadRtable() {
+        if (!rtableDirty) return MV_OK;
+        MV_CUDA(cudaMemcpyAsync(d_rtable.p, h_rtable.p, sizeof(float) * N * MV_R_COUNT, cudaMemcpyHostToDevice, stream));
+        rtableDirty = false;
         return MV_OK;
     }
 
@@ -789,12 +835,10 @@ struct mv_engine {
         if (rc) return rc;
         rc = retire(slotP);  // only if the ring wrapped without retiring
         if (rc) return rc;
-        if (rtableDirty) {
-            MV_CUDA(cudaMemcpyAsync(d_rtable.p, h_rtable.p, sizeof(float) * N * MV_R_COUNT, cudaMemcpyHostToDevice, stream));
-            rtableDirty = false;
-        }
-        rasterToHost = false; sliceCount = 1;
-        rc = launchStep(dActions, false, &slotP, dEnds);  // rewards / dones / true objectives land in the ring slot straight from the kernel
+        rc = uploadRtable();
+        if (rc) return rc;
+        chooseDelivery(false);
+        rc = launchStep(stepParams(dActions, false, &slotP, dEnds), true);  // rewards / dones / true objectives land in the ring slot straight from the kernel
         if (rc) return rc;
         MV_CUDA(cudaEventRecord(slotP.ev, stream));
         slotP.valid = true;
@@ -810,12 +854,10 @@ struct mv_engine {
         if (rc) return rc;
         rc = flushUploads();
         if (rc) return rc;
-        if (rtableDirty) {
-            MV_CUDA(cudaMemcpyAsync(d_rtable.p, h_rtable.p, sizeof(float) * N * MV_R_COUNT, cudaMemcpyHostToDevice, stream));
-            rtableDirty = false;
-        }
+        rc = uploadRtable();
+        if (rc) return rc;
         chooseDelivery(copyObs);
-        rc = launchStep(dActions, false);
+        rc = launchStep(stepParams(dActions, false, nullptr, nullptr), true);
         if (rc) return rc;
         rc = finishStep(copyObs, !split);
         if (rc) return rc;
@@ -826,9 +868,8 @@ struct mv_engine {
     // second half of a split host-facing step (mv_step_begin / mv_step_end): wait for the copies enqueued by stepCommon(split)
     int stepEnd() {
         if (!hostStepPending) { setError("mv_step_end without mv_step_begin"); return MV_ERR_STATE; }
-        MV_CUDA(cudaStreamSynchronize(stream));
-        if (sliceCount > 1) MV_CUDA(cudaStreamSynchronize(copyStream));
-        readKernelTimes();
+        const int rc = waitHostStep();
+        if (rc) return rc;
         hostStepPending = false;
         std::memset(h_actions.p, 0, sizeof(int32_t) * N);  // env.cpp:140-142: actions are cleared after every step
         afterFlip(h_dones.p);
@@ -869,7 +910,8 @@ struct mv_engine {
         const int rc = drain();
         return rc ? rc : flushUploads();
     }
-    // one copy kernel over all listed rows, ev[0] / ev[1] around it.  toStore: engine row pairs[i].x -> store row pairs[i].y, else back.
+    // one copy kernel over all listed rows.  toStore: engine row pairs[i].x -> store row pairs[i].y; else back, and every view is drawn
+    // again behind the copy
     int copyStateRows(StateStore &st, const int32_t *from, const int32_t *to, int n, bool toStore) {
         if (size_t(n) > h_pairs.n) {
             MV_CUDA(cudaStreamSynchronize(stream));  // the previous upload may still read the pinned pairs
@@ -885,12 +927,22 @@ struct mv_engine {
             const size_t rb = sl[size_t(k)].rowBytes();
             table[k] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
         }
-        lastHadFinal = false;
         MV_CUDA(cudaEventRecord(ev[0], stream));
         MV_CUDA(mvs::copyRows(table, kSlabCount, d_pairs.p, n, stream));
-        MV_CUDA(cudaEventRecord(ev[1], stream));
         launches += 1;
-        return MV_OK;
+        if (toStore) return endTimes(Timed::FirstOnly);
+        MV_CUDA(cudaEventRecord(ev[1], stream));
+        const int rc = launchRaster(false);
+        return rc ? rc : endTimes(Timed::Split);
+    }
+    // a state load or an env restart ends like a host-facing step: `launch` enqueues its kernel with every view drawn again behind it
+    // (the views it did not change yield the same bytes), `whileDrawing` is the host's part, run while the device works, and frames and
+    // results are delivered as a step delivers them
+    template <class Launch, class Host> int redrawAndDeliver(Launch &&launch, Host &&whileDrawing) {
+        chooseDelivery(obsToHost);
+        int rc = launch();
+        if (!rc) rc = whileDrawing();
+        return rc ? rc : finishStep(obsToHost);
     }
     int statesSave(StateStore &st, const int32_t *envs, const int32_t *rows, int n) {
         int rc = quiesce();
@@ -921,22 +973,18 @@ struct mv_engine {
             }
         }
         MV_CUDA(cudaStreamSynchronize(stream));
-        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
-        lastMs[1] = 0.0f;
+        readKernelTimes();
         return MV_OK;
     }
+    // the loaded views then show the frames the saved step returned, and rewards / dones / true objectives read as they did after it
     int statesLoad(StateStore &st, const int32_t *rows, const int32_t *envs, int n) {
-        int rc = quiesce();
+        const int rc = quiesce();
         if (rc) return rc;
-        rc = copyStateRows(st, rows, envs, n, false);
-        if (rc) return rc;
-        // re-render every view (the others yield the same bytes again) and deliver as a step would: the loaded views then show the frames
-        // the saved step returned, and rewards / dones / true objectives read as they did after it
-        chooseDelivery(obsToHost);
-        rc = launchRaster(false);
-        if (rc) return rc;
-        MV_CUDA(cudaEventRecord(ev[2], stream));
-        for (int i = 0; i < n; ++i) {  // host state and mirrors, while the device copies and draws; no episode end: no afterFlip, no generation job
+        return redrawAndDeliver([&] { return copyStateRows(st, rows, envs, n, false); }, [&] { restoreHostRows(st, rows, envs, n); return MV_OK; });
+    }
+    // host state and mirrors; no episode end: no afterFlip, no generation job
+    void restoreHostRows(const StateStore &st, const int32_t *rows, const int32_t *envs, int n) {
+        for (int i = 0; i < n; ++i) {
             const int e = envs[i];
             const StateStore::HostRow &r = st.host[size_t(rows[i])];
             gens[size_t(e)] = *r.gen;
@@ -953,11 +1001,6 @@ struct mv_engine {
             }
             if (!lastAsyncDone.empty()) lastAsyncDone[size_t(e)] = -1000;  // the loaded env's last episode end is not this engine's
         }
-        rc = finishStep(obsToHost);
-        if (rc) return rc;
-        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
-        cudaEventElapsedTime(&lastMs[1], ev[1], ev[2]);
-        return MV_OK;
     }
 
     // ------------------------------------------------------------------ per-env restart (mv_reset_envs)
@@ -980,30 +1023,15 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(d_envList.p, h_envList.p, sizeof(uint32_t) * size_t(n), cudaMemcpyHostToDevice, stream));
         mvk::StepParams sp = stepParams(d_actions.p, true, nullptr, nullptr);
         sp.envOrder = d_envList.p; sp.E = n;
-        lastHadFinal = false;
-        MV_CUDA(cudaEventRecord(ev[0], stream));
-        rc = launchStepKernel(sp);
-        if (rc) return rc;
-        launches += 1;
-        MV_CUDA(cudaEventRecord(ev[1], stream));
-        // every view is drawn again (the others yield the same bytes) and delivered as a step would
-        chooseDelivery(obsToHost);
-        rc = launchRaster(false);
-        if (rc) return rc;
-        MV_CUDA(cudaEventRecord(ev[2], stream));
-        std::vector<uint8_t> flipped(size_t(E), 0);
-        for (int i = 0; i < n; ++i) {
-            flipped[size_t(envs[i])] = 1;
-            if (!lastAsyncDone.empty()) lastAsyncDone[size_t(envs[i])] = -1000;  // a restart is not an asynchronous episode end
-        }
-        afterFlip(flipped.data());  // the levels after next, generated while the device draws
-        rc = flushUploads();
-        if (rc) return rc;
-        rc = finishStep(obsToHost);
-        if (rc) return rc;
-        cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]);
-        cudaEventElapsedTime(&lastMs[1], ev[1], ev[2]);
-        return MV_OK;
+        return redrawAndDeliver([&] { return launchStep(sp, false); }, [&] {
+            std::vector<uint8_t> flipped(size_t(E), 0);
+            for (int i = 0; i < n; ++i) {
+                flipped[size_t(envs[i])] = 1;
+                if (!lastAsyncDone.empty()) lastAsyncDone[size_t(envs[i])] = -1000;  // a restart is not an asynchronous episode end
+            }
+            afterFlip(flipped.data());  // the levels after next, generated while the device draws
+            return flushUploads();
+        });
     }
 
     // test hook (mv_debug_warp_agent): w16 = pos[3], basis[9], hvel[3], vvel -- the head of MvAgent, written in one copy after the
@@ -1057,7 +1085,15 @@ int uploadPalette(mv_engine *h) {
     return MV_OK;
 }
 
-void fillConsts(MvConsts &k, int W, int H) {
+int setKernelAttrs(mv_engine *h) {
+    cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
+    return MV_OK;
+}
+
+}  // namespace
+
+static void fillConsts(MvConsts &k, int W, int H) {
     k.dt = 1.0f / 15.0f;                              // env.hpp:160-161
     mvh::yawBasis(3.5f * k.dt, k.look_left);          // agent.cpp:100-108,128-133
     mvh::yawBasis(-3.5f * k.dt, k.look_right);
@@ -1070,18 +1106,6 @@ void fillConsts(MvConsts &k, int W, int H) {
     k.p22 = farZ / (nearZ - farZ);
     k.p32 = farZ * nearZ / (nearZ - farZ);
 }
-
-}  // namespace
-static void fillConstsFor(MvConsts &k, int W, int H) { fillConsts(k, W, H); }
-namespace {
-
-int setKernelAttrs(mv_engine *h) {
-    cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
-    if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
-    return MV_OK;
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -1151,14 +1175,12 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
         e->setError(ex.what());
         return fail(MV_ERR_ARG);
     }
-    e->levelWords.assign(size_t(e->E) * 2, 0);
     e->genQueue.resize(size_t(e->E));
     e->genBusy.assign(size_t(e->E), 0);
     e->pool.reset(new WorkerPool(e->threads));
     // one pitch for all envs: the largest capacity among the engine's scenarios
     e->gridCells = 0; e->decoCap = 0;
     for (int sc : scs) { e->gridCells = std::max(e->gridCells, mv::gridCapacity(sc)); e->decoCap = std::max(e->decoCap, mv::decoCapacity(sc)); }
-    e->instCap = MV_DYN_INSTANCES + e->staticCap + e->decoCap;
     e->gridWords = e->gridCells / 32;
     fillConsts(e->consts, w, h);
 
@@ -1167,10 +1189,9 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     bool ok = ck(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking), "stream") && ck(cudaStreamCreateWithFlags(&e->copyStream, cudaStreamNonBlocking), "copy stream");
     for (auto &evx : e->ev) ok = ok && ck(cudaEventCreate(&evx), "event");
     ok = ok && ck(cudaEventCreate(&e->evFinal), "event");
-    ok = ok && ck(e->d_levels.alloc(E * 2), "levels") && ck(e->d_statics.alloc(E * 2 * size_t(e->staticCap)), "statics") && ck(e->d_staticRot.alloc(E * 2 * size_t(e->staticCap) * 2), "staticRot") &&
-         ck(e->h_statics.alloc(E * 2 * size_t(e->staticCap)), "h_statics") && ck(e->h_staticRot.alloc(E * 2 * size_t(e->staticCap) * 2), "h_staticRot") && ck(e->d_solid.alloc(E * 2 * 3 * e->gridWords), "solid") && ck(e->d_objGrid.alloc(E * e->gridCells), "objGrid") &&
+    ok = ok && e->allocLevelSlots("level slots") == MV_OK && ck(e->d_objGrid.alloc(E * e->gridCells), "objGrid") &&
          ck(e->d_envs.alloc(E), "envs") && ck(e->d_agents.alloc(N), "agents") && ck(e->d_objects.alloc(E * MV_MAX_OBJECTS), "objects") &&
-         ck(e->d_inst.alloc(E * size_t(e->instCap)), "instances") && ck(e->d_deco.alloc(E * 2 * size_t(e->decoCap)), "deco") && ck(e->h_deco.alloc(E * 2 * size_t(e->decoCap)), "h_deco") && ck(e->d_instCounts.alloc(E * 8), "instCounts") && ck(e->d_views.alloc(N * 16), "views") &&
+         ck(e->d_instCounts.alloc(E * 8), "instCounts") && ck(e->d_views.alloc(N * 16), "views") &&
          ck(e->d_actions.alloc(N), "actions") && ck(e->d_rtable.alloc(N * MV_R_COUNT), "rtable") && ck(e->d_rewards.alloc(N), "rewards") &&
          ck(e->d_dones.alloc(E), "dones") && ck(e->d_doneReasons.alloc(E), "doneReasons") && ck(cudaMemset(e->d_doneReasons.p, 0, E), "doneReasons") &&
          ck(e->d_trueObj.alloc(N), "trueObj") && ck(e->d_obs.alloc(N * px * 4), "obs") && ck(e->d_faults.alloc(E), "faults") &&
@@ -1185,7 +1206,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     e->rasterBands = N <= 320 ? 3 : (N <= 640 ? 2 : 1);
     while (e->rasterBands > 1 && (h / 4) % e->rasterBands) --e->rasterBands;
     if (ok && e->configureRaster() != MV_OK) return fail(MV_ERR_CUDA);
-    ok = ok && ck(e->h_levels.alloc(E * 2), "h_levels") && ck(e->h_solid.alloc(E * 2 * 3 * e->gridWords), "h_solid") && ck(e->h_actions.alloc(N), "h_actions") &&
+    ok = ok && ck(e->h_actions.alloc(N), "h_actions") &&
          ck(e->h_rtable.alloc(N * MV_R_COUNT), "h_rtable") && ck(e->h_rewards.alloc(N), "h_rewards") && ck(e->h_dones.alloc(E), "h_dones") && ck(e->h_doneReasons.alloc(E), "h_doneReasons") &&
          ck(e->h_trueObj.alloc(N), "h_trueObj") && ck(e->h_obs.alloc(N * px * 4), "h_obs") && ck(e->h_faults.alloc(E), "h_faults") && ck(e->h_faultWord.alloc(1), "h_faultWord") &&
          ck(e->h_envList.alloc(E), "h_envList") && ck(e->d_envList.alloc(E), "envList");
@@ -1211,7 +1232,8 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
 }
 
 int mv_set_option(mv_handle h, const char *key, int value) {
-    if (!h || !key) return MV_ERR_ARG;
+    if (!key) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     const std::string k = key;
     if (k == "depth") {
         if (h->didReset) { h->setError("option depth must be set before the first reset"); return MV_ERR_STATE; }
@@ -1251,19 +1273,8 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     if (k == "level_slots") {  // level slots per env (see the header): every [E][D] array is allocated again, on the device and pinned
         if (h->didReset) { h->setError("option level_slots must be set before the first reset"); return MV_ERR_STATE; }
         if (value != 2 && value != 4) { h->setError("level_slots must be 2 or 4"); return MV_ERR_ARG; }
-        const size_t rows = size_t(h->E) * size_t(value), cap = size_t(h->staticCap), deco = size_t(h->decoCap), words = size_t(h->gridWords) * 3;
-        h->d_levels.free(); h->d_statics.free(); h->d_staticRot.free(); h->d_deco.free(); h->d_solid.free();
-        h->h_levels.free(); h->h_statics.free(); h->h_staticRot.free(); h->h_deco.free(); h->h_solid.free();
         h->levelSlots = value;
-        h->levelWords.assign(rows, 0);
-        if (h->d_levels.alloc(rows) != cudaSuccess || h->d_statics.alloc(rows * cap) != cudaSuccess || h->d_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
-            h->d_deco.alloc(rows * deco) != cudaSuccess || h->d_solid.alloc(rows * words) != cudaSuccess || h->h_levels.alloc(rows) != cudaSuccess ||
-            h->h_statics.alloc(rows * cap) != cudaSuccess || h->h_staticRot.alloc(rows * cap * 2) != cudaSuccess || h->h_deco.alloc(rows * deco) != cudaSuccess ||
-            h->h_solid.alloc(rows * words) != cudaSuccess) {
-            h->setError("level_slots: allocation failed");
-            return MV_ERR_CUDA;
-        }
-        return MV_OK;
+        return h->allocLevelSlots("level_slots");
     }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches
         if (value < 32 || value > mvr::kMaxTriCap) { h->setError("tri_cap out of range [32,1022]"); return MV_ERR_ARG; }
@@ -1276,16 +1287,8 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     if (k == "static_cap") {  // initial size of the per-level static-box arrays (they grow on demand; tests start small to exercise that)
         if (h->didReset) { h->setError("option static_cap must be set before the first reset"); return MV_ERR_STATE; }
         if (value < 1 || value > (1 << 20)) return MV_ERR_ARG;
-        const size_t rows = size_t(h->E) * h->levelSlots;
-        h->d_statics.free(); h->d_staticRot.free(); h->h_statics.free(); h->h_staticRot.free(); h->d_inst.free();
         h->staticCap = value;
-        h->instCap = MV_DYN_INSTANCES + h->staticCap + h->decoCap;
-        if (h->d_statics.alloc(rows * value) != cudaSuccess || h->d_staticRot.alloc(rows * value * 2) != cudaSuccess || h->h_statics.alloc(rows * value) != cudaSuccess ||
-            h->h_staticRot.alloc(rows * value * 2) != cudaSuccess || h->d_inst.alloc(size_t(h->E) * size_t(h->instCap)) != cudaSuccess) {
-            h->setError("static_cap: allocation failed");
-            return MV_ERR_CUDA;
-        }
-        return MV_OK;
+        return h->allocLevelSlots("static_cap");
     }
     if (k == "raster_bands") {  // row bands per view (each band is one work item of the persistent raster grid)
         if (value < 1 || value > h->H / 4 || (h->H / 4) % value) { h->setError("raster_bands must divide the number of 4-pixel tile rows"); return MV_ERR_ARG; }
@@ -1347,9 +1350,7 @@ int mv_seed_env(mv_handle h, int env, int seed) {
 }
 
 int mv_reset(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     ensureMirrors(h);
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     if (h->didReset) { const int rcd = h->drain(); if (rcd) return rcd; }
@@ -1378,12 +1379,10 @@ int mv_reset(mv_handle h) {
     }
     int rc = h->flushUploads();
     if (rc) return rc;
-    if (h->rtableDirty) {
-        if (cudaMemcpyAsync(h->d_rtable.p, h->h_rtable.p, sizeof(float) * h->N * MV_R_COUNT, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { h->setError("rtable upload failed"); return MV_ERR_CUDA; }
-        h->rtableDirty = false;
-    }
+    rc = h->uploadRtable();
+    if (rc) return rc;
     h->chooseDelivery(h->obsToHost);
-    rc = h->launchStep(h->d_actions.p, true);
+    rc = h->launchStep(h->stepParams(h->d_actions.p, true, nullptr, nullptr), true);
     if (rc) return rc;
     rc = h->finishStep(h->obsToHost);
     if (rc) return rc;
@@ -1408,9 +1407,7 @@ int mv_set_actions(mv_handle h, const int32_t *masks) {
 }
 
 int mv_step(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     if (!h->didReset) { h->setError("mv_step before mv_reset"); return MV_ERR_STATE; }
     if (h->hostStepPending) { h->setError("mv_step_begin is outstanding: call mv_step_end first"); return MV_ERR_STATE; }
     if (cudaMemcpyAsync(h->d_actions.p, h->h_actions.p, sizeof(int32_t) * h->N, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { h->setError("actions upload failed"); return MV_ERR_CUDA; }
@@ -1421,26 +1418,20 @@ int mv_step(mv_handle h) {
 }
 
 int mv_step_begin(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     if (cudaMemcpyAsync(h->d_actions.p, h->h_actions.p, sizeof(int32_t) * h->N, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { h->setError("actions upload failed"); return MV_ERR_CUDA; }
     return h->stepCommon(h->d_actions.p, h->obsToHost, true);
 }
 
 int mv_step_end(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     return h->stepEnd();
 }
 
 int mv_step_device(mv_handle h, const int32_t *d_masks) { return mv_step_device_ends(h, d_masks, nullptr); }
 
 int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     return h->stepAsync(d_masks ? d_masks : h->d_actions.p, d_ends);
 }
 
@@ -1495,9 +1486,7 @@ int mv_debug_count_unfit_levels(const char *scenario, int num_agents, int env_se
 int mv_levels_skipped(mv_handle h) { return h ? h->levelsSkipped.load() : MV_ERR_ARG; }
 
 int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     const int rc = h->drawHires(w, hgt);
     if (rc) return rc;
     if (out) *out = h->hires.h_obs.p;
@@ -1528,9 +1517,8 @@ static int checkStatePairs(mv_handle h, const StateStore &st, const int32_t *env
 }
 
 int mv_states_create(mv_handle h, int rows, int *store) {
-    if (!h || !store) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    if (!store) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_states_create");
     if (rc) return rc;
     if (rows < 1) { h->setError("mv_states_create: rows must be positive"); return MV_ERR_ARG; }
@@ -1538,9 +1526,7 @@ int mv_states_create(mv_handle h, int rows, int *store) {
 }
 
 int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *rows, int n) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_states_save");
     if (rc) return rc;
     StateStore *st = findStore(h, store, "mv_states_save");
@@ -1551,9 +1537,7 @@ int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *r
 }
 
 int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *envs, int n) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_states_load");
     if (rc) return rc;
     StateStore *st = findStore(h, store, "mv_states_load");
@@ -1575,9 +1559,7 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
 }
 
 int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_reset_envs");
     if (rc) return rc;
     if (n < 0 || (n > 0 && !envs)) { h->setError("mv_reset_envs: bad env array"); return MV_ERR_ARG; }
@@ -1591,9 +1573,7 @@ int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n)
 }
 
 int mv_states_destroy(mv_handle h, int store) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     StateStore *st = findStore(h, store, "mv_states_destroy");
     if (!st) return MV_ERR_ARG;
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
@@ -1609,9 +1589,7 @@ int mv_state_row_bytes(mv_handle h, int64_t *out) {
 }
 
 int mv_fetch_obs(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     const int rc = h->drain();
     if (rc) return rc;
@@ -1622,18 +1600,15 @@ int mv_fetch_obs(mv_handle h) {
     }
     // after a zero-copy host-facing step the host buffer holds the newer frames: no copy
     if (h->deviceObsFresh) {
-        if (cudaMemcpyAsync(h->h_obs.p, h->obsOut, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("obs download failed"); return MV_ERR_CUDA; }
-        if (h->wantDepth && cudaMemcpyAsync(h->h_depth.p, h->depthOut, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("depth download failed"); return MV_ERR_CUDA; }
-        if (h->wantSeg && cudaMemcpyAsync(h->h_seg.p, h->d_seg.p, px * sizeof(uint16_t), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("segmentation download failed"); return MV_ERR_CUDA; }
+        const int rcd = h->downloadViews(0, h->N, h->stream);
+        if (rcd) return rcd;
     }
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
     return MV_OK;
 }
 
 int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) return MV_ERR_CUDA;
+    MV_ON_DEVICE(h)
     cudaStreamSynchronize(h->stream);
     if (enable && !h->d_prof.p) {
         if (h->d_prof.alloc(size_t(h->E) * 16) != cudaSuccess) { h->setError("profile buffer allocation failed"); return MV_ERR_CUDA; }
@@ -1645,9 +1620,7 @@ int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable) {
 }
 
 int mv_sync(mv_handle h) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     const int rc = h->drain();
     if (rc) return rc;
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
@@ -1697,9 +1670,7 @@ int mv_final_depth_device(mv_handle h, float **p) {
     return rc;
 }
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     // the pointer is a launch parameter: steps already enqueued keep writing the previous buffer, the next step writes the new one.  No
     // synchronisation here (a consumer that double-buffers its tensor switches every step); mv_sync before freeing a buffer.
     h->obsOut = d_obs ? d_obs : h->d_obs.p;
@@ -1756,7 +1727,8 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
 }
 
 int mv_faults(mv_handle h, int32_t *out) {
-    if (!h || !out) return MV_ERR_ARG;
+    if (!out) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     if (h->stream) cudaStreamSynchronize(h->stream);
     std::vector<MvEnvState> st(size_t(h->E));
     if (cudaMemcpy(st.data(), h->d_envs.p, sizeof(MvEnvState) * st.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -1768,9 +1740,7 @@ int mv_faults(mv_handle h, int32_t *out) {
 }
 // totals since enable: {work items, instances read, instances with visible items, items, clipped items, triangles, batches, -}
 int mv_debug_raster_stats(mv_handle h, unsigned long long *out16, int enable) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) return MV_ERR_CUDA;
+    MV_ON_DEVICE(h)
     cudaStreamSynchronize(h->stream);
     if (out16 && h->d_rasterStats.p && cudaMemcpy(out16, h->d_rasterStats.p, 128, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (enable && !h->d_rasterStats.p) {
@@ -1797,7 +1767,7 @@ int mv_last_final_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_AR
 
 int mv_close(mv_handle h) {
     if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
+    DeviceGuard dg__(h->device);  // not MV_ON_DEVICE: the engine is freed even when the switch fails
     if (h->stream) cudaStreamSynchronize(h->stream);
     h->freeAll();
     delete h;
@@ -1805,59 +1775,59 @@ int mv_close(mv_handle h) {
 }
 
 // ------------------------------------------------------------------------------------------------ introspection (tests)
-// reward-object voxels; for the hexagonal mazes the free-standing colliders instead (bit patterns of centre, half extents, orientation)
-static void dumpLevelExtras(const MvLevel &L, const MvBox *statics, const float *staticRot, std::vector<int32_t> &o) {
-    const bool hex = L.scenario == MV_SCENARIO_HEX_EXPLORE || L.scenario == MV_SCENARIO_HEX_MEMORY || L.scenario == MV_SCENARIO_EMPTY;
-    o.push_back(hex ? 0 : L.n_reward);
-    for (int i = 0; i < L.n_reward && !hex; ++i) for (int a = 0; a < 3; ++a) o.push_back(L.reward_voxel[i][a]);
-    if (!hex) return;
-    o.push_back(L.n_static);
-    for (int i = 0; i < L.n_static; ++i) {
-        const MvBox &b = statics[i];
-        const float rot[2] = {(b.flags & MV_ROTATED) ? staticRot[i * 2] : 1.0f, (b.flags & MV_ROTATED) ? staticRot[i * 2 + 1] : 0.0f};
-        int32_t w[8];
-        std::memcpy(w, b.c, 12); std::memcpy(w + 3, b.h, 12); std::memcpy(w + 6, rot, 8);
-        for (int k = 0; k < 8; ++k) o.push_back(w[k]);
-    }
-}
-
-int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
-    if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
-    const size_t lid = size_t(env) * h->levelSlots + h->hostSlot[size_t(env)];
-    const MvLevel &L = h->h_levels.p[lid];
-    const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
-    const float *staticRot = h->h_staticRot.p + lid * size_t(h->staticCap) * 2;
+// the mv_debug_get_level layout of level L (with its static boxes and their rotations) for A agents; `spawnBasis` appends the agents'
+// spawn yaw bases as float bits
+static int dumpLevel(const MvLevel &L, const MvBox *statics, const float *staticRot, int A, bool spawnBasis, int32_t *out, int cap) {
     std::vector<int32_t> o;
     o.push_back(L.n_grid_static); o.push_back(L.n_terrain); o.push_back(L.n_obj);
     for (int a = 0; a < 3; ++a) o.push_back(L.bz_min[a]);
     for (int a = 0; a < 3; ++a) o.push_back(L.bz_max[a]);
-    static const uint32_t pal[22] = {0xffdd3c, 0x3bb372, 0x50c878, 0x2eb5d0, 0xadd8e6, 0x3a7fa6, 0x2c3e50, 0xffb400, 0xb3b3b3, 0x555555, 0x222222,
-                                     0xffffff, 0xff0000, 0xffa770, 0xd468ee, 0xffe6e6, 0xffffe6, 0xccffcc, 0xe6ecff, 0xd9d9d9, 0xf2e6ff, 0xffebcc};
     for (int i = 0; i < L.n_grid_static; ++i) {
         const MvBox &b = statics[i];
         // invert centre/half back to inclusive voxel bounds: min = c - h, max = c + h - 1
         const float vs = L.scenario == MV_SCENARIO_SOKOBAN ? 2.0f : 1.0f;  // voxel size of the scenario's grid
         for (int a = 0; a < 3; ++a) o.push_back(int(lroundf((b.c[a] - b.h[a]) / vs)));
         for (int a = 0; a < 3; ++a) o.push_back(int(lroundf((b.c[a] + b.h[a]) / vs)) - 1);
-        o.push_back(b.flags & 255); o.push_back(int(pal[b.color]));
+        o.push_back(b.flags & 255); o.push_back(int(kPaletteRgb[b.color]));
     }
     for (int i = 0; i < L.n_terrain; ++i) {
         o.push_back(L.terrain[i].type);
         for (int a = 0; a < 6; ++a) o.push_back(L.terrain[i].bb[a]);
     }
     for (int i = 0; i < L.n_obj; ++i) for (int a = 0; a < 3; ++a) o.push_back(L.obj_init[i].voxel[a]);
-    for (int i = 0; i < h->A; ++i) for (int a = 0; a < 3; ++a) o.push_back(int(L.init_pos[i][a]));
+    for (int i = 0; i < A; ++i) for (int a = 0; a < 3; ++a) o.push_back(int(L.init_pos[i][a]));
     if (L.scenario != MV_SCENARIO_TOWER) {
         o.push_back(L.n_movable);  // numPlatforms
-        dumpLevelExtras(L, statics, staticRot, o);
+        // reward-object voxels; for the hexagonal mazes the free-standing colliders instead (bit patterns of centre, half extents, orientation)
+        const bool hex = L.scenario == MV_SCENARIO_HEX_EXPLORE || L.scenario == MV_SCENARIO_HEX_MEMORY || L.scenario == MV_SCENARIO_EMPTY;
+        o.push_back(hex ? 0 : L.n_reward);
+        for (int i = 0; i < L.n_reward && !hex; ++i) for (int a = 0; a < 3; ++a) o.push_back(L.reward_voxel[i][a]);
+        if (hex) {
+            o.push_back(L.n_static);
+            for (int i = 0; i < L.n_static; ++i) {
+                const MvBox &b = statics[i];
+                const float rot[2] = {(b.flags & MV_ROTATED) ? staticRot[i * 2] : 1.0f, (b.flags & MV_ROTATED) ? staticRot[i * 2 + 1] : 0.0f};
+                int32_t w[8];
+                std::memcpy(w, b.c, 12); std::memcpy(w + 3, b.h, 12); std::memcpy(w + 6, rot, 8);
+                for (int k = 0; k < 8; ++k) o.push_back(w[k]);
+            }
+        }
     }
+    for (int i = 0; i < A && spawnBasis; ++i) for (int k = 0; k < 9; ++k) { int32_t u; std::memcpy(&u, &L.spawn_basis[i][k], 4); o.push_back(u); }
     if (int(o.size()) > cap) return -int(o.size());
     std::memcpy(out, o.data(), o.size() * sizeof(int32_t));
     return int(o.size());
 }
 
+int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
+    if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
+    const size_t lid = size_t(env) * h->levelSlots + h->hostSlot[size_t(env)];
+    return dumpLevel(h->h_levels.p[lid], h->h_statics.p + lid * size_t(h->staticCap), h->h_staticRot.p + lid * size_t(h->staticCap) * 2, h->A, false, out, cap);
+}
+
 int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     MvEnvState es;
     std::vector<MvAgent> ag(size_t(h->A));
     std::vector<MvObject> ob(MV_MAX_OBJECTS);
@@ -1908,6 +1878,7 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
 
 int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     MvEnvState es;
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -1946,6 +1917,7 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
 
 int mv_debug_get_instances(mv_handle h, int env, float *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     int32_t cnt[8];
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(cnt, h->d_instCounts.p + size_t(env) * 8, 32, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -1961,15 +1933,14 @@ int mv_debug_get_instances(mv_handle h, int env, float *out, int cap) {
 
 int mv_debug_get_view(mv_handle h, int env, int agent, float *out16) {
     if (!h || env < 0 || env >= h->E || agent < 0 || agent >= h->A || !h->didReset) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(out16, h->d_views.p + (size_t(env) * h->A + agent) * 16, 64, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     return MV_OK;
 }
 
 int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]) {
-    if (!h) return MV_ERR_ARG;
-    DeviceGuard dg__(h->device);
-    if (!dg__.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_debug_warp_agent");
     if (rc) return rc;
     if (env < 0 || env >= h->E || agent < 0 || agent >= h->A) { h->setError("mv_debug_warp_agent: env / agent out of range"); return MV_ERR_ARG; }
@@ -2024,11 +1995,9 @@ int mv_debug_render_instances(const float *view16, const float *inst18, int n, i
         cudaMemcpy(dCnt, cnt, 32, cudaMemcpyHostToDevice);
         cudaMemcpy(dView, view16, 64, cudaMemcpyHostToDevice);
         cudaMemset(dCtr, 0, 16);
-        mvr::ViewParams vp = {};
+        mvr::ViewParams vp = frameParams(w, h, bands, bandRows, dSpill, triCap, k);
         vp.instances = dInst; vp.instCounts = dCnt; vp.views = dView; vp.instStride = int(inst.size()); vp.obs = dObs; vp.depth = depth ? dDepth : nullptr;
-        vp.workCounter = dCtr; vp.counterBase = 0; vp.ready = nullptr; vp.readyStamp = 0; vp.spill = dSpill; vp.spillStride = w * bandRows;
-        vp.viewBase = 0; vp.N = 1; vp.A = 1; vp.W = w; vp.H = h; vp.bands = bands; vp.bandRows = bandRows; vp.triCap = triCap;
-        vp.p00 = k.p00; vp.p11 = k.p11; vp.p22 = k.p22; vp.p32 = k.p32;
+        vp.workCounter = dCtr; vp.viewBase = 0; vp.N = 1; vp.A = 1;
         mvr::viewKernel<false><<<bands, mvr::kThreads, smem>>>(vp);
         ok = cudaDeviceSynchronize() == cudaSuccess;
         if (ok) {
@@ -2054,33 +2023,8 @@ int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, 
     try {
         for (int ep = 0; ep <= episode; ++ep) gen.generate(lo, ep, 1 << 30);
     } catch (const std::exception &ex) { g_createError = ex.what(); return MV_ERR_CAPACITY; }  // mv_last_error(NULL) tells why
-    const MvLevel &L = lo.level;
-    std::vector<int32_t> o;
-    o.push_back(L.n_grid_static); o.push_back(L.n_terrain); o.push_back(L.n_obj);
-    for (int a = 0; a < 3; ++a) o.push_back(L.bz_min[a]);
-    for (int a = 0; a < 3; ++a) o.push_back(L.bz_max[a]);
-    for (int i = 0; i < L.n_grid_static; ++i) {
-        const MvBox &b = lo.statics[size_t(i)];
-        const float vs = L.scenario == MV_SCENARIO_SOKOBAN ? 2.0f : 1.0f;  // voxel size of the scenario's grid
-        for (int a = 0; a < 3; ++a) o.push_back(int(lroundf((b.c[a] - b.h[a]) / vs)));
-        for (int a = 0; a < 3; ++a) o.push_back(int(lroundf((b.c[a] + b.h[a]) / vs)) - 1);
-        o.push_back(b.flags & 255); o.push_back(int(kPaletteRgb[b.color]));
-    }
-    for (int i = 0; i < L.n_terrain; ++i) {
-        o.push_back(L.terrain[i].type);
-        for (int a = 0; a < 6; ++a) o.push_back(L.terrain[i].bb[a]);
-    }
-    for (int i = 0; i < L.n_obj; ++i) for (int a = 0; a < 3; ++a) o.push_back(L.obj_init[i].voxel[a]);
-    for (int i = 0; i < num_agents; ++i) for (int a = 0; a < 3; ++a) o.push_back(int(L.init_pos[i][a]));
-    if (L.scenario != MV_SCENARIO_TOWER) {
-        o.push_back(L.n_movable);  // numPlatforms
-        dumpLevelExtras(L, lo.statics.data(), lo.staticRot.data(), o);
-    }
-    // spawn yaw basis bits, so the float side of spawnAgents is pinned too
-    for (int i = 0; i < num_agents; ++i) for (int k = 0; k < 9; ++k) { int32_t u; std::memcpy(&u, &L.spawn_basis[i][k], 4); o.push_back(u); }
-    if (int(o.size()) > cap) return -int(o.size());
-    std::memcpy(out, o.data(), o.size() * sizeof(int32_t));
-    return int(o.size());
+    // with the spawn yaw basis bits, so the float side of spawnAgents is pinned too
+    return dumpLevel(lo.level, lo.statics.data(), lo.staticRot.data(), num_agents, true, out, cap);
 }
 
 int mv_debug_bzset(const int32_t *ops, int nops, int32_t *out_xyz, int cap) {
