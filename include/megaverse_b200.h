@@ -85,6 +85,26 @@ int mv_step(mv_handle h);
  * finished step (mv_reset, mv_step_device, mv_fetch_obs) ends an outstanding begin first; a second begin is MV_ERR_STATE. */
 int mv_step_begin(mv_handle h);
 int mv_step_end(mv_handle h);
+/* Steps with an active set: only the chosen envs advance.  In such a call an INACTIVE env does nothing: it runs no tick (at any
+ * action_repeat), its env, agent, object and grid state, episode clock and step counter, level slots, instance lists and camera views are
+ * unchanged, its action masks and its end request (d_ends) are ignored, and no level is generated or uploaded for it.  It reports reward 0
+ * for each of its agents, done 0 and reason MV_END_NONE, its true objectives unchanged, and no terminal frame.  Its views' rows in every
+ * engine-owned output buffer the call delivers to still hold its current frame: obs, and depth and segmentation when they are on -- the pinned
+ * host buffers for mv_step_envs, HBM for mv_step_device_active, and the copy mv_fetch_obs makes.  An ACTIVE env is stepped exactly as by the
+ * corresponding full call (action repeat, end requests, level slots, terminal frames, depth, segmentation, mixed engines): env e delivers
+ * over any sequence of such calls what env e of an engine with the same seeds and options delivers when it is stepped by mv_step (or
+ * mv_step_device_ends with the same requests) only at the calls where e was active.  The asynchronous call's contract (three calls per
+ * episode with two level slots) counts calls as before: an inactive env cannot end.
+ * The raster launch draws only the active envs' views when its destination already holds every view's current frame: the pinned host
+ * buffers after host-facing calls and the re-renders of mv_reset / mv_reset_envs / mv_states_load, but not after mv_step_device* until
+ * mv_fetch_obs; the engine's own HBM buffers after a call that drew into them.  A caller-owned buffer (mv_set_obs_buffer) always has every
+ * view drawn: the engine cannot vouch for its rows.  Otherwise every view is drawn; only the step is masked.  mv_last_kernel_ms and
+ * mv_kernel_launches read as for the corresponding full call.  mv_step_begin / mv_step_end always step every env.
+ * mv_step_envs: the synchronous, host-facing call, like mv_step, with an EnvPool-style list envs[0..n): the listed envs are active.  Actions
+ * come from mv_set_actions; the entries of unlisted envs are ignored.  n == 0 is a call in which every env is inactive.  MV_ERR_ARG (n < 0, a
+ * null list with n > 0, an env out of range or listed twice) and MV_ERR_STATE (before mv_reset, an outstanding mv_step_begin) change
+ * nothing. */
+int mv_step_envs(mv_handle h, const int32_t *envs, int n);
 
 /* MegaverseGym::getObservation (megaverse.cpp:139-143): uint8[N][h][w][4] RGBA, view index env*A+agent, host memory */
 int mv_obs_host(mv_handle h, const uint8_t **out);
@@ -202,6 +222,9 @@ int mv_step_device(mv_handle h, const int32_t *d_masks);
  * call is ignored: that end stands, with its own reason.  A call's reward is the sum of its ticks before the end.
  * With option "level_slots" 4 every request is honoured, including one in a new episode's first call: the next level is always staged. */
 int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends);
+/* mv_step_device_ends with an active set (see mv_step_envs for what an inactive env does and reports): d_active = uint8[num_envs] in DEVICE
+ * memory, read in the engine stream's order; non-zero means active.  d_active == NULL is mv_step_device_ends: the same kernels and launches. */
+int mv_step_device_active(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends, const uint8_t *d_active);
 /* Restart chosen envs now: envs[i] start a new episode.  seeds == NULL: each continues its own level stream (it takes its pre-staged
  * next level, as at a natural episode end); else env envs[i] is first reseeded with seeds[i] and plays the first level of that stream --
  * it then behaves exactly as env envs[i] of a fresh engine after mv_seed_env and mv_reset (unlike mv_seed_env, a Sokoban env also drops
@@ -218,7 +241,8 @@ int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n)
  * megaverse_env.py:27-39 -- write into slices of ONE contiguous tensor that a consumer or an NCCL gather reads without a staging copy.
  * NULL, NULL restores the engine's own buffers.  The pointer takes effect with the next step; steps already enqueued keep writing the
  * previous buffer (no synchronisation: a consumer that double-buffers its tensor -- e.g. to gather step t over NCCL while step t+1 is
- * drawn -- switches every step); mv_sync before freeing a buffer. */
+ * drawn -- switches every step); mv_sync before freeing a buffer.  Steps with an active set (mv_step_device_active) draw every view into a
+ * caller's buffer. */
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth);
 /* mv_step_device is ASYNCHRONOUS: it returns after enqueueing the step on the engine stream (device tensors are valid in
  * stream order).  mv_sync waits for everything enqueued and publishes the last step's rewards/dones/true objectives to the

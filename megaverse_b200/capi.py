@@ -41,6 +41,8 @@ def lib():
         L.mv_encode_action.argtypes = [vp]
         L.mv_step_device.argtypes = [vp, vp]
         L.mv_step_device_ends.argtypes = [vp, vp, vp]
+        L.mv_step_device_active.argtypes = [vp, vp, vp, vp]
+        L.mv_step_envs.argtypes = [vp, vp, ci]
         L.mv_reset_envs.argtypes = [vp, vp, vp, ci]
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
@@ -78,7 +80,7 @@ EXPORTS = [
     "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
-    "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device",
+    "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device", "mv_step_envs", "mv_step_device_active",
 ]
 
 
@@ -153,6 +155,21 @@ class Engine:
             self._ck(lib().mv_step_device(self._h, m))
         else:
             self._ck(lib().mv_step_device_ends(self._h, m, C.c_void_p(d_ends_ptr) if d_ends_ptr else None))
+
+    def step_envs(self, masks, envs):
+        """step() of the listed envs only (mv_step_envs): the others run nothing, report reward 0 and not done, and keep their frames;
+        masks covers every agent, the entries of unlisted envs are ignored"""
+        m = np.ascontiguousarray(masks, dtype=np.int32)
+        assert m.size == self.N
+        e = np.ascontiguousarray(envs, dtype=np.int32)
+        self._ck(lib().mv_set_actions(self._h, m.ctypes.data))
+        self._ck(lib().mv_step_envs(self._h, e.ctypes.data if e.size else None, e.size))
+
+    def step_device_active(self, d_masks_ptr, d_ends_ptr, d_active_ptr):
+        """step_device() of the envs whose byte of the device uint8[E] at d_active_ptr is non-zero (mv_step_device_active); a 0 / None
+        pointer is the engine's own actions, no end requests, every env active"""
+        p = [C.c_void_p(x) if x else None for x in (d_masks_ptr, d_ends_ptr, d_active_ptr)]
+        self._ck(lib().mv_step_device_active(self._h, *p))
 
     def reset_envs(self, envs, seeds=None):
         """envs[i] start a new episode now; with seeds, env envs[i] is reseeded with seeds[i] first (mv_reset_envs)"""

@@ -8,7 +8,7 @@
 //   * extra batched methods (set_actions_batch, get_observations, get_dones, ...) next to the per-agent ones, because the
 //     reference's 2N+E+2 pybind round trips per step (SURVEY.md 3.2) would cap throughput far below the kernels.
 //   * the GIL is released around reset()/step(), around states_save()/states_load() (env state store, not in the reference) and around
-//     reset_envs() (restart chosen envs, not in the reference).
+//     reset_envs() / step_envs() (restart chosen envs, step chosen envs; not in the reference).
 //   * a second constructor takes a list of num_envs scenario names: a mixed-scenario batch in one engine (mv_create_mixed).
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
@@ -101,6 +101,18 @@ public:
             if (rc == MV_OK) rc = mv_step(h__);
         }
         std::fill(masks_.begin(), masks_.end(), 0);  // env.cpp:140-142
+        check(rc);
+    }
+    // (extension) step() of the listed envs only (mv_step_envs): the others run nothing, report reward 0 and not done, and keep their frames
+    void stepEnvs(const std::vector<int32_t> &envs) {
+        alive();
+        int rc;
+        {
+            py::gil_scoped_release nogil;
+            rc = mv_set_actions(h__, masks_.data());
+            if (rc == MV_OK) rc = mv_step_envs(h__, envs.data(), int(envs.size()));
+        }
+        if (rc == MV_OK) std::fill(masks_.begin(), masks_.end(), 0);  // as after step(); a refused call changes nothing
         check(rc);
     }
     bool isDone(int envIdx) {
@@ -296,5 +308,7 @@ PYBIND11_MODULE(megaverse, m) {
         .def("states_save", &MegaverseGym::statesSave)
         .def("states_load", &MegaverseGym::statesLoad)
         .def("states_destroy", &MegaverseGym::statesDestroy)
-        .def("reset_envs", &MegaverseGym::resetEnvs, py::arg("envs"), py::arg("seeds") = py::none());
+        .def("reset_envs", &MegaverseGym::resetEnvs, py::arg("envs"), py::arg("seeds") = py::none())
+        .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),
+             "step the listed envs only: the others run nothing, report reward 0 and done 0, and keep their observations");
 }

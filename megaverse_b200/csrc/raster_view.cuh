@@ -122,7 +122,8 @@ struct ViewParams {
     int bands, bandRows;         // bandRows: multiple of 4; bands * bandRows >= H
     int triCap;                  // triangle list capacity of a CTA (shared memory), <= kMaxTriCap
     float p00, p11, p22, p32;
-    // masked launches only (viewKernel<FAST, true>, natural order, viewBase == 0): [E] the items of an env whose byte is 0 are skipped
+    // masked launches only (Items::Ended and Items::Active): the items of env e of this launch's views (viewBase / A + e) are skipped where
+    // envMask[e] is 0
     const uint8_t *envMask;
 };
 
@@ -808,15 +809,29 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
 }
 
 // ---------------------------------------------------------------------------------------------------- work queue
+// Which items a launch draws: every item, in natural or cost order (All); the items of the envs whose P.envMask byte is set, in natural order
+// (Ended: the terminal frames of the envs that ended); or those of the envs P.envMask names, in cost order when P.viewCost is set (Active: the
+// live frames of a step with an active set).  Ended and Active differ only in the claim, so that the terminal-frame launch keeps its code.
+enum class Items { All, Ended, Active };
+
 // Next work item of the CTA (called by one thread): an index into [0, total), or >= total when the queue is empty.  Natural order: the
 // claim itself; cost-ordered: the view the previous launch's sort put at that position.  Masked: claims of unmasked envs are passed over, so
 // every item is still claimed once and every CTA still ends on exactly one failing claim (the counter advances by items + grid).
-template <bool MASKED> __device__ __forceinline__ uint32_t claimWork(const ViewParams &P, uint32_t total) {
-    if (MASKED) {
+template <Items ITEMS> __device__ __forceinline__ uint32_t claimWork(const ViewParams &P, uint32_t total) {
+    if (ITEMS == Items::Ended) {
         const uint32_t perEnv = uint32_t(P.A) * uint32_t(P.bands);
         uint32_t m = atomicAdd(P.workCounter, 1u) - P.counterBase;
         while (m < total && !P.envMask[m / perEnv]) m = atomicAdd(P.workCounter, 1u) - P.counterBase;
         return m;
+    }
+    if (ITEMS == Items::Active) {  // a passed-over claim costs the atomic and one or two dependent reads, no item work
+        const uint32_t perEnv = uint32_t(P.A) * uint32_t(P.bands);
+        for (;;) {
+            const uint32_t c = atomicAdd(P.workCounter, 1u) - P.counterBase;
+            if (c >= total) return c;
+            const uint32_t e = P.viewCost ? __ldcg(P.order + c / perEnv) : c / perEnv;
+            if (P.envMask[e]) return e * perEnv + c % perEnv;
+        }
     }
     const uint32_t c = atomicAdd(P.workCounter, 1u) - P.counterBase;
     if (P.viewCost && c < total) {
@@ -832,9 +847,9 @@ template <bool MASKED> __device__ __forceinline__ uint32_t claimWork(const ViewP
 #else
 #define MV_VIEW_BOUNDS __launch_bounds__(kThreads, MV_VIEW_MIN_CTAS)
 #endif
-// MASKED: a terminal-frame launch (option "final_obs") that draws only the views of the envs P.envMask names
-// SEG: P.seg is set (option "segmentation"); never with MASKED
-template <bool FAST, bool MASKED = false, bool SEG = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
+// ITEMS: which work items the launch draws (Items: every item, the terminal frames of option "final_obs", or the active envs' live frames)
+// SEG: P.seg is set (option "segmentation"); never with Items::Ended
+template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
     unsigned char *smem = g_viewSmem;
     const SmemLayout L = smemLayout(P.triCap);
     MvInstance *stage = reinterpret_cast<MvInstance *>(smem + L.stage);
@@ -878,7 +893,7 @@ template <bool FAST, bool MASKED = false, bool SEG = false> __global__ void MV_V
     const int tilesX = P.W >> 5;
     unsigned long long *spill = P.spill + size_t(blockIdx.x) * size_t(P.spillStride);
 
-    if (tid == 0) { M.claim = claimWork<MASKED>(P, total); M.prefetched = 0; }
+    if (tid == 0) { M.claim = claimWork<ITEMS>(P, total); M.prefetched = 0; }
     for (;;) {
         const long long tc0 = P.stats ? clock64() : 0;
         long long tcWait = 0, tcInst = 0, tcItem = 0;
@@ -1185,7 +1200,7 @@ template <bool FAST, bool MASKED = false, bool SEG = false> __global__ void MV_V
         // instance chunk while this item's tiles are drawn (the stage buffers, M.view and M.counts are idle during the tile pass): the
         // global round trips of the item head then cost nothing.  One thread; its warp joins the tile pass a little later.
         if (tid == 0) {
-            const uint32_t nc = claimWork<MASKED>(P, total);
+            const uint32_t nc = claimWork<ITEMS>(P, total);
             int pre = 0;
             if (nc < total) {
                 const int nview = P.viewBase + int(nc / uint32_t(bands)), nenv = nview / P.A;

@@ -70,6 +70,7 @@ struct StepParams {
     uint32_t readyStamp;
     const uint32_t *envOrder;  // optional [E]: warp w of the grid steps env envOrder[w] (the order in which the rasteriser will ask for the envs)
     const uint8_t *ends;         // optional [num_envs] (mv_step_device_ends): ends[env] != 0 ends the episode after this call's last tick (with 2 slots: once it has run >= 3 * repeat ticks)
+    const uint8_t *active;       // optional [num_envs] (mv_step_envs, mv_step_device_active): an env whose byte is 0 runs nothing this call
     int repeat;                  // option "action_repeat": physics ticks per call (1..4), the episode stops them early
     int slots;                   // option "level_slots": level slots per env (2 or 4), one live and the rest staged in episode order
     int maxObj;                  // upper bound of n_obj over the live and staged levels (sizes the staging copy)
@@ -886,6 +887,25 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     asm volatile("griddepcontrol.launch_dependents;");
     if (slotInGrid >= P.E) return;
     const int env = P.envOrder ? int(__ldg(P.envOrder + slotInGrid)) : slotInGrid;
+    if (P.active && !P.active[env]) {
+        // an inactive env: no staging, no tick, no write to its state.  It reports reward 0, not done and its unchanged true objective -- the
+        // host mirror too, since a ring slot may still hold a value from three calls earlier -- and publishes its stamp for the raster launch
+        for (int i = lane; i < P.A; i += 32) {
+            const size_t idx = size_t(env) * P.A + i;
+            P.rewards[idx] = 0.0f;
+            if (P.hostRewards) { P.hostRewards[idx] = 0.0f; P.hostTrueObjectives[idx] = P.trueObjectives[idx]; }
+        }
+        __syncwarp();
+        if (lane == 0) {
+            P.dones[env] = 0;
+            P.doneReasons[env] = MV_END_NONE;
+            if (P.hostDones) P.hostDones[env] = 0;
+            if (P.hostDoneReasons) P.hostDoneReasons[env] = MV_END_NONE;
+            __threadfence();
+            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
+        }
+        return;
+    }
     WarpShared &S = reinterpret_cast<WarpShared *>(smemRaw)[warpInBlock];
     const int A = P.A;
     const float dt = P.k.dt;

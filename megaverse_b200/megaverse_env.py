@@ -163,7 +163,18 @@ class MegaverseEnv(Env):
         self.env.set_actions_batch(np.asarray(actions, dtype=np.int32).reshape(self.num_agents, 6))
         self.env.step()
         self.check_faults()
+        return self._step_results()
 
+    def step_envs(self, envs, actions):
+        """(extension) step only the envs listed in `envs` (EnvPool's step(actions, env_id)); the others run nothing and keep their state.
+        `actions` covers every agent, as in step(), and the entries of unlisted envs are ignored.  Returns step()'s 4-tuple for every agent:
+        the agents of unlisted envs get reward 0, done False, {} and their unchanged observation."""
+        self.env.set_actions_batch(np.asarray(actions, dtype=np.int32).reshape(self.num_agents, 6))
+        self.env.step_envs([int(e) for e in envs])
+        self.check_faults()
+        return self._step_results()
+
+    def _step_results(self):
         env_dones = self.env.get_dones()
         if self.final_observation:
             reasons = self.env.get_done_reasons()
