@@ -200,7 +200,9 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * levels of 33 248 B, their static boxes (32 B each, static_cap of them) and rotations (8 B each), decorations (80 B each) and three
  * bit planes of the dense grid -- 374 KiB per Collect env (392 MB at 1 024 envs), 139 KiB per TowerBuilding env, 509 KiB per env of a
  * batch with an Obstacles env, plus 240 KiB per env for the hex mazes' decorations; state-store rows grow by the same.  The first
- * mv_reset generates three levels per env instead of one),
+ * mv_reset generates three levels per env instead of one.  Ignored with option "level_set": nothing is staged),
+ * "level_set" (L >= 0, before the first reset (MV_ERR_STATE after it), default 0 = off) and "level_set_seed" (s, default 0): train or
+ * evaluate on a fixed set of levels, see "Level sets" below,
  * "overlap" (0/1, default 1: the raster kernel is a programmatic dependent launch of the step kernel and synchronises per env;
  * 0 serialises the kernels so that mv_last_kernel_ms can time them separately) */
 int mv_set_option(mv_handle h, const char *key, int value);
@@ -268,6 +270,43 @@ int mv_true_objectives_device(mv_handle h, float **d_true_objectives);
 /* the CUDA stream (cudaStream_t) all engine work is ordered on */
 int mv_stream(mv_handle h, void **stream);
 
+/* Level sets, option "level_set" L > 0 with option "level_set_seed" s (Procgen's num_levels / start_level).  The first mv_reset
+ * generates, once, L levels for every distinct scenario name of the engine: level j of a scenario is the first level (episode 0) of a
+ * fresh generator of that scenario seeded s + j with the engine's params -- what mv_debug_generate_level(scenario, A, s + j, 0, params)
+ * dumps.  Generation runs on the worker pool; "skip_unfit_levels" and generation errors behave as for the streams.  The levels stay in
+ * HBM as a bank of immutable rows that the envs share, and every env plays levels of its own scenario's rows only.  At each start of an
+ * episode (a natural end, a requested end, mv_reset, mv_reset_envs) the step kernel chooses the env's next level j:
+ *   1. the env's entry of the next-level array when it is in [0, L): used once, then set back to -1;
+ *   2. else mv_level_set_pick(pick seed of the env, index of the new episode, L), a hash: uniform over the set, no state.
+ * mv_seed, mv_seed_env and the seeds of mv_reset_envs set pick seeds (mv_seed: the value it would seed the env's generator with); they
+ * never regenerate the bank, and the episode counter keeps counting.  Engines with the same options, seeds and actions play the same
+ * level sequences and produce the same bytes.  A second mv_reset keeps the bank and starts every env on its next pick.
+ * The host does nothing at an episode end, so mv_step_device[_ends|_active] takes every episode length at every action_repeat and honours
+ * every end request (as with "level_slots" 4, which is ignored here), and mv_reset_envs waits for no generator.
+ * Everything else is unchanged: frames, rewards, dones and reasons of an episode on level j equal those of a stream engine's episode on
+ * the same level; final_obs, active sets, action repeat, segmentation, depth, mv_set_obs_buffer and mixed engines work as before.
+ * State store: a row holds no level (the bank is the engine's): it carries the env's live row, pick seed and episode counter, so a
+ * loaded or cloned env replays bit for bit, later levels included; mv_state_row_bytes shrinks by the level slabs.  The next-level array is
+ * caller input like the actions and is not saved.
+ * Memory (HBM, and again pinned for the host mirrors): one row per level and scenario, of 33 248 B + 40 B per static box (the capacity
+ * is raised once to the largest level of the bank) + 80 B per decoration slot + three bit planes of the dense grid; DESIGN.md section 3
+ * has the figures.  The per-env slot rings are not allocated.
+ * mv_level_ids: host int32[num_envs], valid like mv_dones: the level each env is on after the last call -- for an env that just ended,
+ *   the level of the NEW episode (the one the returned frame shows).  Inactive envs keep their value.  mv_level_ids_device: the same in
+ *   HBM, written by the step kernel in stream order.
+ * mv_next_levels_device: device int32[num_envs], engine-owned, initially -1 everywhere.  The caller writes it in the order of mv_stream
+ *   (a prioritised-replay sampler's output, say).  The array is input from outside the engine: the kernel bounds every entry before use,
+ *   and a value outside [0, L) is ignored (the engine picks) and left as it is.
+ * mv_set_next_levels: the host form: entry envs[i] = levels[i], uploaded ahead of the next kernel.  MV_ERR_ARG for an env out of range or
+ *   a level outside [0, L); nothing changes then.  Followed by mv_reset_envs(envs) it starts chosen envs on chosen levels now.
+ * mv_level_set_pick: the hash itself (host-only, no handle), so that a caller can predict or verify a sequence.
+ * The four calls with a handle return MV_ERR_STATE while "level_set" is 0. */
+int mv_level_ids(mv_handle h, const int32_t **out);
+int mv_level_ids_device(mv_handle h, int32_t **d_ids);
+int mv_next_levels_device(mv_handle h, int32_t **d_next);
+int mv_set_next_levels(mv_handle h, const int32_t *envs, const int32_t *levels, int n);
+uint32_t mv_level_set_pick(uint32_t pick_seed, int32_t episode, int32_t count);
+
 /* Env state store: save envs mid-episode and rewind or clone them later, on the device.  A store holds `rows` env states; a row is the
  * complete state of one env -- every per-env device array (env, agents, objects, object grid, instance list, views, both level slots,
  * rewards, dones, true objectives, fault bits) and the host state (the env's level generator and RNG, its live slot and episode index,
@@ -289,7 +328,7 @@ int mv_states_create(mv_handle h, int rows, int *store);
 int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *rows, int n);
 int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *envs, int n);
 int mv_states_destroy(mv_handle h, int store);
-/* device bytes one row holds (grows with the static-box arrays, see option "static_cap") */
+/* device bytes one row holds (grows with the static-box arrays, see option "static_cap"; without the level slabs with a level set) */
 int mv_state_row_bytes(mv_handle h, int64_t *out);
 
 /* sticky per-env fault bits ORed over all envs (MV_FAULT_* in mv_types.h); 0 = healthy */

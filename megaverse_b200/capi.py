@@ -47,7 +47,7 @@ def lib():
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
                      "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device",
-                     "mv_segmentation_host", "mv_segmentation_device"):
+                     "mv_segmentation_host", "mv_segmentation_device", "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
         L.mv_get_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(ci)]
         L.mv_set_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci]
@@ -68,6 +68,9 @@ def lib():
         L.mv_states_load.argtypes = [vp, ci, vp, vp, ci]
         L.mv_states_destroy.argtypes = [vp, ci]
         L.mv_state_row_bytes.argtypes = [vp, C.POINTER(C.c_int64)]
+        L.mv_set_next_levels.argtypes = [vp, vp, vp, ci]
+        L.mv_level_set_pick.argtypes = [C.c_uint32, C.c_int32, C.c_int32]
+        L.mv_level_set_pick.restype = C.c_uint32
         _lib = L
     return _lib
 
@@ -81,6 +84,7 @@ EXPORTS = [
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
     "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device", "mv_step_envs", "mv_step_device_active",
+    "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device", "mv_set_next_levels", "mv_level_set_pick",
 ]
 
 
@@ -172,7 +176,8 @@ class Engine:
         self._ck(lib().mv_step_device_active(self._h, *p))
 
     def reset_envs(self, envs, seeds=None):
-        """envs[i] start a new episode now; with seeds, env envs[i] is reseeded with seeds[i] first (mv_reset_envs)"""
+        """envs[i] start a new episode now; with seeds, env envs[i] is reseeded with seeds[i] first (mv_reset_envs).  With option level_set,
+        set_next_levels(envs, levels) before it chooses the levels they start on."""
         e = np.ascontiguousarray(envs, dtype=np.int32)
         s = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.int32)
         assert s is None or s.size == e.size
@@ -199,11 +204,12 @@ class Engine:
         (`torch.as_tensor(eng.device_array("obs"), device="cuda")`, CuPy, Numba): "obs" uint8[N,h,w,4], "depth" float32[N,h,w],
         "rewards" float32[N], "dones" uint8[E], "done_reasons" uint8[E] (MV_END_*), "true_objectives" float32[N], with option final_obs
         "final_obs" uint8[N,h,w,4] / "final_depth" float32[N,h,w] (terminal frames of mv_step_device steps), and with option segmentation
-        "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index).  Valid in the engine stream's order (mv_stream) until mv_close."""
+        "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index), and with option level_set "level_ids" int32[E] (the level each env is on) and
+        "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream).  Valid in the engine stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
                   "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
-                  "segmentation": (px, "<u2")}
+                  "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4")}
         shape, typestr = shapes[what]
         ptr, stream = self.device_ptr(what), self.stream()
 
@@ -244,6 +250,17 @@ class Engine:
     def done_reasons(self):
         """uint8[E] MV_END_* of the last step: 0 not done, 1 time limit, 2 solved, 3 requested"""
         return self._host("mv_done_reasons", (self.E,), np.uint8)
+
+    def level_ids(self):
+        """int32[E] (option level_set): the level of the set each env is on after the last call; for an env that just ended, the new episode's"""
+        return self._host("mv_level_ids", (self.E,), np.int32)
+
+    def set_next_levels(self, envs, levels):
+        """(option level_set) env envs[i] plays level levels[i] of the set in its next episode, once (mv_set_next_levels).  Followed by
+        reset_envs(envs) it starts those envs on those levels now."""
+        e, lv = np.ascontiguousarray(envs, dtype=np.int32), np.ascontiguousarray(levels, dtype=np.int32)
+        assert e.size == lv.size
+        self._ck(lib().mv_set_next_levels(self._h, e.ctypes.data if e.size else None, lv.ctypes.data if lv.size else None, e.size))
 
     def final_obs(self):
         """uint8[N,h,w,4] terminal frames (option final_obs): views of env e hold the frame its last episode ended on"""
@@ -407,6 +424,11 @@ def generate_level(scenario, num_agents, env_seed, episode, params=None):
     if n < 0:
         raise MegaverseError(n, "mv_debug_generate_level failed")
     return out[:n].copy()
+
+
+def level_set_pick(pick_seed, episode, count):
+    """host-only: the level of a set of `count` an env with this pick seed plays in episode `episode` when nobody names one (mv_level_set_pick)"""
+    return int(lib().mv_level_set_pick(int(pick_seed) & 0xFFFFFFFF, int(episode), int(count)))
 
 
 def bzset_order(ops):

@@ -32,6 +32,7 @@
 
 #include "../../include/megaverse_b200.h"
 #include "hostmath.hpp"
+#include "level_set.h"
 #include "levelgen.hpp"
 #include "raster_view.cuh"
 #include "state_copy.h"
@@ -128,7 +129,8 @@ template <typename T> struct PinBuf {
     void free() { if (p) cudaFreeHost(p); p = nullptr; }
 };
 
-// one per-env device array as the state store sees it: `units` rows per env (the slot count for the arrays that hold the level slots) of unitBytes
+// one per-env device array as the state store sees it: `units` rows per env (the slot count for the arrays that hold the level slots, none
+// of them with a level set) of unitBytes
 struct EnvSlab {
     uint8_t *base;
     int units;
@@ -143,7 +145,8 @@ struct StateStore {
     int rows = 0;
     DevBuf<uint8_t> slabs[kSlabCount];  // same order as mv_engine::envSlabs()
     struct HostRow {
-        std::optional<mv::LevelGenerator> gen;  // empty: the row was never saved
+        bool saved = false;
+        std::optional<mv::LevelGenerator> gen;  // the env's level stream; empty with a level set (the bank is the engine's, the pick is in MvEnvState)
         std::string scenario;                   // the saved env's scenario name: only an env of the same name may load the row
         int slot = 0, episode = 0;
         // the host mirrors of every level slot that the debug dumps and the uploads read, one entry per slot (option "level_slots")
@@ -241,6 +244,22 @@ struct mv_engine {
     // Level slots (option "level_slots" D, 2 or 4): each env has one live slot and D - 1 staged ones that hold its next episodes' levels in
     // order; the step kernel moves to the next slot of the ring at an episode end.  Every [E][D] array below is laid out by it.
     int levelSlots = 2;
+    // Level set (option "level_set" L > 0): the level arrays hold a bank instead, L levels per distinct scenario name of the engine, generated
+    // once by the first reset and never written again.  Row bank * L + j is level j of scenario `bank`: episode 0 of a generator of that
+    // scenario seeded levelSetSeed + j.  Envs share the rows: MvEnvState::slot is an env's live row, the step kernel chooses the next one
+    // at an episode end (StepParams::levelSet), and the host does nothing per end.  "level_slots" is unused
+    int levelSet = 0, levelSetSeed = 0;
+    int numBanks = 1;                  // distinct scenario names among the envs
+    std::vector<int> envBank;          // [E] which of them env e runs (in order of first appearance)
+    std::vector<uint32_t> pickSeed;    // [E] the envs' pick seeds as last set by the host (MvEnvState::pad[0] is the live copy)
+    DevBuf<int32_t> d_bankBase, d_levelIds, d_nextLevels;  // [E] each, see StepParams
+    PinBuf<int32_t> h_levelIds;        // [E] level ids of the last retired call, beside h_dones
+    PinBuf<int32_t> h_nextLevels;      // [E] staging of mv_set_next_levels
+    size_t levelRows() const { return levelSet ? size_t(levelSet) * size_t(numBanks) : size_t(E) * size_t(levelSlots); }
+    // the row of the level arrays and their host mirrors that holds what MvEnvState::slot names for env e
+    size_t rowOfSlot(int e, int slot) const { return levelSet ? size_t(slot) : size_t(e) * size_t(levelSlots) + size_t(slot); }
+    // ... and the row of env e's live level as of the last retired call
+    size_t liveRow(int e) const { return levelSet ? size_t(envBank[size_t(e)]) * size_t(levelSet) + size_t(h_levelIds.p[e]) : rowOfSlot(e, hostSlot[size_t(e)]); }
     DevBuf<MvLevel> d_levels;      // [E][D]
     DevBuf<MvBox> d_statics;       // [E][D][staticCap]
     DevBuf<float> d_staticRot;     // [E][D][staticCap][2]
@@ -307,7 +326,7 @@ struct mv_engine {
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
     // mv_step_device pipeline: results of step k are consumed by the host while steps k+1, k+2 already run
-    struct Pending { bool valid = false; uint64_t step = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; };
+    struct Pending { bool valid = false; uint64_t step = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
     std::vector<int64_t> lastAsyncDone;  // [E] asynchronous step index of the env's previous episode end
     bool asyncContractBroken = false;
     Pending ring[3];
@@ -375,17 +394,26 @@ struct mv_engine {
         });
     }
     // worker thread: one level of env e's stream into slot s
-    void generateLevel(int e, int s, int serial) {
+    void generateLevel(int e, int s, int serial) { generateInto(gens[size_t(e)], envScenario[size_t(e)], e * levelSlots + s, serial); }
+    // worker thread: level j of the level set of the scenario env `first` runs, into bank row `row` -- the first level of that env's
+    // generator (scenario, agents, params) as constructed and seeded levelSetSeed + j, which is what mv_debug_generate_level(..., 0) dumps
+    void generateBankLevel(int first, int row, int j) {
+        mv::LevelGenerator gen = gens[size_t(first)];
+        gen.restart((unsigned long)(levelSetSeed + j));
+        generateInto(gen, envScenario[size_t(first)], row, 0);
+    }
+    // worker thread: the next level of `gen` (of MV_SCENARIO_* sc) into row `id` of the level arrays
+    void generateInto(mv::LevelGenerator &gen, int sc, int id, int serial) {
         {
             mv::LevelOut out;
             // the env's own scenario's capacity, not the engine's pitch: a level is accepted exactly as in a single-scenario engine
-            const int cap = mv::gridCapacity(envScenario[size_t(e)]);
+            const int cap = mv::gridCapacity(sc);
             try {
                 if (skipUnfitLevels) {
-                    const int skipped = gens[size_t(e)].generateFitting(out, serial, cap);
+                    const int skipped = gen.generateFitting(out, serial, cap);
                     if (skipped) levelsSkipped.fetch_add(skipped);
                 } else {
-                    gens[size_t(e)].generate(out, serial, cap);
+                    gen.generate(out, serial, cap);
                 }
             } catch (const std::exception &ex) {
                 std::lock_guard<std::mutex> lk(genMutex);
@@ -399,10 +427,10 @@ struct mv_engine {
             if (int(out.statics.size()) > staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
                 std::lock_guard<std::mutex> lk(genMutex);
                 wantStaticCap = std::max(wantStaticCap, int(out.statics.size()));
-                oversize.emplace_back(e * levelSlots + s, std::move(out));
+                oversize.emplace_back(id, std::move(out));
                 return;
             }
-            stageLevel(e * levelSlots + s, out);
+            stageLevel(id, out);
         }
     }
     // worker thread (or flushUploads for parked levels): copy a generated level into the pinned staging mirrors and queue its upload
@@ -424,10 +452,10 @@ struct mv_engine {
             pendingUpload.push_back(id);
         }
     }
-    // (re)allocate the [E][D] level-slot arrays, on the device and pinned: levels, static boxes and their rotations (staticCap per level),
+    // (re)allocate the level arrays ([E][D] slots, or the rows of a level set), on the device and pinned: levels, static boxes and their rotations (staticCap per level),
     // decorations and the three bit planes; and the instance rows, whose pitch staticCap sets as well
     int allocLevelSlots(const char *what) {
-        const size_t rows = size_t(E) * size_t(levelSlots), cap = size_t(staticCap), deco = size_t(decoCap), words = size_t(gridWords) * 3;
+        const size_t rows = levelRows(), cap = size_t(staticCap), deco = size_t(decoCap), words = size_t(gridWords) * 3;
         d_levels.free(); d_statics.free(); d_staticRot.free(); d_deco.free(); d_solid.free(); d_inst.free();
         h_levels.free(); h_statics.free(); h_staticRot.free(); h_deco.free(); h_solid.free();
         levelWords.assign(rows, 0);
@@ -448,12 +476,13 @@ struct mv_engine {
         if (newInstCap > mvr::kMaxInstancesPerEnv) { setError("a level needs more drawables than the draw-order key can number"); return MV_ERR_CAPACITY; }
         MV_CUDA(cudaStreamSynchronize(stream));
         DevBuf<MvBox> nStat; DevBuf<float> nRot; DevBuf<MvInstance> nInst; PinBuf<MvBox> hStat; PinBuf<float> hRot;
-        const size_t rows = size_t(E) * levelSlots;
-        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside
+        const size_t rows = levelRows();
+        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside (with a level set the
+        // only growth is the first reset's, before any store exists)
         struct Repitch { DevBuf<uint8_t> *buf; DevBuf<uint8_t> next; size_t rows, oldPitch, newPitch; };
         std::vector<Repitch> storeGrow;
         for (auto &st : stores) {
-            if (!st) continue;
+            if (!st || levelSet) continue;
             const size_t r = size_t(st->rows);
             storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * levelSlots, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
             storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * levelSlots, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
@@ -550,6 +579,8 @@ struct mv_engine {
         sp.ends = dEnds;
         sp.repeat = actionRepeat;
         sp.slots = levelSlots;
+        sp.levelSet = levelSet; sp.bankBase = d_bankBase.p; sp.nextLevels = d_nextLevels.p; sp.levelIds = d_levelIds.p;
+        sp.hostLevelIds = (mirror && levelSet) ? mirror->levelIds.p : nullptr;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
@@ -562,7 +593,8 @@ struct mv_engine {
         const int warpsPerBlock = 2;
         const int blocks = (sp.E + warpsPerBlock - 1) / warpsPerBlock;
         const size_t smem = sizeof(mvk::WarpShared) * warpsPerBlock;
-        mvk::stepKernel<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        if (sp.levelSet) mvk::stepKernel<true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        else mvk::stepKernel<false><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
         launches += 1;
         return MV_OK;
@@ -762,6 +794,7 @@ struct mv_engine {
         const int D = levelSlots;
         for (int e = 0; e < E; ++e) {
             if (!flipped || flipped[e]) {
+                if (levelSet) { hostEpisode[size_t(e)] += 1; continue; }  // the kernel chose a bank row: nothing to generate, nothing to upload
                 hostSlot[size_t(e)] = (hostSlot[size_t(e)] + 1) % D;
                 hostEpisode[size_t(e)] += 1;
                 scheduleGen(e, (hostSlot[size_t(e)] + D - 1) % D, hostEpisode[size_t(e)] + D - 1);
@@ -770,6 +803,7 @@ struct mv_engine {
     }
     // (re)build env e's staged levels, episodes after the live one in order, from its generator's current state
     void restage(int e) {
+        if (levelSet) return;  // nothing is staged: every level of the set is in the bank
         for (int i = 1; i < levelSlots; ++i) scheduleGen(e, (hostSlot[size_t(e)] + i) % levelSlots, hostEpisode[size_t(e)] + i);
     }
 
@@ -791,6 +825,7 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
+        if (levelSet) MV_CUDA(cudaMemcpyAsync(h_levelIds.p, d_levelIds.p, sizeof(int32_t) * E, cudaMemcpyDeviceToHost, stream));
         if (copyObs && !rasterToHost && sliceCount <= 1) {
             const int rc = downloadViews(0, N, stream);
             if (rc) return rc;
@@ -820,17 +855,19 @@ struct mv_engine {
         std::memcpy(h_dones.p, p.dones.p, E);
         std::memcpy(h_doneReasons.p, p.reasons.p, E);
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
+        if (levelSet) std::memcpy(h_levelIds.p, p.levelIds.p, sizeof(int32_t) * E);
         p.valid = false;
         // with two level slots the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes
         // again sooner flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on.  Counted
         // in calls whatever option "action_repeat" is: retiring, regenerating and uploading happen once per call, so the level pipeline is
         // three calls deep (the kernel's request rule, num_frames >= 3 * repeat ticks, is the same three calls counted on the device).  With
         // four slots an env ends at most once per call, and the level replacing the end of call j is uploaded before kernel j + 3, when the
-        // ends of calls j, j + 1 and j + 2 have used the three staged levels at most: there is nothing to check
+        // ends of calls j, j + 1 and j + 2 have used the three staged levels at most: there is nothing to check.  Nor with a level set,
+        // whose levels never arrive
         if (lastAsyncDone.empty()) lastAsyncDone.assign(size_t(E), -1000);
         for (int e = 0; e < E; ++e)
             if (h_dones.p[e]) {
-                if (levelSlots == 2 && int64_t(p.step) - lastAsyncDone[size_t(e)] < 3) asyncContractBroken = true;
+                if (levelSlots == 2 && !levelSet && int64_t(p.step) - lastAsyncDone[size_t(e)] < 3) asyncContractBroken = true;
                 lastAsyncDone[size_t(e)] = int64_t(p.step);
             }
         afterFlip(h_dones.p);
@@ -917,10 +954,13 @@ struct mv_engine {
     // every per-env device row, in the order of StateStore::slabs
     std::array<EnvSlab, kSlabCount> envSlabs() {
         auto s = [](void *p, int units, size_t bytes) { return EnvSlab{static_cast<uint8_t *>(p), units, bytes}; };
-        const int D = levelSlots;
+        // with a level set a row holds no level: the bank is shared and immutable, MvEnvState names the row.  The levels' place in the
+        // list is taken by the env's level id, so that a loaded env reports its level before it is stepped again
+        const int D = levelSet ? 0 : levelSlots;
+        const EnvSlab levelsOrId = levelSet ? s(d_levelIds.p, 1, sizeof(int32_t)) : s(d_levels.p, D, sizeof(MvLevel));
         return {{s(d_envs.p, 1, sizeof(MvEnvState)), s(d_agents.p, 1, sizeof(MvAgent) * A), s(d_objects.p, 1, sizeof(MvObject) * MV_MAX_OBJECTS),
                  s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instCap), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
-                 s(d_views.p, 1, sizeof(float) * 16 * A), s(d_levels.p, D, sizeof(MvLevel)), s(d_statics.p, D, sizeof(MvBox) * staticCap),
+                 s(d_views.p, 1, sizeof(float) * 16 * A), levelsOrId, s(d_statics.p, D, sizeof(MvBox) * staticCap),
                  s(d_staticRot.p, D, sizeof(float) * 2 * staticCap), s(d_deco.p, D, sizeof(MvDeco) * decoCap), s(d_solid.p, D, sizeof(uint32_t) * 3 * gridWords),
                  s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t)),
                  s(d_doneReasons.p, 1, 1)}};
@@ -989,9 +1029,11 @@ struct mv_engine {
         for (int i = 0; i < n; ++i) {  // host state; the workers are idle (flushUploads waited for them)
             const int e = envs[i];
             StateStore::HostRow &r = st.host[size_t(rows[i])];
-            r.gen = gens[size_t(e)];
+            r.saved = true;
             r.scenario = envScenarioName[size_t(e)];
             r.slot = hostSlot[size_t(e)]; r.episode = hostEpisode[size_t(e)];
+            if (levelSet) continue;  // no generator, no mirrors: the pick seed and the live row travel in MvEnvState
+            r.gen = gens[size_t(e)];
             const size_t D = size_t(levelSlots);
             r.words.resize(D); r.level.resize(D); r.statics.resize(D); r.staticRot.resize(D); r.deco.resize(D); r.solid.resize(D);
             for (size_t s = 0; s < D; ++s) {
@@ -1024,7 +1066,7 @@ struct mv_engine {
         for (int i = 0; i < n; ++i) {
             const int e = envs[i];
             const StateStore::HostRow &r = st.host[size_t(rows[i])];
-            gens[size_t(e)] = *r.gen;
+            if (r.gen) gens[size_t(e)] = *r.gen;
             hostSlot[size_t(e)] = r.slot; hostEpisode[size_t(e)] = r.episode;
             for (size_t s = 0; s < r.level.size(); ++s) {  // the store's slot count is the engine's
                 const size_t id = size_t(e) * size_t(levelSlots) + s;
@@ -1052,6 +1094,8 @@ struct mv_engine {
                 const int e = envs[i];
                 gens[size_t(e)].restart((unsigned long)seeds[i]);
                 restage(e);
+                pickSeed[size_t(e)] = uint32_t(seeds[i]);  // with a level set a seed names a pick sequence, not a stream
+                if ((rc = uploadPickSeeds(e, 1))) return rc;
             }
             rc = flushUploads();
             if (rc) return rc;
@@ -1071,6 +1115,62 @@ struct mv_engine {
         });
     }
 
+    // ------------------------------------------------------------------ level set
+    // pickSeed[first .. first + count) into the envs' MvEnvState (after the first reset, which otherwise writes them itself), in stream
+    // order behind the steps already enqueued
+    int uploadPickSeeds(int first, int count) {
+        if (!levelSet || !didReset) return MV_OK;
+        static_assert(sizeof(MvEnvState::pad[0]) == sizeof(uint32_t), "the pick seed lives in MvEnvState::pad[0]");
+        MV_CUDA(cudaMemcpy2DAsync(&d_envs.p[first].pad[0], sizeof(MvEnvState), &pickSeed[size_t(first)], sizeof(uint32_t), sizeof(uint32_t), size_t(count),
+                                  cudaMemcpyHostToDevice, stream));
+        MV_CUDA(cudaStreamSynchronize(stream));  // pageable source
+        return MV_OK;
+    }
+    // option "level_set": the bank's rows replace the slot rings, and the per-env arrays of the mode appear (or go)
+    int allocLevelSet() {
+        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free();
+        for (auto &p : ring) p.levelIds.free();
+        if (const int rc = allocLevelSlots("level_set")) return rc;
+        if (!levelSet) return MV_OK;
+        const size_t n = size_t(E);
+        bool ok = d_bankBase.alloc(n) == cudaSuccess && d_levelIds.alloc(n) == cudaSuccess && d_nextLevels.alloc(n) == cudaSuccess &&
+                  h_levelIds.alloc(n) == cudaSuccess && h_nextLevels.alloc(n) == cudaSuccess;
+        for (auto &p : ring) ok = ok && p.levelIds.alloc(n) == cudaSuccess;
+        if (!ok) { setError("level_set: allocation failed"); return MV_ERR_CUDA; }
+        std::memset(h_levelIds.p, 0, sizeof(int32_t) * n);
+        for (auto &p : ring) std::memset(p.levelIds.p, 0, sizeof(int32_t) * n);
+        std::vector<int32_t> base(n);
+        for (size_t e = 0; e < n; ++e) base[e] = envBank[e] * levelSet;
+        MV_CUDA(cudaMemcpy(d_bankBase.p, base.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice));
+        MV_CUDA(cudaMemset(d_levelIds.p, 0, sizeof(int32_t) * n));
+        MV_CUDA(cudaMemset(d_nextLevels.p, 0xFF, sizeof(int32_t) * n));  // -1: the engine picks
+        return MV_OK;
+    }
+    // first reset with a level set: every level of the bank, on the worker pool; flushUploads then grows the static-box arrays once, to
+    // the largest level of the bank, and uploads the rows
+    void scheduleBank() {
+        std::vector<int> first(size_t(numBanks), -1);
+        for (int e = E - 1; e >= 0; --e) first[size_t(envBank[size_t(e)])] = e;
+        for (int b = 0; b < numBanks; ++b)
+            for (int j = 0; j < levelSet; ++j) {
+                const int f = first[size_t(b)], row = b * levelSet + j;
+                pool->submit([this, f, row, j] { generateBankLevel(f, row, j); });
+            }
+    }
+    // mv_set_next_levels: the listed entries of the next-level array, in stream order ahead of the next kernel; runs of consecutive envs
+    // go up in one copy
+    int setNextLevels(const int32_t *envs, const int32_t *levels, int n) {
+        MV_CUDA(cudaStreamSynchronize(stream));  // a previous call's copies may still read the staging array
+        for (int i = 0; i < n; ++i) h_nextLevels.p[envs[i]] = levels[i];
+        for (int i = 0; i < n;) {
+            int len = 1;
+            while (i + len < n && envs[i + len] == envs[i] + len) ++len;
+            MV_CUDA(cudaMemcpyAsync(d_nextLevels.p + envs[i], h_nextLevels.p + envs[i], sizeof(int32_t) * size_t(len), cudaMemcpyHostToDevice, stream));
+            i += len;
+        }
+        return MV_OK;
+    }
+
     // test hook (mv_debug_warp_agent): w16 = pos[3], basis[9], hvel[3], vvel -- the head of MvAgent, written in one copy after the
     // asynchronous ring is retired.  Every other position-derived value (colliders, candidate lists, object_t, views) is rebuilt from
     // MvAgent::pos by the next step kernel.
@@ -1087,6 +1187,7 @@ struct mv_engine {
         if (pool) { pool->waitAll(); pool.reset(); }
         for (auto &st : stores) if (st) st->free();
         stores.clear();
+        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free();
         h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free(); h_active.free(); d_active.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
         d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_seg.free(); d_faults.free();
@@ -1097,7 +1198,7 @@ struct mv_engine {
         d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
         for (auto &e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
         if (evFinal) { cudaEventDestroy(evFinal); evFinal = nullptr; }
-        for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); }
+        for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); p.levelIds.free(); }
         for (auto &e2 : sliceEv) if (e2) cudaEventDestroy(e2);
         sliceEv.clear();
         if (copyStream) { cudaStreamDestroy(copyStream); copyStream = nullptr; }
@@ -1123,7 +1224,8 @@ int uploadPalette(mv_engine *h) {
 }
 
 int setKernelAttrs(mv_engine *h) {
-    cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
     if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
     return MV_OK;
 }
@@ -1211,6 +1313,16 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     } catch (const std::exception &ex) {  // e.g. Sokoban without a Boxoban dataset (the reference exit()s here, scenario_sokoban.cpp:76-78)
         e->setError(ex.what());
         return fail(MV_ERR_ARG);
+    }
+    {   // the distinct scenario names, in order of first appearance: a level set keeps one run of bank rows for each
+        std::vector<std::string> distinct;
+        for (const std::string &name : names) {
+            const size_t b = size_t(std::find(distinct.begin(), distinct.end(), name) - distinct.begin());
+            if (b == distinct.size()) distinct.push_back(name);
+            e->envBank.push_back(int(b));
+        }
+        e->numBanks = int(distinct.size());
+        for (int i = 0; i < e->E; ++i) e->pickSeed.push_back(uint32_t(std::uniform_int_distribution<>{0, (1 << 30) - 1}(e->master)));
     }
     e->genQueue.resize(size_t(e->E));
     e->genBusy.assign(size_t(e->E), 0);
@@ -1313,6 +1425,13 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         h->levelSlots = value;
         return h->allocLevelSlots("level_slots");
     }
+    if (k == "level_set" || k == "level_set_seed") {  // a fixed bank of levels instead of the endless streams (see the header)
+        if (h->didReset) { h->setError("option " + k + " must be set before the first reset"); return MV_ERR_STATE; }
+        if (k == "level_set_seed") { h->levelSetSeed = value; return MV_OK; }
+        if (value < 0 || value > (1 << 20)) { h->setError("level_set out of range [0, 1048576]"); return MV_ERR_ARG; }
+        h->levelSet = value;
+        return h->allocLevelSet();
+    }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches
         if (value < 32 || value > mvr::kMaxTriCap) { h->setError("tri_cap out of range [32,1022]"); return MV_ERR_ARG; }
         const int old = h->triCap;
@@ -1370,7 +1489,15 @@ int mv_seed(mv_handle h, int seed) {
     if (!h) return MV_ERR_ARG;
     h->pool->waitAll();
     h->master.seed((unsigned long)seed);
-    for (int e = 0; e < h->E; ++e) h->gens[size_t(e)].seed((unsigned long)std::uniform_int_distribution<>{0, (1 << 30) - 1}(h->master));
+    for (int e = 0; e < h->E; ++e) {  // one draw per env: its generator's seed, and its pick seed in a level set
+        const int s = std::uniform_int_distribution<>{0, (1 << 30) - 1}(h->master);
+        h->gens[size_t(e)].seed((unsigned long)s);
+        h->pickSeed[size_t(e)] = uint32_t(s);
+    }
+    if (h->levelSet && h->didReset) {  // the bank stays; the envs' pick seeds change
+        MV_ON_DEVICE(h)
+        return h->uploadPickSeeds(0, h->E);
+    }
     if (h->didReset) {  // the staged next levels were drawn from the old streams: redo them
         { std::lock_guard<std::mutex> lk(h->genMutex); h->pendingUpload.clear(); }
         regenerateNext(h);
@@ -1382,6 +1509,11 @@ int mv_seed_env(mv_handle h, int env, int seed) {
     if (!h || env < 0 || env >= h->E) return MV_ERR_ARG;
     h->pool->waitAll();
     h->gens[size_t(env)].seed((unsigned long)seed);
+    h->pickSeed[size_t(env)] = uint32_t(seed);
+    if (h->levelSet && h->didReset) {
+        MV_ON_DEVICE(h)
+        if (const int rc = h->uploadPickSeeds(env, 1)) return rc;
+    }
     if (h->didReset) h->restage(env);  // every staged level, from the new stream in order
     return MV_OK;
 }
@@ -1397,6 +1529,8 @@ int mv_reset(mv_handle h) {
         std::vector<MvEnvState> init(size_t(h->E));
         std::memset(init.data(), 0, sizeof(MvEnvState) * init.size());
         for (auto &s : init) { s.slot = h->levelSlots - 1; s.episode_idx = -1; mvBzInit(s); }
+        // level set: any row of the bank to start from, and the pick seed with which the forced flip chooses episode 0's row
+        for (int e = 0; e < h->E && h->levelSet; ++e) { init[size_t(e)].slot = 0; init[size_t(e)].pad[0] = int32_t(h->pickSeed[size_t(e)]); }
         if (cudaMemcpy(h->d_envs.p, init.data(), sizeof(MvEnvState) * init.size(), cudaMemcpyHostToDevice) != cudaSuccess) { h->setError("env init upload failed"); return MV_ERR_CUDA; }
         if (h->wantFinal) {
             const size_t E = size_t(h->E), N = size_t(h->N), px = size_t(h->W) * h->H;
@@ -1411,7 +1545,8 @@ int mv_reset(mv_handle h) {
             std::memset(h->h_finalObs.p, 0, N * px * 4);
             if (h->wantDepth) std::memset(h->h_finalDepth.p, 0, sizeof(float) * N * px);
         }
-        regenerateNext(h);
+        if (h->levelSet) h->scheduleBank();
+        else regenerateNext(h);
         h->didReset = true;
     }
     int rc = h->flushUploads();
@@ -1579,7 +1714,7 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
     if (rc || n == 0) return rc;
     for (int i = 0; i < n; ++i) {
         const StateStore::HostRow &r = st->host[size_t(rows[i])];
-        if (!r.gen) { h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was never saved"); return MV_ERR_ARG; }
+        if (!r.saved) { h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was never saved"); return MV_ERR_ARG; }
         // the generator travels by value and the reward-shaping row stays with the env: a row of another scenario would turn the env into
         // that scenario with a reward table that does not fit it
         if (r.scenario != h->envScenarioName[size_t(envs[i])]) {
@@ -1636,6 +1771,42 @@ int mv_state_row_bytes(mv_handle h, int64_t *out) {
     *out = int64_t(h->stateRowBytes());
     return MV_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ level sets
+static int levelSetCall(mv_handle h, const char *fn) {
+    if (!h->levelSet) { h->setError(std::string(fn) + ": option level_set is off"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+int mv_level_ids(mv_handle h, const int32_t **out) {
+    if (!h || !out) return MV_ERR_ARG;
+    const int rc = levelSetCall(h, "mv_level_ids");
+    if (rc == MV_OK) *out = h->h_levelIds.p;
+    return rc;
+}
+int mv_level_ids_device(mv_handle h, int32_t **p) {
+    if (!h || !p) return MV_ERR_ARG;
+    const int rc = levelSetCall(h, "mv_level_ids_device");
+    if (rc == MV_OK) *p = h->d_levelIds.p;
+    return rc;
+}
+int mv_next_levels_device(mv_handle h, int32_t **p) {
+    if (!h || !p) return MV_ERR_ARG;
+    const int rc = levelSetCall(h, "mv_next_levels_device");
+    if (rc == MV_OK) *p = h->d_nextLevels.p;
+    return rc;
+}
+int mv_set_next_levels(mv_handle h, const int32_t *envs, const int32_t *levels, int n) {
+    MV_ON_DEVICE(h)
+    const int rc = levelSetCall(h, "mv_set_next_levels");
+    if (rc) return rc;
+    if (n < 0 || (n > 0 && (!envs || !levels))) { h->setError("mv_set_next_levels: bad env / level arrays"); return MV_ERR_ARG; }
+    for (int i = 0; i < n; ++i) {
+        if (envs[i] < 0 || envs[i] >= h->E) { h->setError("mv_set_next_levels: env " + std::to_string(envs[i]) + " out of range"); return MV_ERR_ARG; }
+        if (levels[i] < 0 || levels[i] >= h->levelSet) { h->setError("mv_set_next_levels: level " + std::to_string(levels[i]) + " is outside the set of " + std::to_string(h->levelSet)); return MV_ERR_ARG; }
+    }
+    return n ? h->setNextLevels(envs, levels, n) : MV_OK;
+}
+uint32_t mv_level_set_pick(uint32_t pick_seed, int32_t episode, int32_t count) { return mvLevelSetPick(pick_seed, episode, count); }
 
 int mv_fetch_obs(mv_handle h) {
     MV_ON_DEVICE(h)
@@ -1872,7 +2043,7 @@ static int dumpLevel(const MvLevel &L, const MvBox *statics, const float *static
 
 int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
-    const size_t lid = size_t(env) * h->levelSlots + h->hostSlot[size_t(env)];
+    const size_t lid = h->liveRow(env);
     return dumpLevel(h->h_levels.p[lid], h->h_statics.p + lid * size_t(h->staticCap), h->h_staticRot.p + lid * size_t(h->staticCap) * 2, h->A, false, out, cap);
 }
 
@@ -1886,7 +2057,7 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cudaMemcpy(ag.data(), &h->d_agents.p[size_t(env) * h->A], sizeof(MvAgent) * h->A, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cudaMemcpy(ob.data(), &h->d_objects.p[size_t(env) * MV_MAX_OBJECTS], sizeof(MvObject) * MV_MAX_OBJECTS, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
-    const size_t lid = size_t(env) * h->levelSlots + es.slot;
+    const size_t lid = h->rowOfSlot(env, es.slot);
     const MvLevel &L = h->h_levels.p[lid];
     std::vector<float> o;
     int ncol = h->A + L.n_obj;
@@ -1933,7 +2104,7 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     MvEnvState es;
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
-    const size_t lid = size_t(env) * h->levelSlots + es.slot;
+    const size_t lid = h->rowOfSlot(env, es.slot);
     const MvLevel &L = h->h_levels.p[lid];
     const uint32_t *sol = h->h_solid.p + lid * 3 * h->gridWords;
     const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);

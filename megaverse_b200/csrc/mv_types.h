@@ -1,7 +1,7 @@
 // Shared host/device plain-old-data layouts for the H100 voxel-world engine.
 //
 // HBM layout (one GPU, E envs, A agents per env, N = E*A views):
-//   levels   MvLevel[E][2]          double-buffered immutable level description (host-generated, H2D on reset only)
+//   levels   MvLevel[E][2]          double-buffered immutable level description (host-generated, H2D on reset only); [bank rows] with "level_set"
 //   statics  MvBox[E][2][staticCap] the levels' static layout boxes (collider order == draw order); staticCap grows on demand
 //   staticRot float[E][2][staticCap][2]  MV_ROTATED boxes: local x axis in world space (ax, az)
 //   solid    uint32[E][2][3][GW]    bit-packed voxel planes over the level's bounding grid: solid, exit terrain, lava terrain
@@ -192,7 +192,7 @@ struct MvEnvState {
     float episode_sec;
     int32_t num_frames;
     int32_t episode_idx;
-    int32_t slot;            // which MvLevel[2] is live
+    int32_t slot;            // the live slot of the env's ring of level slots; with option "level_set" the env's live row of the bank
     int32_t highest_tower;
     float bz_reward;         // currBuildingZoneReward
     int32_t faults;
@@ -203,7 +203,7 @@ struct MvEnvState {
     int32_t positive_collected;  // Collect; Sokoban: numBoxesOnGoal
     int32_t bz_count, bz_nb, bz_next_resize;
     int16_t bz_items[MV_MAX_OBJECTS][4];
-    int32_t pad[2];
+    int32_t pad[2];          // pad[0]: with option "level_set" the env's pick seed (uint32 bits), set by the host, never by the kernel; pad[1]: 0
 };
 
 // One drawable of an env, in the reference's draw order (mesh type major, insertion order minor,

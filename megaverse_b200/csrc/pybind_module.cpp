@@ -253,6 +253,19 @@ public:
         check(rc);
     }
 
+    // (extension, option "level_set") the level of the set each env is on: for an env that just ended, the new episode's
+    py::array_t<int32_t> getLevelIds() {
+        alive();
+        const int32_t *ids;
+        check(mv_level_ids(h__, &ids));
+        return py::array_t<int32_t>({numEnvs_}, ids, py::none{});
+    }
+    void setNextLevels(const std::vector<int32_t> &envs, const std::vector<int32_t> &levels) {
+        alive();
+        if (envs.size() != levels.size()) throw std::invalid_argument("set_next_levels: envs and levels differ in length");
+        check(mv_set_next_levels(h__, envs.data(), levels.data(), int(envs.size())));
+    }
+
     void close() {
         if (h__) { mv_close(h__); h__ = nullptr; }
     }
@@ -309,6 +322,9 @@ PYBIND11_MODULE(megaverse, m) {
         .def("states_load", &MegaverseGym::statesLoad)
         .def("states_destroy", &MegaverseGym::statesDestroy)
         .def("reset_envs", &MegaverseGym::resetEnvs, py::arg("envs"), py::arg("seeds") = py::none())
+        .def("level_ids", &MegaverseGym::getLevelIds, "int32[num_envs] (option level_set): the level of the set each env is on; after an end, the new episode's")
+        .def("set_next_levels", &MegaverseGym::setNextLevels, py::arg("envs"), py::arg("levels"),
+             "(option level_set) env envs[i] plays level levels[i] in its next episode, once; followed by reset_envs(envs) it starts them on those levels now")
         .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),
              "step the listed envs only: the others run nothing, report reward 0 and done 0, and keep their observations");
 }

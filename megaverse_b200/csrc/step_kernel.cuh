@@ -21,6 +21,7 @@
 #pragma once
 #include "bzset.h"
 #include "dev_math.cuh"
+#include "level_set.h"
 #include "mv_types.h"
 #include "../../include/megaverse_b200.h"  // MV_SEG_*
 
@@ -40,6 +41,7 @@ constexpr float kMaxAcceleration = 35.0f + 15.0f, kMaxAirAcceleration = 3.0f, kE
 constexpr unsigned FULL = 0xffffffffu;
 
 struct StepParams {
+    // the level arrays are indexed by level row (levelRow): [E][slots] rows with the slot ring, [level-set bank rows] with option "level_set"
     const MvLevel *levels;       // [E][slots]
     const MvBox *statics;        // [E][slots][staticCap] static layout boxes of the level slots (collider order == draw order)
     const float *staticRot;      // [E][slots][staticCap][2] MV_ROTATED boxes: local x axis in world space (ax, az)
@@ -74,6 +76,13 @@ struct StepParams {
     int repeat;                  // option "action_repeat": physics ticks per call (1..4), the episode stops them early
     int slots;                   // option "level_slots": level slots per env (2 or 4), one live and the rest staged in episode order
     int maxObj;                  // upper bound of n_obj over the live and staged levels (sizes the staging copy)
+    // Level set (option "level_set"; levelSet == 0: off, the pointers are unused).  The level arrays are a bank of immutable rows shared by
+    // the envs, MvEnvState::slot is the env's live bank row and MvEnvState::pad[0] its pick seed; an episode end chooses the next row here
+    int levelSet;                // levels per scenario
+    const int32_t *bankBase;     // [E] first bank row of the env's scenario: an env only ever reads rows [bankBase, bankBase + levelSet)
+    int32_t *nextLevels;         // [E] the caller's choice for the env's next episode, -1 (or anything outside [0, levelSet)): the hash picks
+    int32_t *levelIds;           // [E] the live level of every env stepped, within its scenario, written beside dones
+    int32_t *hostLevelIds;       // optional pinned host mirror (or nullptr)
     uint32_t *prof;              // optional [E][16] per-phase cycle stamps (mv_debug_step_profile); nullptr in production
     uint8_t *doneReasons;        // [E] MV_END_* of this step, written beside dones (MV_END_NONE where dones is 0)
     uint8_t *hostDoneReasons;    // optional pinned host mirror (or nullptr)
@@ -84,6 +93,11 @@ struct StepParams {
     float *termViews;
     MvConsts k;
 };
+
+// row of the level arrays that holds slot `slot` of env `env`: the env's own ring of slots, or, with a level set, the bank row itself
+template <bool kLevelSet> __device__ __forceinline__ size_t levelRow(const StepParams &P, int env, int slot) {
+    return kLevelSet ? size_t(slot) : size_t(env) * P.slots + slot;
+}
 
 // One per warp.  A call runs up to P.repeat ticks (option "action_repeat") on this state and then writes its outputs once; every field
 // is one of: [state] the env's state, staged once per call, carried from tick to tick and committed once; [tick] scratch rewritten by
@@ -879,7 +893,9 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
 }
 
 // ---------------------------------------------------------------- the kernel
-__global__ void __launch_bounds__(128) stepKernel(StepParams P) {
+// kLevelSet: the level-set variant (StepParams::levelSet > 0).  A template parameter, not a run-time branch, so that the default
+// variant is the code it was before level sets existed
+template <bool kLevelSet> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     extern __shared__ __align__(128) unsigned char smemRaw[];
     const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slotInGrid = blockIdx.x * (blockDim.x >> 5) + warpInBlock;
@@ -901,6 +917,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
             P.doneReasons[env] = MV_END_NONE;
             if (P.hostDones) P.hostDones[env] = 0;
             if (P.hostDoneReasons) P.hostDoneReasons[env] = MV_END_NONE;
+            if (kLevelSet && P.hostLevelIds) P.hostLevelIds[env] = P.levelIds[env];  // unchanged; the ring slot may hold an older call's
             __threadfence();
             asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
         }
@@ -935,9 +952,9 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     }
     __syncwarp();
     int slot = S.env.slot;
-    const MvLevel *L = &P.levels[size_t(env) * P.slots + slot];
-    const MvBox *statics = P.statics + (size_t(env) * P.slots + slot) * size_t(P.staticCap);
-    const float *staticRot = P.staticRot + (size_t(env) * P.slots + slot) * size_t(P.staticCap) * 2;
+    const MvLevel *L = &P.levels[levelRow<kLevelSet>(P, env, slot)];
+    const MvBox *statics = P.statics + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap);
+    const float *staticRot = P.staticRot + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap) * 2;
     int ns = L->n_static, no = L->n_obj;
     if (!P.forceReset) mbarWait(&S.mbar, 0);
 
@@ -1167,7 +1184,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                             toVoxel(v3(S.agents[j].object_t[12], S.agents[j].object_t[13], S.agents[j].object_t[14]), cx, cy, cz);
                             if (cx == vx && cy == vy && cz == vz) { collidesWithAgent = true; break; }
                         }
-                        const uint32_t *sol = P.solid + (size_t(env) * P.slots + slot) * 3 * P.gridWords;
+                        const uint32_t *sol = P.solid + levelRow<kLevelSet>(P, env, slot) * 3 * P.gridWords;
                         auto solidAt = [&](int g) { return g >= 0 && ((sol[g >> 5] >> (g & 31)) & 1u); };
                         auto objAt = [&](int g) { return g >= 0 ? int(objGrid[g]) : int(MV_NO_OBJECT); };
                         const bool empty = !solidAt(gi) && objAt(gi) == MV_NO_OBJECT;
@@ -1234,7 +1251,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                         }
                     }
                 }
-                const uint32_t *planes = P.solid + (size_t(env) * P.slots + slot) * 3 * P.gridWords;
+                const uint32_t *planes = P.solid + levelRow<kLevelSet>(P, env, slot) * 3 * P.gridWords;
                 auto planeBit = [&](int plane, int g) { return g >= 0 && ((planes[size_t(plane) * P.gridWords + (g >> 5)] >> (g & 31)) & 1u); };
                 // FallDetectionComponent::resetAgent (component_fall_detection.hpp:44-56) -> KinematicCharacterController::warp
                 auto resetAgent = [&](int i) {
@@ -1439,8 +1456,8 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
                 e.num_frames += 1;
                 // a requested end (mv_step_device_ends) is a timer end after the call's last tick; with two level slots, before the episode's
                 // third call the env's next level may not be staged yet (every call of an episode but one that ends runs all its ticks, so that
-                // is 3 * repeat ticks).  Four slots always hold the next level
-                const bool requested = P.ends && P.ends[env] && tick == P.repeat - 1 && (P.slots != 2 || e.num_frames >= 3 * P.repeat);
+                // is 3 * repeat ticks).  Four slots always hold the next level, and so does a level set
+                const bool requested = P.ends && P.ends[env] && tick == P.repeat - 1 && (kLevelSet || P.slots != 2 || e.num_frames >= 3 * P.repeat);
                 S.doneFlag = (e.episode_sec >= len || requested) ? 1 : 0;
             }
             __syncwarp();
@@ -1488,17 +1505,32 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
         if (lane < 8) tCounts[lane] = counts[lane];
         for (int i = lane; i < A * 16; i += 32) tViews[i] = P.views[size_t(env) * A * 16 + i];
         __syncwarp();
-        writeInstances(S, *L, statics, P.deco + (size_t(env) * P.slots + slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
+        writeInstances(S, *L, statics, P.deco + levelRow<kLevelSet>(P, env, slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
         __syncwarp();
     }
 
     if (resetNow) {
-        // flip to the pre-staged next level (episode end, or mv_reset forcing a new episode everywhere): the slots form a ring
-        slot = slot + 1 == P.slots ? 0 : slot + 1;
-        L = &P.levels[size_t(env) * P.slots + slot];
-        statics = P.statics + (size_t(env) * P.slots + slot) * size_t(P.staticCap);
-        staticRot = P.staticRot + (size_t(env) * P.slots + slot) * size_t(P.staticCap) * 2;
-        if (lane == 0) {
+        if (kLevelSet) {
+            // level set: the next level is a row of the bank, chosen here -- the caller's choice when it names a level of the set (used once),
+            // else the hash of the env's pick seed and the new episode's index.  The entry comes from outside the engine: it is bounded
+            // before it indexes anything, and a value out of range is left alone and ignored.  Bank rows are always there: no serial check
+            if (lane == 0) {
+                S.env.episode_idx += 1;
+                int j = P.nextLevels[env];
+                if (j >= 0 && j < P.levelSet) P.nextLevels[env] = -1;
+                else j = int(mvLevelSetPick(uint32_t(S.env.pad[0]), S.env.episode_idx, P.levelSet));
+                S.env.slot = P.bankBase[env] + j;
+            }
+            __syncwarp();
+            slot = S.env.slot;
+        } else {
+            // flip to the pre-staged next level (episode end, or mv_reset forcing a new episode everywhere): the slots form a ring
+            slot = slot + 1 == P.slots ? 0 : slot + 1;
+        }
+        L = &P.levels[levelRow<kLevelSet>(P, env, slot)];
+        statics = P.statics + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap);
+        staticRot = P.staticRot + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap) * 2;
+        if (lane == 0 && !kLevelSet) {
             S.env.slot = slot;
             S.env.episode_idx += 1;
             if (L->serial != S.env.episode_idx) S.env.faults |= MV_FAULT_LEVEL_NOT_READY;
@@ -1525,7 +1557,7 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     __syncwarp();
     MV_PROBE(6);  // outputs, flip/reset, object write-back
 
-    writeInstances(S, *L, statics, P.deco + (size_t(env) * P.slots + slot) * P.decoCap, P.instances + size_t(env) * P.instStride, P.instCounts + size_t(env) * 8, P.views + size_t(env) * A * 16, A, resetNow, lane);
+    writeInstances(S, *L, statics, P.deco + levelRow<kLevelSet>(P, env, slot) * P.decoCap, P.instances + size_t(env) * P.instStride, P.instCounts + size_t(env) * 8, P.views + size_t(env) * A * 16, A, resetNow, lane);
 
     MV_PROBE(7);  // instance list + views
 
@@ -1543,6 +1575,11 @@ __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     // publish: everything this warp wrote (state, instance list, views, zeroed triangle counters) before the stamp
     __syncwarp();
     if (lane == 0) {
+        if (kLevelSet) {  // the level the returned frame shows: after an end, the new episode's
+            const int32_t id = S.env.slot - P.bankBase[env];
+            P.levelIds[env] = id;
+            if (P.hostLevelIds) P.hostLevelIds[env] = id;
+        }
         __threadfence();
         asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
     }

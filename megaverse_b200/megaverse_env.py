@@ -70,7 +70,7 @@ class MegaverseEnv(Env):
     SKIP_UNFIT_LEVELS = False
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
-                 action_repeat=1, segmentation=False):
+                 action_repeat=1, segmentation=False, num_levels=None, start_level=0):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
@@ -78,6 +78,9 @@ class MegaverseEnv(Env):
         # once; an episode end stops the ticks, and the rewards returned are each agent's sum over the ticks run (option "action_repeat")
         # (extension) segmentation=True: segmentation() gives, per agent, the class and index of the drawable behind every pixel of its
         # current observation (option "segmentation"); step()'s return values do not change
+        # (extension) num_levels=L, start_level=s (Procgen's names): the envs play a fixed set of L levels per scenario, the first levels of
+        # the generators seeded s .. s + L - 1, kept on the GPU (option "level_set").  level_ids() tells which level each env is on,
+        # set_next_levels() chooses an env's next one, and the infos of done agents carry 'level', the level the finished episode was played on
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -116,6 +119,13 @@ class MegaverseEnv(Env):
             self.env.set_option("segmentation", 1)
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
+        self.num_levels = None if num_levels is None else int(num_levels)
+        self._levels_played = None  # per env: the level of the episode in progress, i.e. level_ids() as of the previous call
+        if self.num_levels is not None:
+            if self.num_levels < 1:
+                raise ValueError('num_levels must be positive')
+            self.env.set_option("level_set_seed", int(start_level))
+            self.env.set_option("level_set", self.num_levels)
         self.default_shaping_scheme = self.env.get_reward_shaping(0, 0)
         # each scenario's default scheme, read from its first env before anyone could change it
         self._default_shaping = {}
@@ -154,9 +164,23 @@ class MegaverseEnv(Env):
             names = [n for b, n in FAULT_NAMES.items() if word & b]
             raise MegaverseFault("megaverse_b200 engine fault bits 0x%x (%s)" % (word, ", ".join(names)))
 
+    def _note_levels(self):
+        if self.num_levels is not None:
+            self._levels_played = [int(j) for j in self.env.level_ids()]
+
+    def level_ids(self):
+        """(extension, num_levels given) per env, the level of the set it is on now (after a done: the new episode's)"""
+        return [int(j) for j in self.env.level_ids()]
+
+    def set_next_levels(self, envs, levels):
+        """(extension, num_levels given) env envs[i] plays level levels[i] in its next episode, once; afterwards the engine picks again.
+        set_next_levels(envs, levels) followed by reset_envs(envs) starts the listed envs on the listed levels now."""
+        self.env.set_next_levels([int(e) for e in envs], [int(j) for j in levels])
+
     def reset(self):
         self.env.reset()
         self.check_faults()
+        self._note_levels()
         return self.observations()
 
     def step(self, actions):
@@ -185,6 +209,9 @@ class MegaverseEnv(Env):
             dones.extend([done for _ in range(self.num_agents_per_env)])
             if done:
                 infos.extend([dict(true_reward=float(self.env.true_objective(env_i, j))) for j in range(self.num_agents_per_env)])
+                if self.num_levels is not None:
+                    for j in range(self.num_agents_per_env):
+                        infos[env_i * self.num_agents_per_env + j]['level'] = self._levels_played[env_i]
                 if self.final_observation:
                     for j in range(self.num_agents_per_env):
                         view = env_i * self.num_agents_per_env + j
@@ -200,6 +227,7 @@ class MegaverseEnv(Env):
             if skipped:
                 for info in infos:
                     info['levels_skipped'] = skipped
+        self._note_levels()
         rewards = self.env.get_last_rewards()
         obs = self.observations()
         return obs, rewards, dones, infos
@@ -260,13 +288,16 @@ class MegaverseEnv(Env):
             envs = [state.envs[r] for r in rows]
         self.env.states_load(state._store, [int(r) for r in rows], [int(e) for e in envs])
         self.check_faults()
+        self._note_levels()
         return self.observations()
 
     def reset_envs(self, envs, seeds=None):
         """(extension) envs[i] start a new episode now, the other envs keep going; with seeds, env envs[i] first takes seed seeds[i] and
-        plays the first level of that stream.  Returns the observations of every agent, like reset()."""
+        plays the first level of that stream.  Returns the observations of every agent, like reset().  With num_levels, a seed names a
+        pick sequence instead, and set_next_levels(envs, levels) before this call chooses the levels the envs start on."""
         self.env.reset_envs([int(e) for e in envs], None if seeds is None else [int(s) for s in seeds])
         self.check_faults()
+        self._note_levels()
         return self.observations()
 
     def levels_skipped(self):
