@@ -147,7 +147,8 @@ int mv_final_depth_device(mv_handle h, float **d_final_depth);
  * dones, done reasons, true objectives and terminal frames are byte-identical with it on and off.
  * Memory: 2 B per pixel in HBM and again pinned (18 432 B per view at 128 x 72: 75.5 MB each at Collect 1 024 x 4); nothing is
  * allocated while the option is off.
- * Limits: mv_draw_hires and mv_debug_render_instances draw no segmentation; mv_set_obs_buffer does not redirect it (it stays in the
+ * Limits: mv_draw_hires and mv_debug_render_instances draw no segmentation (the debug call mv_debug_render_instances_ex can, with its
+ * own tags); mv_set_obs_buffer does not redirect it (it stays in the
  * engine's own buffer); terminal frames (option final_obs) carry none; the multi-GPU gather does not gather it.
  * Both calls return MV_ERR_ARG when the option is off; the device pointer is refused (MV_ERR_STATE) exactly when mv_depth_device's is. */
 int mv_segmentation_host(mv_handle h, const uint16_t **out);
@@ -252,7 +253,8 @@ int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth);
  * three steps (true with the scenarios' own parameters at action_repeat 1); a violation raises MV_FAULT_LEVEL_NOT_READY in mv_faults and
  * the next call returns MV_ERR_STATE.  Option "level_slots" 4 removes the limit. */
 /* MegaverseGym::drawHires + getHiresObservation (megaverse.cpp:154-177,199-203): renders every agent view once more at w x h
- * (multiples of 32 x 4, e.g. the reference's 768 x 432) from the state of the last step; *out = uint8[N][h][w][4], engine-owned,
+ * (multiples of 32 x 4 up to 768 x 4096, e.g. the reference's 768 x 432: wider frames would take the window coordinates of the scenarios'
+ * scenes past the range the rasteriser's integer set-up is exact in; mv_create takes the same width limit) from the state of the last step; *out = uint8[N][h][w][4], engine-owned,
  * valid until the next mv_draw_hires / mv_close */
 int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out);
 int mv_sync(mv_handle h);
@@ -362,8 +364,18 @@ int mv_debug_get_view(mv_handle h, int env, int agent, float *out16);
  * value.  On any error nothing changes. */
 int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]);
 /* render caller-supplied instances (18 floats each: mesh, colour, 16 model) with one view matrix through the CUDA
- * rasteriser: rgba uint8[h][w][4], depth float[h][w] or NULL.  Host pointers. */
+ * rasteriser: rgba uint8[h][w][4], depth float[h][w] or NULL.  Host pointers.  Sizes with at most 128 tiles of 32 x 4; exact shading,
+ * no segmentation, tri_cap 96, two row bands when the tile rows split evenly (else one): mv_debug_render_instances_ex with those options. */
 int mv_debug_render_instances(const float *view16, const float *inst18, int n, int w, int h, uint8_t *rgba, float *depth);
+/* The same with every variant of the raster kernel a step may launch.  opts[4] = {fast (0/1: the fast fragment stage of option
+ * "fast_shading"), segmentation (0/1), tri_cap (0 = the engine default, else 32..1022), bands (0 = the rule of mv_draw_hires, about a
+ * hundred 32 x 4 tiles per band; else 1..h/4 bands of equal height, the last one shorter)}.  Sizes as mv_draw_hires: multiples of 32 x 4
+ * up to 768 x 4096; n <= 4096 instances sorted by mesh type, colours 0..21.  seg: uint16[h][w], required with segmentation 1: the tag of
+ * each pixel's winner, instance i (0-based) drawn with tag i + 1, 0 where nothing was drawn.  stats: NULL or the kernel's 16 counters
+ * (the ViewParams::stats layout: [4] clipped items, [5] triangles, [6] batches).  depth, seg and stats may be NULL.  MV_ERR_ARG for
+ * a null view, instance, opts or rgba pointer or any value outside these ranges. */
+int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n, int w, int h, const int *opts, uint8_t *rgba, float *depth,
+                                 uint16_t *seg, unsigned long long *stats);
 /* host-only (no CUDA needed): run the level generator for the env RNG stream seeded with env_seed and dump the level of
  * episode `episode` (mv_debug_get_level layout, followed by each agent's 9 spawn-basis floats as bit patterns) */
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *param_keys,

@@ -61,6 +61,7 @@ def lib():
         L.mv_debug_get_view.argtypes = [vp, ci, ci, vp]
         L.mv_debug_warp_agent.argtypes = [vp, ci, ci, vp, vp]
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
+        L.mv_debug_render_instances_ex.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, vp, vp]
         L.mv_debug_bzset.argtypes = [vp, ci, vp, ci]
         L.mv_debug_generate_level.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp, ci]
         L.mv_states_create.argtypes = [vp, ci, C.POINTER(ci)]
@@ -80,7 +81,7 @@ EXPORTS = [
     "mv_rewards", "mv_dones", "mv_true_objectives", "mv_get_reward_shaping", "mv_set_reward_shaping", "mv_set_option", "mv_step_device", "mv_set_obs_buffer",
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
     "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view", "mv_debug_warp_agent",
-    "mv_debug_render_instances", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
+    "mv_debug_render_instances", "mv_debug_render_instances_ex", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
     "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device", "mv_step_envs", "mv_step_device_active",
@@ -403,15 +404,31 @@ class Engine:
         self._ck(lib().mv_debug_warp_agent(self._h, int(env), int(agent), p.ctypes.data, b.ctypes.data))
 
 
-def render_instances(view16, inst18, w, h, want_depth=False):
+def render_instances(view16, inst18, w, h, want_depth=False, fast=None, segmentation=False, tri_cap=None, bands=None, stats=False):
+    """debug: draw caller-supplied instances (18 floats each) with one view through the CUDA rasteriser.  Without the keyword options this
+    is mv_debug_render_instances (exact shading, tri_cap 96, one or two bands); any of them selects mv_debug_render_instances_ex with
+    fast (0/1), segmentation, tri_cap (0 = engine default) and bands (0 = the hi-res rule).  Returns rgba, then depth (want_depth), the
+    uint16 segmentation image (instance i drawn with tag i + 1) and the kernel's 16 counters (stats), those asked for, in that order."""
     view16 = np.ascontiguousarray(view16, dtype=np.float32)
     inst18 = np.ascontiguousarray(inst18, dtype=np.float32).reshape(-1, 18)
     rgba = np.zeros((h, w, 4), dtype=np.uint8)
     depth = np.zeros((h, w), dtype=np.float32)
-    rc = lib().mv_debug_render_instances(view16.ctypes.data, inst18.ctypes.data, inst18.shape[0], w, h, rgba.ctypes.data, depth.ctypes.data if want_depth else None)
-    if rc != MV_OK:
-        raise MegaverseError(rc, "mv_debug_render_instances failed")
-    return (rgba, depth) if want_depth else rgba
+    out = [rgba] + ([depth] if want_depth else [])
+    if fast is None and not segmentation and tri_cap is None and bands is None and not stats:
+        rc = lib().mv_debug_render_instances(view16.ctypes.data, inst18.ctypes.data, inst18.shape[0], w, h, rgba.ctypes.data, depth.ctypes.data if want_depth else None)
+        if rc != MV_OK:
+            raise MegaverseError(rc, "mv_debug_render_instances failed")
+    else:
+        opts = np.array([int(bool(fast)), int(bool(segmentation)), int(tri_cap or 0), int(bands or 0)], dtype=np.int32)
+        seg = np.zeros((h, w), dtype=np.uint16)
+        st = np.zeros(16, dtype=np.uint64)
+        rc = lib().mv_debug_render_instances_ex(view16.ctypes.data, inst18.ctypes.data, inst18.shape[0], w, h, opts.ctypes.data, rgba.ctypes.data,
+                                                depth.ctypes.data if want_depth else None, seg.ctypes.data if segmentation else None,
+                                                st.ctypes.data if stats else None)
+        if rc != MV_OK:
+            raise MegaverseError(rc, "mv_debug_render_instances_ex failed")
+        out += ([seg] if segmentation else []) + ([st] if stats else [])
+    return tuple(out) if len(out) > 1 else rgba
 
 
 def generate_level(scenario, num_agents, env_seed, episode, params=None):

@@ -174,6 +174,15 @@ static mvr::ViewParams frameParams(int W, int H, int bands, int bandRows, unsign
     return vp;
 }
 
+// Widest frame the rasteriser draws (mv_create, mv_draw_hires, the debug entries).  Its integer set-up -- int32 snapped positions and
+// edge coefficients, int64 edge constants and bounds -- is exact while every snapped window coordinate |s| < 2^30.5 sub-pixels and every
+// difference of two corners < 2^31 (tests/test_raster_conformance_gpu.py pins it; just beyond, the snap saturates or the coefficients wrap).
+// A vertex the near clip makes lies on w = 0.01, so window coordinates grow with the lateral extent of the geometry crossing the camera
+// plane, and with the frame's width only (the projection's y scale carries the aspect).  The scenarios' scenes reach |x_ndc| ~ 11 400 with
+// corner differences ~ 17 400 (the hex mazes; tests/test_raster_independent.py measures them): at 768 wide |s| <= 2^30.06 and the
+// differences <= 2^30.67; at 1024 the differences reach 2^31.08.
+constexpr int kMaxRasterWidth = 768;
+
 // the raster kernel variant of a launch: the items it draws, whether it writes segmentation (never with terminal frames), the shading mode
 using ViewKernel = void (*)(mvr::ViewParams);
 static ViewKernel viewKernelOf(mvr::Items items, bool seg, bool fast) {
@@ -728,7 +737,10 @@ struct mv_engine {
     // the last step -- the same kernel over row bands of the large frame.  Result in hires.h_obs, uint8[N][h][w][4].
     int drawHires(int w, int hgt) {
         if (!didReset) { setError("mv_draw_hires before mv_reset"); return MV_ERR_STATE; }
-        if (w < 32 || hgt < 4 || (w % 32) || (hgt % 4) || w > 4096 || hgt > 4096) { setError("hi-res size must be a multiple of 32 x 4"); return MV_ERR_ARG; }
+        if (w < 32 || hgt < 4 || (w % 32) || (hgt % 4) || w > kMaxRasterWidth || hgt > 4096) {
+            setError("hi-res size must be a multiple of 32 x 4, at most 768 x 4096");
+            return MV_ERR_ARG;
+        }
         int rc = drain();
         if (rc) return rc;
         // bands of about a hundred 32x4 tiles each
@@ -1271,7 +1283,10 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
         names[size_t(i)] = s;
         for (char &c : names[size_t(i)]) c = char(std::tolower(static_cast<unsigned char>(c)));  // one spelling per scenario (the state store compares them)
     }
-    if (w <= 0 || h <= 0 || w % 32 != 0 || h % 4 != 0 || (w / 32) * (h / 4) > 128) { g_createError = "render size must be a multiple of 32x4 with at most 128 tiles"; return MV_ERR_ARG; }
+    if (w <= 0 || h <= 0 || w % 32 != 0 || h % 4 != 0 || (w / 32) * (h / 4) > 128 || w > kMaxRasterWidth) {
+        g_createError = "render size must be a multiple of 32x4 with at most 128 tiles, at most 768 wide";
+        return MV_ERR_ARG;
+    }
     for (int i = 0; i < nparams; ++i) {
         if (!keys || !keys[i] || !vals) { g_createError = "null parameter key / value array"; return MV_ERR_ARG; }
         // the interactive viewer's reward-indicator HUD (scenario_default.hpp:144-160, set by viewer_app.cpp:147 only) adds drawables this
@@ -2176,59 +2191,81 @@ int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], con
     return h->warpAgent(env, agent, w);
 }
 
-int mv_debug_render_instances(const float *view16, const float *inst18, int n, int w, int h, uint8_t *rgba, float *depth) {
-    if (!view16 || !inst18 || n < 0 || n > 4096 || w % 32 || h % 4 || (w / 32) * (h / 4) > 128) return MV_ERR_ARG;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return MV_ERR_CUDA;
-    // instances must arrive boxes-first (draw order); count the leading boxes
+int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n, int w, int h, const int *opts, uint8_t *rgba, float *depth,
+                                 uint16_t *seg, unsigned long long *stats) {
+    if (!view16 || !inst18 || !opts || !rgba || n < 0 || n > 4096) return MV_ERR_ARG;
+    if (w < 32 || h < 4 || w % 32 || h % 4 || w > kMaxRasterWidth || h > 4096) return MV_ERR_ARG;  // what mv_draw_hires accepts
+    const bool fast = opts[0] != 0, wantSeg = opts[1] != 0;
+    if ((opts[0] | opts[1]) & ~1 || (wantSeg && !seg)) return MV_ERR_ARG;
+    mv_engine tmp;  // the engine default of tri_cap; the palette upload
+    const int triCap = opts[2] ? opts[2] : tmp.triCap;
+    if (triCap < 32 || triCap > mvr::kMaxTriCap) return MV_ERR_ARG;
+    // row bands: opts[3] of them (the last one may be shorter), or 0 = the rule of mv_draw_hires (bands of about a hundred tiles)
+    int bandRows;
+    if (opts[3] == 0) bandRows = std::max(1, 96 / (w / 32)) * 4;
+    else if (opts[3] > 0 && opts[3] <= h / 4) bandRows = ((h / 4 + opts[3] - 1) / opts[3]) * 4;
+    else return MV_ERR_ARG;
+    const int bands = (h + bandRows - 1) / bandRows;
+    int ndev = 0, dev = 0, maxOptin = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&maxOptin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
+        return MV_ERR_CUDA;
+    const size_t smem = mvr::smemLayout(triCap).total;
+    if (smem > size_t(maxOptin)) return MV_ERR_ARG;
+    // instances must arrive sorted by mesh type, boxes first (draw order); instance i carries segmentation tag i + 1
     std::vector<MvInstance> inst(size_t(n ? n : 1));
-    int nBox = 0;
-    for (int i = 0; i < n; ++i) {
-        inst[size_t(i)].mesh = int(inst18[i * 18]); inst[size_t(i)].color = int(inst18[i * 18 + 1]);
-        std::memcpy(inst[size_t(i)].model, inst18 + i * 18 + 2, 64);
-        if (inst[size_t(i)].mesh == 0) { if (nBox != i) return MV_ERR_ARG; ++nBox; }
+    int32_t cnt[8] = {0, n, 0, 0, 0, 0, 0, 0};
+    for (int i = 0, last = 0; i < n; ++i) {
+        MvInstance &d = inst[size_t(i)];
+        d.mesh = int(inst18[i * 18]); d.color = int(inst18[i * 18 + 1]);
+        std::memcpy(d.model, inst18 + i * 18 + 2, 64);
+        d.pad[0] = i + 1; d.pad[1] = 0;
+        if (d.mesh < last || d.mesh > 4 || d.color < 0 || d.color >= 22) return MV_ERR_ARG;
+        last = d.mesh;
+        cnt[d.mesh == 0 ? 0 : 1 + d.mesh] += 1;
     }
-    mv_engine tmp;  // only for the constants / palette
     MvConsts k;
     fillConsts(k, w, h);
     if (uploadPalette(&tmp) != MV_OK) return MV_ERR_CUDA;
-    int32_t cnt[8] = {nBox, n, 0, 0, 0, 0, 0, 0};
-    {   // instances must be sorted by mesh type (draw order)
-        int last = 0;
-        for (int i = 0; i < n; ++i) {
-            const int m = inst[size_t(i)].mesh;
-            if (m < last || m > 4) return MV_ERR_ARG;
-            last = m;
-            if (m >= 1) cnt[1 + m] += 1;
-        }
-    }
-    // a small triangle list on purpose: scenes of a few hundred triangles exercise the multi-batch path
-    const int triCap = 96;
-    const size_t smem = mvr::smemLayout(triCap).total;
-    MvInstance *dInst = nullptr; int32_t *dCnt = nullptr; float *dView = nullptr, *dDepth = nullptr; uint8_t *dObs = nullptr;
-    uint32_t *dCtr = nullptr; unsigned long long *dSpill = nullptr;
-    const int bands = (h / 4) % 2 == 0 ? 2 : 1, bandRows = (h / 4 / bands) * 4;
+    const ViewKernel fn = viewKernelOf(mvr::Items::All, wantSeg, fast);
+    MvInstance *dInst = nullptr; int32_t *dCnt = nullptr; float *dView = nullptr, *dDepth = nullptr; uint8_t *dObs = nullptr; uint16_t *dSeg = nullptr;
+    uint32_t *dCtr = nullptr; unsigned long long *dSpill = nullptr, *dStats = nullptr;
+    const size_t px = size_t(w) * size_t(h);
+    // the attribute is the device maximum, as configureRaster sets it: an engine alive in this process keeps launching with its own tri_cap
     bool ok = cudaMalloc(&dInst, sizeof(MvInstance) * inst.size()) == cudaSuccess && cudaMalloc(&dCnt, 32) == cudaSuccess &&
-              cudaMalloc(&dView, 64) == cudaSuccess && cudaMalloc(&dObs, size_t(w) * h * 4) == cudaSuccess && cudaMalloc(&dDepth, size_t(w) * h * 4) == cudaSuccess &&
+              cudaMalloc(&dView, 64) == cudaSuccess && cudaMalloc(&dObs, px * 4) == cudaSuccess && cudaMalloc(&dDepth, px * 4) == cudaSuccess &&
+              cudaMalloc(&dSeg, px * 2) == cudaSuccess && cudaMalloc(&dStats, 16 * sizeof(unsigned long long)) == cudaSuccess &&
               cudaMalloc(&dCtr, 16) == cudaSuccess && cudaMalloc(&dSpill, sizeof(unsigned long long) * size_t(bands) * size_t(w) * bandRows) == cudaSuccess &&
-              cudaFuncSetAttribute(mvr::viewKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) == cudaSuccess;
+              cudaFuncSetAttribute(reinterpret_cast<const void *>(fn), cudaFuncAttributeMaxDynamicSharedMemorySize, maxOptin) == cudaSuccess;
     if (ok) {
         cudaMemcpy(dInst, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice);
         cudaMemcpy(dCnt, cnt, 32, cudaMemcpyHostToDevice);
         cudaMemcpy(dView, view16, 64, cudaMemcpyHostToDevice);
         cudaMemset(dCtr, 0, 16);
+        cudaMemset(dStats, 0, 16 * sizeof(unsigned long long));
         mvr::ViewParams vp = frameParams(w, h, bands, bandRows, dSpill, triCap, k);
         vp.instances = dInst; vp.instCounts = dCnt; vp.views = dView; vp.instStride = int(inst.size()); vp.obs = dObs; vp.depth = depth ? dDepth : nullptr;
+        vp.seg = wantSeg ? dSeg : nullptr; vp.stats = stats ? dStats : nullptr;
         vp.workCounter = dCtr; vp.viewBase = 0; vp.N = 1; vp.A = 1;
-        mvr::viewKernel<false><<<bands, mvr::kThreads, smem>>>(vp);
+        fn<<<bands, mvr::kThreads, smem>>>(vp);
         ok = cudaDeviceSynchronize() == cudaSuccess;
         if (ok) {
-            cudaMemcpy(rgba, dObs, size_t(w) * h * 4, cudaMemcpyDeviceToHost);
-            if (depth) cudaMemcpy(depth, dDepth, size_t(w) * h * 4, cudaMemcpyDeviceToHost);
+            cudaMemcpy(rgba, dObs, px * 4, cudaMemcpyDeviceToHost);
+            if (depth) cudaMemcpy(depth, dDepth, px * 4, cudaMemcpyDeviceToHost);
+            if (wantSeg) cudaMemcpy(seg, dSeg, px * 2, cudaMemcpyDeviceToHost);
+            if (stats) cudaMemcpy(stats, dStats, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
         }
     }
-    cudaFree(dCtr); cudaFree(dSpill); cudaFree(dInst); cudaFree(dCnt); cudaFree(dView); cudaFree(dObs); cudaFree(dDepth);
+    cudaFree(dCtr); cudaFree(dSpill); cudaFree(dInst); cudaFree(dCnt); cudaFree(dView); cudaFree(dObs); cudaFree(dDepth); cudaFree(dSeg); cudaFree(dStats);
     return ok ? MV_OK : MV_ERR_CUDA;
+}
+
+int mv_debug_render_instances(const float *view16, const float *inst18, int n, int w, int h, uint8_t *rgba, float *depth) {
+    if (w < 32 || h < 4 || w % 32 || h % 4 || (w / 32) * (h / 4) > 128) return MV_ERR_ARG;
+    // exact shading, no segmentation, a small triangle list on purpose (scenes of a few hundred triangles exercise the multi-batch path),
+    // two bands when the tile rows split evenly
+    const int opts[4] = {0, 0, 96, (h / 4) % 2 == 0 ? 2 : 1};
+    return mv_debug_render_instances_ex(view16, inst18, n, w, h, opts, rgba, depth, nullptr, nullptr);
 }
 
 // host-only (no CUDA): run the product's level generator for env stream `env_seed` and dump episode `episode`'s level in

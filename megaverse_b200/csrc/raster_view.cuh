@@ -981,11 +981,13 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
                 if (instanceMayBeVisible(mv, mesh == 1 ? 2.0f : 1.0f, P.p00, P.p11)) {
                     float nm[9];
                     const float det = normalMatrix(mv, nm);
-                    if (!(det > 0.0f)) meta |= 1 << 16;  // a mirroring transform turns the winding round: no object-space face test for its triangles
+                    const bool mirrored = !(det > 0.0f);
+                    if (mirrored) meta |= 1 << 16;  // a mirroring transform turns the winding round: no object-space face test for its triangles
                     if (mesh == 0) {
                         // a box face whose plane clearly faces away from the eye (the view-space origin) only yields triangles the
-                        // winding test drops: outward normal n, face centre = origin + n (unit cube), cull when n_view . c_view > 0
-                        int mask = 0;
+                        // winding test drops: outward normal n, face centre = origin + n (unit cube), cull when n_view . c_view > 0.
+                        // Not so under a mirroring transform: there the faces turned away are the ones drawn, so all six stay
+                        int mask = mirrored ? 63 : 0;
 #pragma unroll
                         for (int face = 0; face < 6; ++face) {
                             const float *fn = meshV + (face * 4) * 6 + 3;

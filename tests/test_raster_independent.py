@@ -7,142 +7,40 @@ specification's: view-volume clipping 0 <= z_c <= w_c, the viewport transform, f
 one sample at the pixel centre, the top-left rule for samples exactly on an edge, depth interpolated linearly in window space,
 perspective-correct interpolation of the varyings (here: clip-space w, which V4R writes out as its depth image).
 
-This file implements those rules a second time, in a different form and in different arithmetic:
-
-  * coverage: exact integers, a sample on an edge is decided by displacing it infinitesimally to the right and, second order, down
-    (lexicographic sign of (E, dE/dx, dE/dy)) -- no top-left classification of edges, no bias constants;
-  * depth and w: float64 barycentrics from the exact integer edge values;
-  * hidden-surface removal: per pixel over all covering triangles, nearest depth, the later draw on ties;
-  * clipping: Sutherland-Hodgman in float64 on the clip coordinates.
-
-Only the vertex stage is shared knowledge (float32 arithmetic in the order of uber.vert / Magnum, pinned elsewhere against the real
-shader text and the real Magnum): it is recomputed here in numpy float32 so that both sides snap the same window coordinates.
+raster_ref.py implements those rules a second time, in a different form and in different arithmetic (exact integer coverage with an
+infinitesimal-displacement tie rule, float64 depth and w, float64 Sutherland-Hodgman clipping, unbounded window coordinates); this file
+checks it against the oracle, on random scenes here and on every constructed scene family of test_raster_conformance_gpu.py, and
+bounds the window coordinates the product's own scenes produce (the envelope inside which the kernel's integer set-up is exact).
 
 Compared: the oracle's depth image (view-space w of the visible fragment, 0 = nothing drawn) -- its zero pattern IS the coverage
 mask.  Scenes without clipping must agree in every pixel (coverage exactly, depth to float32 rounding); scenes cut by the near
 plane (the clipper creates new vertices, whose float32 vs float64 positions can snap one sub-pixel apart) in all but a handful.
 """
+import warnings
+
 import numpy as np
 import pytest
 
 import orc
+import raster_ref as ref
 
 W, H = 128, 72
 F32 = np.float32
 
 
 def _projection():
-    aspect = F32(W) / F32(H)
-    half_tan = F32(np.tan(np.float64(F32(100.0) * F32(0.01745329251994329576923690768489)) / 2.0))  # correctly rounded tan, as the oracle's crtan
-    near, far = F32(0.01), F32(120.0)
-    return F32(1.0) / half_tan, -aspect / half_tan, far / (near - far), far * near / (near - far)
-
-
-def _mesh(kind):
-    vtx, idx = orc.mesh(kind)
-    return vtx.view(np.float32).reshape(-1, 6)[:, :3].copy(), idx.reshape(-1, 3).astype(np.int64)
-
-
-def _vertex_stage(view16, model16, verts):
-    """clip-space positions, float32, in the operation order of the vertex stage (uber.vert:53-110 on Magnum's column-major matrices)"""
-    v = view16.reshape(4, 4)   # v[col][row]
-    m = model16.reshape(4, 4)
-    mv = np.zeros((4, 4), dtype=F32)
-    for col in range(4):
-        for row in range(4):
-            acc = F32(0.0)
-            for pos in range(4):
-                acc = F32(acc + F32(v[pos][row] * m[col][pos]))
-            mv[col][row] = acc
-    p00, p11, p22, p32 = _projection()
-    out = np.zeros((len(verts), 4), dtype=F32)
-    for i, p in enumerate(verts):
-        cam = []
-        for row in range(3):
-            acc = F32(0.0)
-            acc = F32(acc + F32(mv[0][row] * p[0])); acc = F32(acc + F32(mv[1][row] * p[1])); acc = F32(acc + F32(mv[2][row] * p[2])); acc = F32(acc + F32(mv[3][row] * F32(1.0)))
-            cam.append(acc)
-        out[i] = (F32(cam[0] * p00), F32(cam[1] * p11), F32(F32(cam[2] * p22) + p32), F32(-cam[2]))
-    return out
-
-
-def _snap(clip):
-    """viewport transform + fixed point, the window coordinates a rasteriser with 8 sub-pixel bits works on (float32 like the oracle)"""
-    r = F32(1.0) / clip[3]
-    hw, hh = F32(W) * F32(0.5), F32(H) * F32(0.5)
-    x = F32(F32(F32(clip[0] * r) * hw) + hw)
-    y = F32(F32(F32(clip[1] * r) * hh) + hh)
-    return int(np.floor(np.float64(F32(F32(x * F32(256.0)) + F32(0.5))))), int(np.floor(np.float64(F32(F32(y * F32(256.0)) + F32(0.5))))), np.float64(F32(clip[2] * r)), np.float64(r)
-
-
-def _clip_polygon(poly):
-    """Sutherland-Hodgman against 0 <= z <= w in float64 (Vulkan 'primitive clipping', depth range zero-to-one)"""
-    for plane in (0, 1):
-        dist = (lambda c: c[2]) if plane == 0 else (lambda c: c[3] - c[2])
-        out = []
-        for i in range(len(poly)):
-            a, b = poly[i], poly[(i + 1) % len(poly)]
-            da, db = dist(a), dist(b)
-            if da >= 0:
-                out.append(a)
-            if (da >= 0) != (db >= 0):
-                t = da / (da - db)
-                out.append(a + t * (b - a))
-        poly = out
-        if len(poly) < 3:
-            return []
-    return poly
+    return ref.projection(W, H)
 
 
 STATS = {"ties": 0}  # samples that lay exactly on an edge of a front-facing triangle (the cases the tie rule decides)
 
 
 def _independent_depth(view16, instances):
-    """depth image (view-space w of the visible fragment, 0 = empty) by the rules of the specification; also returns whether any
-    primitive needed clipping"""
-    ys, xs = np.mgrid[0:H, 0:W]
-    sx = (xs * 256 + 128).astype(np.int64)
-    sy = (ys * 256 + 128).astype(np.int64)
-    best_z = np.full((H, W), np.inf)
-    best_w = np.zeros((H, W))
-    clipped_any = False
-    for row in instances:
-        verts, tris = _mesh(int(row[0]))
-        clip = _vertex_stage(view16, row[2:18].astype(F32), verts)
-        for tri in tris:
-            c = clip[tri]
-            needs_clip = bool((c[:, 2] < 0).any() or (c[:, 3] - c[:, 2] < 0).any())
-            if needs_clip:
-                clipped_any = True
-                poly = _clip_polygon([c[k].astype(np.float64) for k in range(3)])
-                pieces = [(poly[0], poly[k], poly[k + 1]) for k in range(1, len(poly) - 1)]
-            else:
-                pieces = [(c[0], c[1], c[2])]
-            for piece in pieces:
-                sv = [_snap(np.asarray(v, dtype=F32)) for v in piece]
-                (x0, y0, z0, r0), (x1, y1, z1, r1), (x2, y2, z2, r2) = sv
-                area2 = (x1 - x0) * (y2 - y0) - (y1 - y0) * (x2 - x0)
-                if area2 >= 0:
-                    continue  # clockwise on a y-down screen = back face (front faces are counter-clockwise in y-up NDC), or degenerate
-                inside = np.ones((H, W), dtype=bool)
-                lam = []
-                for (ax, ay), (bx, by) in (((x1, y1), (x2, y2)), ((x2, y2), (x0, y0)), ((x0, y0), (x1, y1))):
-                    # edge function oriented so that the interior is positive; a sample ON the edge counts iff an infinitesimal step
-                    # right (then down) enters the interior: sign of (E, dE/dx, dE/dy) in lexicographic order
-                    dEdx, dEdy = (by - ay), -(bx - ax)
-                    E = dEdx * (sx - ax) + dEdy * (sy - ay)
-                    tie = dEdx > 0 or (dEdx == 0 and dEdy > 0)
-                    inside &= (E > 0) | ((E == 0) & tie)
-                    STATS["ties"] += int((E == 0).sum())
-                    lam.append(E.astype(np.float64) / float(-area2))
-                if not inside.any():
-                    continue
-                z = lam[0] * z0 + lam[1] * z1 + lam[2] * z2                 # depth: linear in window space
-                w = 1.0 / (lam[0] * r0 + lam[1] * r1 + lam[2] * r2)        # perspective-correct w
-                win = inside & (z <= 1.0) & (z <= best_z)                     # LESS_OR_EQUAL: the later draw replaces an equal depth
-                best_z = np.where(win, z, best_z)
-                best_w = np.where(win, w, best_w)
-    return best_w, clipped_any
+    """depth image (view-space w of the visible fragment, 0 = empty) by the rules of the specification at 128 x 72; also returns whether
+    any primitive needed clipping"""
+    R = ref.render(view16, instances, W, H)
+    STATS["ties"] += R.ties
+    return R.w, R.clipped
 
 
 def _random_scene(rng, n, near_camera):
@@ -291,3 +189,112 @@ def test_cuda_rasteriser_against_the_independent_rules(kind, seed):
     both = cov_dev & cov_mine
     rel = np.abs(dev[both].astype(np.float64) - mine[both]) / mine[both]
     assert (rel > (1e-4 if kind == "near" else 2e-5)).sum() <= (8 if kind == "near" else 0)
+
+
+# ---------------------------------------------------------------------------------------------------- constructed scene families
+import raster_scenes as scenes  # noqa: E402
+
+
+@pytest.mark.parametrize("size", [(128, 72), (64, 64), (32, 512), (512, 32), (160, 96)])
+@pytest.mark.parametrize("family", sorted(scenes.FAMILIES))
+def test_scene_families_reach_their_branch_and_agree_with_the_oracle(family, size):
+    """every constructed family of test_raster_conformance_gpu.py, drawn by the restatement: it reaches what it was built for, and the
+    oracle agrees with it as on the random scenes (the window coordinates stay far inside the int32 range the oracle snaps to)"""
+    W, H = size
+    view16, inst = scenes.build(family, W, H)
+    R = ref.render(view16, inst, W, H)
+    scenes.check_reach(family, R, W, H)
+    assert max(t["max_coord"] for t in R.tris) < (1 << 30)
+    _, od = orc.render_instances(view16, inst, W, H, want_depth=True)
+    cov_ref, cov_mine = od > 0, R.w > 0
+    mism = int((cov_ref != cov_mine).sum())
+    both = cov_ref & cov_mine
+    rel = np.abs(od[both].astype(np.float64) - R.w[both]) / R.w[both]
+    if family in scenes.CLIPPED:
+        assert mism <= 8 and (rel > 1e-4).sum() <= 8, "coverage differs in %d pixels" % mism
+    else:
+        assert mism == 0, "coverage differs in %d pixels" % mism
+        assert rel.max() < 1e-4 and (rel > 2e-5).sum() <= (0 if size == (128, 72) else 8), "depth differs by %.3g" % rel.max()
+
+
+def test_reference_takes_window_coordinates_unbounded():
+    """a vertex 2^24 pixels off-screen, just in front of the near plane: the restatement keeps its snapped coordinate exact (no int32
+    saturation or wrap) and still draws the on-screen part of the triangle, which covers the samples a guard-band rasteriser covers"""
+    view16, inst = scenes.offscreen_vertex(128, 72, 24, opposite=False)
+    R = ref.render(view16, inst, 128, 72)
+    assert max(t["max_coord"] for t in R.tris) > (1 << 31)
+    assert (R.w > 0).sum() > 100
+
+
+# ---------------------------------------------------------------------------------------------------- the window-coordinate envelope
+SCENARIOS = ["TowerBuilding", "ObstaclesEasy", "ObstaclesHard", "Collect", "Sokoban", "HexMemory", "HexExplore", "Rearrange"]
+
+
+def _window_extent(view16, inst):
+    """largest |x_ndc|, |y_ndc| and largest difference of x_ndc, y_ndc between two corners of a triangle, over every vertex a rasteriser sets
+    up for this view at 128 x 72 (inside both planes, or made by the near / far clip), excluding triangles wholly beyond one side plane"""
+    ext = np.zeros(4)
+    for mesh_kind in np.unique(inst[:, 0]).astype(int):
+        rows = inst[inst[:, 0] == mesh_kind]
+        verts, tris = ref.mesh(mesh_kind)
+        for row in rows:
+            c = ref.vertex_stage(view16, row[2:18], verts, W, H).astype(np.float64)[tris]   # [t][3][4]
+            d_near, d_far = c[..., 2], c[..., 3] - c[..., 2]
+            pts, ok = [c], [(d_near >= 0) & (d_far >= 0)]
+            for d, other in ((d_near, d_far), (d_far, d_near)):
+                for a, b in ((0, 1), (1, 2), (2, 0)):
+                    cross = (d[:, a] >= 0) != (d[:, b] >= 0)
+                    t = np.where(cross, d[:, a] / np.where(cross, d[:, a] - d[:, b], 1.0), 0.0)
+                    p = c[:, a] + t[:, None] * (c[:, b] - c[:, a])
+                    pts.append(p[:, None]); ok.append((cross & ((other[:, a] >= 0) | (other[:, b] >= 0)))[:, None])
+            P = np.concatenate(pts, axis=1)
+            K = np.concatenate(ok, axis=1)
+            side = np.stack([P[..., 0] > P[..., 3], P[..., 0] < -P[..., 3], P[..., 1] > P[..., 3], P[..., 1] < -P[..., 3]], -1)
+            keep = ~(np.where(K[..., None], side, True).all(axis=1).any(axis=-1))      # not wholly beyond one side plane
+            K &= keep[:, None]
+            if not K.any():
+                continue
+            with np.errstate(divide="ignore", invalid="ignore"):
+                nx, ny = P[..., 0] / P[..., 3], P[..., 1] / P[..., 3]
+            nx, ny = np.where(K, nx, np.nan), np.where(K, ny, np.nan)
+            ext[0] = max(ext[0], np.nanmax(np.abs(nx))); ext[1] = max(ext[1], np.nanmax(np.abs(ny)))
+            ext[2] = max(ext[2], np.nanmax(np.nanmax(nx, 1) - np.nanmin(nx, 1))); ext[3] = max(ext[3], np.nanmax(np.nanmax(ny, 1) - np.nanmin(ny, 1)))
+    return ext
+
+
+ENVELOPE_S, ENVELOPE_DS = 2.0 ** 30.5, 2.0 ** 31  # |snapped coordinate| and |difference of two corners|, sub-pixels
+MAX_WIDTH = 768                                   # the widest frame mv_create, mv_draw_hires and the debug entries accept
+
+
+@pytest.mark.parametrize("scenario", SCENARIOS)
+def test_product_scenes_stay_inside_the_exact_envelope(scenario):
+    """The kernel's integer set-up is exact while every snapped window coordinate has |s| < 2^30.5 sub-pixels and every difference of two
+    corners of a triangle is below 2^31 (int32 positions and coefficients, int64 edge constants and bounds; test_raster_conformance_gpu.py
+    pins it).  Here the scenarios' own scenes, a few hundred steps of purposeful actions, are measured at 128 x 72 and scaled to the widest
+    frame the API accepts, 768 x 4096 (window x = (x_ndc + 1) W / 2; y_ndc scales with the aspect W / H, so both grow with the width
+    only).  Vertices made by the near clip lie on w = 0.01, so the measure is the lateral extent of geometry crossing the camera plane:
+    the hex mazes set the limit (at 1024 wide their corner differences would pass 2^31)."""
+    import helpers
+
+    o = orc.Oracle(scenario, 2, 2)
+    o.seed(7)
+    o.reset()
+    rng = np.random.default_rng(0)
+    ext = np.zeros(4)
+    for t in range(150):
+        o.step(helpers.purposeful_actions(rng, 4, t))
+        if t % 3:
+            continue
+        for e in range(2):
+            inst = o.instances(e)
+            for a in range(2):
+                with np.errstate(all="ignore"), warnings.catch_warnings():
+                    warnings.simplefilter("ignore", RuntimeWarning)
+                    ext = np.maximum(ext, _window_extent(o.view(e, a), inst))
+    o.close()
+    Wmax, Hmax = MAX_WIDTH, 4096
+    s_max = max((ext[0] + 1) * Wmax / 2 * 256, (ext[1] * (H / W) * Wmax / 2 + Hmax / 2) * 256)
+    ds_max = max(ext[2] * Wmax / 2 * 256, ext[3] * (H / W) * Wmax / 2 * 256)
+    print("%s: |x_ndc| <= %.1f, |y_ndc| <= %.1f (128 x 72): |s| <= 2^%.2f, |ds| <= 2^%.2f at %d x %d" % (scenario, ext[0], ext[1], np.log2(s_max), np.log2(ds_max), Wmax, Hmax))
+    assert s_max < ENVELOPE_S, "window coordinates of %s reach 2^%.2f sub-pixels at %d wide" % (scenario, np.log2(s_max), Wmax)
+    assert ds_max < ENVELOPE_DS, "corner differences of %s reach 2^%.2f sub-pixels at %d wide" % (scenario, np.log2(ds_max), Wmax)
