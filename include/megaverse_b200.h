@@ -153,6 +153,37 @@ int mv_final_depth_device(mv_handle h, float **d_final_depth);
  * Both calls return MV_ERR_ARG when the option is off; the device pointer is refused (MV_ERR_STATE) exactly when mv_depth_device's is. */
 int mv_segmentation_host(mv_handle h, const uint16_t **out);
 int mv_segmentation_device(mv_handle h, uint16_t **d_seg);
+/* State tensors, option "state_tensors" (0/1, before the first reset: MV_ERR_STATE after it, MV_ERR_ARG for any other value; default 0).
+ * The state behind the frames, written by the step kernel in the same call: four float32 tensors whose every value is a bit copy of an
+ * engine field (integers are stored exactly, all are below 2^24).
+ *   agents  [N][16], row env*A + agent: 0-2 MvAgent::pos; 3-6 the yaw block of the ghost basis, basis[0], basis[2], basis[6], basis[8] (the
+ *           controller's forward is normalise(b6, b7, -b8)); 7 cur_x (camera pitch, radians); 8-10 hvel; 11 vvel; 12 was_on_ground;
+ *           13 was_jumping; 14 carrying (object index, -1 = none); 15 total_reward
+ *   envs    [E][16]: 0 episode_sec; 1 episode_len of the live level; 2 num_frames; 3 scenario (MV_SCENARIO_*); 4 n_obj; 5 n_reward; 6 solved;
+ *           7 reached_exit; 8 highest_tower; 9 bz_reward; 10 positive_collected; 11-15 0
+ *   objects [E][128][4] (MV_MAX_OBJECTS): rows < n_obj: world position x, y, z -- the translation column of the model matrix the object is
+ *           drawn with, ((agent * camera) * pickup) * local for a carried one, as mv_debug_get_state reports it -- then the carrier
+ *           (MvObject::parent: agent index, -1 when not carried); rows beyond are 0
+ *   rewards [E][128][4] (MV_MAX_REWARD): rows < n_reward: the translation of the reward object's root matrix, then 0 once it is collected,
+ *           else -1 for a penalising object (Collect: not GREEN; HexMemory: a bad object) and +1 otherwise; rows beyond are 0
+ * A row shows the state the returned frame shows: for an env that ended in the call, the new episode's first.  Inactive envs (mv_step_envs,
+ * mv_step_device_active) keep their rows; mv_reset and mv_reset_envs write the restarted envs' rows; mv_states_load restores the saved
+ * step's rows (the state store carries them: mv_state_row_bytes grows by 64 * A + 4 160 bytes with the option on); mv_debug_warp_agent
+ * changes no row until the next call.  With option final_obs as well, an env that ends in a step gets terminal rows in four more tensors of
+ * the same shapes: the state after the ending tick, before the flip -- the state its terminal frame shows.  Other rows are left alone.
+ * Delivery follows the observations: host-facing calls (mv_step, mv_step_envs, mv_step_begin/end, mv_reset, mv_reset_envs, mv_states_load)
+ * return with every tensor in pinned host memory (one copy of the whole block, on a copy stream while the frames are drawn);
+ * mv_step_device* leaves them in HBM in stream order, and mv_fetch_obs copies them down.  Nothing else changes with the option: obs,
+ * depth, segmentation, rewards, dones, reasons, true objectives, terminal frames and level ids are byte-identical with it on and off.
+ * Memory: 64 * A + 4 160 B per env in HBM and again pinned (4.5 MB each at 1 024 envs x 4 agents), twice that with final_obs; nothing is
+ * allocated while the option is off.  Any out pointer may be NULL.  MV_ERR_ARG for a null handle and while the option (or, for the
+ * terminal rows, option final_obs) is off; MV_ERR_STATE before mv_reset. */
+#define MV_STATE_OBJECT_ROWS 128
+#define MV_STATE_REWARD_ROWS 128
+int mv_state_tensors_host(mv_handle h, const float **agents, const float **envs, const float **objects, const float **rewards);
+int mv_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards);
+int mv_final_state_tensors_host(mv_handle h, const float **agents, const float **envs, const float **objects, const float **rewards);
+int mv_final_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards);
 
 /* MegaverseGym::getRewardShaping / setRewardShaping (megaverse.cpp:214-222).  get: fills up to cap entries, returns the
  * number of keys in *n.  Key strings are owned by the engine. */
@@ -183,6 +214,7 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * "final_obs" (0/1, before the first reset, default 0: terminal frames of ended episodes, see mv_final_obs_host),
  * "segmentation" (0/1, before the first reset, default 0: the class and index of the drawable behind every pixel, see
  * mv_segmentation_host),
+ * "state_tensors" (0/1, before the first reset, default 0: agent, env, object and reward rows beside the frames, see mv_state_tensors_host),
  * "action_repeat" (1..4, before the first reset (MV_ERR_STATE after it, MV_ERR_ARG outside the range), default 1: action repeat, or
  * frame skip, inside the engine.  Every step call (mv_step, mv_step_begin/end, mv_step_device[_ends]) runs up to k physics ticks of
  * 1/15 s per env with the same action masks, then draws once.  Interact acts on the first tick only (it toggles carrying, so one call

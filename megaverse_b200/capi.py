@@ -72,6 +72,8 @@ def lib():
         L.mv_set_next_levels.argtypes = [vp, vp, vp, ci]
         L.mv_level_set_pick.argtypes = [C.c_uint32, C.c_int32, C.c_int32]
         L.mv_level_set_pick.restype = C.c_uint32
+        for name in ("mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device"):
+            getattr(L, name).argtypes = [vp] + [C.POINTER(vp)] * 4
         _lib = L
     return _lib
 
@@ -86,7 +88,10 @@ EXPORTS = [
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
     "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device", "mv_step_envs", "mv_step_device_active",
     "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device", "mv_set_next_levels", "mv_level_set_pick",
+    "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
 ]
+
+STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
 
 
 class Engine:
@@ -205,14 +210,23 @@ class Engine:
         (`torch.as_tensor(eng.device_array("obs"), device="cuda")`, CuPy, Numba): "obs" uint8[N,h,w,4], "depth" float32[N,h,w],
         "rewards" float32[N], "dones" uint8[E], "done_reasons" uint8[E] (MV_END_*), "true_objectives" float32[N], with option final_obs
         "final_obs" uint8[N,h,w,4] / "final_depth" float32[N,h,w] (terminal frames of mv_step_device steps), and with option segmentation
-        "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index), and with option level_set "level_ids" int32[E] (the level each env is on) and
+        "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index), with option state_tensors "state_agents" float32[N,16], "state_envs"
+        float32[E,16], "state_objects" / "state_rewards" float32[E,128,4] and, with option final_obs too, the terminal rows "final_state_agents",
+        ... (state_tensors()), and with option level_set "level_ids" int32[E] (the level each env is on) and
         "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream).  Valid in the engine stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
                   "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
                   "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4")}
+        for prefix in ("state_", "final_state_"):
+            for k, shp in self._state_shapes().items():
+                shapes[prefix + k] = (shp, "<f4")
         shape, typestr = shapes[what]
-        ptr, stream = self.device_ptr(what), self.stream()
+        if what.startswith(("state_", "final_state_")):
+            ptr = self._state_ptrs("mv_%s_tensors_device" % what.rsplit("_", 1)[0])[what.rsplit("_", 1)[1]]
+        else:
+            ptr = self.device_ptr(what)
+        stream = self.stream()
 
         class _DeviceArray:
             __cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None, "stream": stream or 1}
@@ -262,6 +276,31 @@ class Engine:
         e, lv = np.ascontiguousarray(envs, dtype=np.int32), np.ascontiguousarray(levels, dtype=np.int32)
         assert e.size == lv.size
         self._ck(lib().mv_set_next_levels(self._h, e.ctypes.data if e.size else None, lv.ctypes.data if lv.size else None, e.size))
+
+    def _state_shapes(self):
+        return {"agents": (self.N, 16), "envs": (self.E, 16), "objects": (self.E, 128, 4), "rewards": (self.E, 128, 4)}
+
+    def _state_ptrs(self, fn):
+        p = [C.c_void_p() for _ in STATE_TENSORS]
+        self._ck(getattr(lib(), fn)(self._h, *[C.byref(x) for x in p]))
+        return {k: x.value for k, x in zip(STATE_TENSORS, p)}
+
+    def _state_views(self, fn):
+        shapes = self._state_shapes()
+        out = {}
+        for k, ptr in self._state_ptrs(fn).items():
+            n = int(np.prod(shapes[k])) * 4
+            out[k] = np.frombuffer((C.c_char * n).from_address(ptr), dtype=np.float32).reshape(shapes[k])
+        return out
+
+    def state_tensors(self):
+        """option state_tensors: {"agents": float32[N,16], "envs": float32[E,16], "objects": float32[E,128,4], "rewards": float32[E,128,4]},
+        views of the engine's pinned rows after the last host-facing call (or mv_fetch_obs); the layout is in include/megaverse_b200.h"""
+        return self._state_views("mv_state_tensors_host")
+
+    def final_state_tensors(self):
+        """options state_tensors and final_obs: the same dict of terminal rows, the state each env's last episode ended on"""
+        return self._state_views("mv_final_state_tensors_host")
 
     def final_obs(self):
         """uint8[N,h,w,4] terminal frames (option final_obs): views of env e hold the frame its last episode ended on"""

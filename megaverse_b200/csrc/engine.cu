@@ -144,6 +144,7 @@ enum { kSlabInst = 4, kSlabStatics = 8, kSlabStaticRot = 9, kSlabCount = 17 };
 struct StateStore {
     int rows = 0;
     DevBuf<uint8_t> slabs[kSlabCount];  // same order as mv_engine::envSlabs()
+    DevBuf<uint8_t> stateSlabs[4];      // option state_tensors: the live rows of the four state tensors (mv_engine::stateTensor order)
     struct HostRow {
         bool saved = false;
         std::optional<mv::LevelGenerator> gen;  // the env's level stream; empty with a level set (the bank is the engine's, the pick is in MvEnvState)
@@ -158,12 +159,13 @@ struct StateStore {
         std::vector<std::vector<uint32_t>> solid;  // the three bit planes, levelWords words each
     };
     std::vector<HostRow> host;
-    void free() { for (auto &s : slabs) s.free(); }
+    void free() { for (auto &s : slabs) s.free(); for (auto &s : stateSlabs) s.free(); }
 };
 
 }  // namespace
 
 static void fillConsts(MvConsts &k, int W, int H);
+static_assert(MV_STATE_OBJECT_ROWS == MV_MAX_OBJECTS && MV_STATE_REWARD_ROWS == MV_MAX_REWARD, "state tensor rows");
 
 // the frame part of a raster launch: frame size, row bands of bandRows rows, the per-CTA spill slab (one band of the frame per CTA), the
 // triangle-list capacity and the projection of k; the rest is zero (no stats, no ready stamps, no mask, natural order)
@@ -380,6 +382,38 @@ struct mv_engine {
     PinBuf<uint8_t> h_finalObs;
     PinBuf<float> h_finalDepth;
 
+    // state tensors (option "state_tensors", allocated at the first reset): the step kernel writes every stepped env's rows (layout in the
+    // header) into one HBM block, agents [N][16], envs [E][16], objects [E][MV_MAX_OBJECTS][4], rewards [E][MV_MAX_REWARD][4], followed
+    // with option final_obs by the terminal rows in the same four shapes.  A host-facing call copies the whole block into its pinned twin
+    // on copyStream while the frames are drawn; mv_step_device leaves it in HBM (mv_fetch_obs copies it down).
+    bool wantState = false;
+    bool stateCopyPending = false;  // this call's block download is on copyStream
+    cudaEvent_t evState = nullptr;  // the step kernel's rows are written: the download may start
+    DevBuf<float> d_state;
+    PinBuf<float> h_state;
+    size_t stateFloats() const { return size_t(N) * 16 + size_t(E) * (16 + 4 * MV_MAX_OBJECTS + 4 * MV_MAX_REWARD); }
+    size_t stateBlockFloats() const { return stateFloats() * (wantFinal ? 2 : 1); }
+    // tensor k (0 agents, 1 envs, 2 objects, 3 rewards) of the live rows, or of the terminal rows
+    float *stateTensor(float *block, int k, bool terminal) const {
+        if (!block) return nullptr;
+        const size_t off[4] = {0, size_t(N) * 16, size_t(N) * 16 + size_t(E) * 16, size_t(N) * 16 + size_t(E) * (16 + 4 * MV_MAX_OBJECTS)};
+        return block + (terminal ? stateFloats() : 0) + off[k];
+    }
+    // bytes per env of tensor k (the state store's slabs)
+    size_t stateRowBytes(int k) const {
+        const size_t b[4] = {sizeof(float) * 16 * size_t(A), sizeof(float) * 16, sizeof(float) * 4 * MV_MAX_OBJECTS, sizeof(float) * 4 * MV_MAX_REWARD};
+        return b[k];
+    }
+    // host-facing calls: the block into its pinned twin on copyStream, behind everything enqueued on the stream so far
+    int downloadState() {
+        if (!wantState) return MV_OK;
+        MV_CUDA(cudaEventRecord(evState, stream));
+        MV_CUDA(cudaStreamWaitEvent(copyStream, evState, 0));
+        MV_CUDA(cudaMemcpyAsync(h_state.p, d_state.p, sizeof(float) * stateBlockFloats(), cudaMemcpyDeviceToHost, copyStream));
+        stateCopyPending = true;
+        return MV_OK;
+    }
+
     // ------------------------------------------------------------------ level generation scheduling
     // generate the level for episode `serial` of env e into staging slot s, after every job scheduled for the env before
     void scheduleGen(int e, int s, int serial) {
@@ -592,6 +626,10 @@ struct mv_engine {
         sp.hostLevelIds = (mirror && levelSet) ? mirror->levelIds.p : nullptr;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
+        float *st = wantState ? d_state.p : nullptr, *termSt = wantFinal ? st : nullptr;
+        sp.stAgents = stateTensor(st, 0, false); sp.stEnvs = stateTensor(st, 1, false); sp.stObjects = stateTensor(st, 2, false); sp.stRewards = stateTensor(st, 3, false);
+        sp.termStAgents = stateTensor(termSt, 0, true); sp.termStEnvs = stateTensor(termSt, 1, true); sp.termStObjects = stateTensor(termSt, 2, true);
+        sp.termStRewards = stateTensor(termSt, 3, true);
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
         sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = gridWords; sp.forceReset = forceReset ? 1 : 0;
         sp.k = consts;
@@ -602,7 +640,9 @@ struct mv_engine {
         const int warpsPerBlock = 2;
         const int blocks = (sp.E + warpsPerBlock - 1) / warpsPerBlock;
         const size_t smem = sizeof(mvk::WarpShared) * warpsPerBlock;
-        if (sp.levelSet) mvk::stepKernel<true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        if (sp.levelSet && sp.stAgents) mvk::stepKernel<true, true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        else if (sp.levelSet) mvk::stepKernel<true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        else if (sp.stAgents) mvk::stepKernel<false, true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         else mvk::stepKernel<false><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
         launches += 1;
@@ -618,7 +658,11 @@ struct mv_engine {
         if (timed) MV_CUDA(cudaEventRecord(ev[0], stream));
         if (const int rc = launchStepKernel(sp)) return rc;
         if (timed && !dep) MV_CUDA(cudaEventRecord(ev[1], stream));  // an event between the two kernels would serialise them
+        // host-facing: the state block goes down while the frames are drawn -- or, behind a programmatic dependent raster launch, while its
+        // terminal frames are (the event the download waits for would serialise the two kernels)
+        if (!async && !dep) { if (const int rc = downloadState()) return rc; }
         if (const int rc = launchRaster(dep, sp.active)) return rc;
+        if (!async && dep) { if (const int rc = downloadState()) return rc; }
         if (final) {  // after the step's own frames: the terminal frames of the envs that ended (stream order, no stamps)
             if (timed) MV_CUDA(cudaEventRecord(evFinal, stream));
             if (const int rc = launchFinal(!async)) return rc;
@@ -847,7 +891,8 @@ struct mv_engine {
     // the end of a host-facing call: its stream and the slice downloads drained, then its kernel times
     int waitHostStep() {
         MV_CUDA(cudaStreamSynchronize(stream));
-        if (sliceCount > 1) MV_CUDA(cudaStreamSynchronize(copyStream));
+        if (sliceCount > 1 || stateCopyPending) MV_CUDA(cudaStreamSynchronize(copyStream));
+        stateCopyPending = false;
         readKernelTimes();
         return MV_OK;
     }
@@ -980,6 +1025,7 @@ struct mv_engine {
     size_t stateRowBytes() {
         size_t b = 0;
         for (const EnvSlab &s : envSlabs()) b += s.rowBytes();
+        for (int k = 0; k < 4 && wantState; ++k) b += stateRowBytes(k);
         return b;
     }
     int statesCreate(int rows, int *id) {
@@ -988,6 +1034,8 @@ struct mv_engine {
         const auto sl = envSlabs();
         for (int k = 0; k < kSlabCount; ++k)
             if (st->slabs[k].alloc(size_t(rows) * sl[size_t(k)].rowBytes()) != cudaSuccess) { st->free(); setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
+        for (int k = 0; k < 4 && wantState; ++k)
+            if (st->stateSlabs[k].alloc(size_t(rows) * stateRowBytes(k)) != cudaSuccess) { st->free(); setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
         st->host.resize(size_t(rows));
         stores.push_back(std::move(st));
         *id = int(stores.size()) - 1;
@@ -1019,7 +1067,18 @@ struct mv_engine {
         MV_CUDA(cudaEventRecord(ev[0], stream));
         MV_CUDA(mvs::copyRows(table, kSlabCount, d_pairs.p, n, stream));
         launches += 1;
+        if (wantState) {  // the state-tensor rows: a second launch of the same kernel, so that its table keeps its size
+            mvs::Slab stTable[4];
+            for (int k = 0; k < 4; ++k) {
+                uint8_t *eng = reinterpret_cast<uint8_t *>(stateTensor(d_state.p, k, false)), *sto = st.stateSlabs[k].p;
+                const size_t rb = stateRowBytes(k);
+                stTable[k] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
+            }
+            MV_CUDA(mvs::copyRows(stTable, 4, d_pairs.p, n, stream));
+            launches += 1;
+        }
         if (toStore) return endTimes(Timed::FirstOnly);
+        if (const int rc = downloadState()) return rc;  // the loaded rows, while the views are drawn again
         MV_CUDA(cudaEventRecord(ev[1], stream));
         const int rc = launchRaster(false, nullptr);
         return rc ? rc : endTimes(Timed::Split);
@@ -1208,6 +1267,8 @@ struct mv_engine {
         h_faults.free(); h_faultWord.free();
         d_doneReasons.free(); h_doneReasons.free();
         d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
+        d_state.free(); h_state.free();
+        if (evState) { cudaEventDestroy(evState); evState = nullptr; }
         for (auto &e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
         if (evFinal) { cudaEventDestroy(evFinal); evFinal = nullptr; }
         for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); p.levelIds.free(); }
@@ -1238,6 +1299,8 @@ int uploadPalette(mv_engine *h) {
 int setKernelAttrs(mv_engine *h) {
     cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
     if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
     if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
     return MV_OK;
 }
@@ -1428,6 +1491,12 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         h->wantFinal = value != 0;
         return MV_OK;
     }
+    if (k == "state_tensors") {  // agent / env / object / reward rows beside the frames (see the header); allocated by the first reset
+        if (h->didReset) { h->setError("option state_tensors must be set before the first reset"); return MV_ERR_STATE; }
+        if (value != 0 && value != 1) { h->setError("state_tensors must be 0 or 1"); return MV_ERR_ARG; }
+        h->wantState = value != 0;
+        return MV_OK;
+    }
     if (k == "action_repeat") {  // physics ticks per step call (see the header); the state store keeps no copy: it belongs to the engine
         if (h->didReset) { h->setError("option action_repeat must be set before the first reset"); return MV_ERR_STATE; }
         if (value < 1 || value > 4) { h->setError("action_repeat out of range [1,4]"); return MV_ERR_ARG; }
@@ -1559,6 +1628,16 @@ int mv_reset(mv_handle h) {
             }
             std::memset(h->h_finalObs.p, 0, N * px * 4);
             if (h->wantDepth) std::memset(h->h_finalDepth.p, 0, sizeof(float) * N * px);
+        }
+        if (h->wantState) {  // the live rows and, with final_obs, the terminal rows: one block, zero until written
+            const size_t n = h->stateBlockFloats();
+            if (h->d_state.alloc(n) != cudaSuccess || h->h_state.alloc(n) != cudaSuccess || cudaMemset(h->d_state.p, 0, sizeof(float) * n) != cudaSuccess ||
+                cudaEventCreateWithFlags(&h->evState, cudaEventDisableTiming) != cudaSuccess) {
+                h->d_state.free(); h->h_state.free();
+                h->setError("state_tensors: allocation failed");
+                return MV_ERR_CUDA;
+            }
+            std::memset(h->h_state.p, 0, sizeof(float) * n);
         }
         if (h->levelSet) h->scheduleBank();
         else regenerateNext(h);
@@ -1833,6 +1912,12 @@ int mv_fetch_obs(mv_handle h) {
         if (cudaMemcpyAsync(h->h_finalObs.p, h->d_finalObs.p, px * 4, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("final obs download failed"); return MV_ERR_CUDA; }
         if (h->wantDepth && cudaMemcpyAsync(h->h_finalDepth.p, h->d_finalDepth.p, px * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) { h->setError("final depth download failed"); return MV_ERR_CUDA; }
     }
+    // the state tensors (live and terminal rows): always current in HBM
+    if (h->wantState && h->didReset &&
+        cudaMemcpyAsync(h->h_state.p, h->d_state.p, sizeof(float) * h->stateBlockFloats(), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) {
+        h->setError("state tensor download failed");
+        return MV_ERR_CUDA;
+    }
     // after a zero-copy host-facing step the host buffer holds the newer frames: no copy.  Rows copied from a caller's tensor are not the
     // engine's to vouch for: the next step with an active set draws every view again
     if (h->deviceObsFresh) {
@@ -1904,6 +1989,42 @@ int mv_final_depth_device(mv_handle h, float **p) {
     if (!h || !p) return MV_ERR_ARG;
     const int rc = finalBuffer(h, true, "mv_final_depth_device");
     if (rc == MV_OK) *p = h->d_finalDepth.p;
+    return rc;
+}
+// option state_tensors (and final_obs, for the terminal rows) is on and the engine reset
+static int stateTensorCall(mv_handle h, bool terminal, const char *fn) {
+    if (!h) return MV_ERR_ARG;
+    if (!h->wantState || (terminal && !h->wantFinal)) {
+        h->setError(std::string(fn) + ": option state_tensors" + (terminal ? " or option final_obs is" : " is") + " off");
+        return MV_ERR_ARG;
+    }
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+// the four tensors of the live or terminal rows in `block` into the non-null outs
+static void stateTensorOuts(mv_handle h, float *block, bool terminal, float **agents, float **envs, float **objects, float **rewards) {
+    float **outs[4] = {agents, envs, objects, rewards};
+    for (int k = 0; k < 4; ++k)
+        if (outs[k]) *outs[k] = h->stateTensor(block, k, terminal);
+}
+int mv_state_tensors_host(mv_handle h, const float **agents, const float **envs, const float **objects, const float **rewards) {
+    const int rc = stateTensorCall(h, false, "mv_state_tensors_host");
+    if (rc == MV_OK) stateTensorOuts(h, h->h_state.p, false, const_cast<float **>(agents), const_cast<float **>(envs), const_cast<float **>(objects), const_cast<float **>(rewards));
+    return rc;
+}
+int mv_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards) {
+    const int rc = stateTensorCall(h, false, "mv_state_tensors_device");
+    if (rc == MV_OK) stateTensorOuts(h, h->d_state.p, false, agents, envs, objects, rewards);
+    return rc;
+}
+int mv_final_state_tensors_host(mv_handle h, const float **agents, const float **envs, const float **objects, const float **rewards) {
+    const int rc = stateTensorCall(h, true, "mv_final_state_tensors_host");
+    if (rc == MV_OK) stateTensorOuts(h, h->h_state.p, true, const_cast<float **>(agents), const_cast<float **>(envs), const_cast<float **>(objects), const_cast<float **>(rewards));
+    return rc;
+}
+int mv_final_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards) {
+    const int rc = stateTensorCall(h, true, "mv_final_state_tensors_device");
+    if (rc == MV_OK) stateTensorOuts(h, h->d_state.p, true, agents, envs, objects, rewards);
     return rc;
 }
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth) {

@@ -260,6 +260,20 @@ public:
         check(mv_level_ids(h__, &ids));
         return py::array_t<int32_t>({numEnvs_}, ids, py::none{});
     }
+    // (extension, option "state_tensors") {"agents": [N,16], "envs": [E,16], "objects": [E,128,4], "rewards": [E,128,4]}, views of the
+    // engine's pinned rows (layout in the header); the terminal rows with option final_obs as well
+    py::dict getStateTensors(bool terminal) {
+        alive();
+        const float *p[4];
+        check(terminal ? mv_final_state_tensors_host(h__, &p[0], &p[1], &p[2], &p[3]) : mv_state_tensors_host(h__, &p[0], &p[1], &p[2], &p[3]));
+        py::dict d;
+        const int N = int(masks_.size());
+        d["agents"] = py::array_t<float>({N, 16}, p[0], py::none{});
+        d["envs"] = py::array_t<float>({numEnvs_, 16}, p[1], py::none{});
+        d["objects"] = py::array_t<float>({numEnvs_, MV_STATE_OBJECT_ROWS, 4}, p[2], py::none{});
+        d["rewards"] = py::array_t<float>({numEnvs_, MV_STATE_REWARD_ROWS, 4}, p[3], py::none{});
+        return d;
+    }
     void setNextLevels(const std::vector<int32_t> &envs, const std::vector<int32_t> &levels) {
         alive();
         if (envs.size() != levels.size()) throw std::invalid_argument("set_next_levels: envs and levels differ in length");
@@ -325,6 +339,10 @@ PYBIND11_MODULE(megaverse, m) {
         .def("level_ids", &MegaverseGym::getLevelIds, "int32[num_envs] (option level_set): the level of the set each env is on; after an end, the new episode's")
         .def("set_next_levels", &MegaverseGym::setNextLevels, py::arg("envs"), py::arg("levels"),
              "(option level_set) env envs[i] plays level levels[i] in its next episode, once; followed by reset_envs(envs) it starts them on those levels now")
+        .def("get_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(false); },
+             "dict of float32 views (option state_tensors): agents [N,16], envs [E,16], objects [E,128,4], rewards [E,128,4]")
+        .def("get_final_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(true); },
+             "the terminal rows (options state_tensors and final_obs): the state each env's last episode ended on, same dict")
         .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),
              "step the listed envs only: the others run nothing, report reward 0 and done 0, and keep their observations");
 }

@@ -92,6 +92,12 @@ struct StepParams {
     int32_t *termCounts;
     float *termViews;
     MvConsts k;
+    // option "state_tensors" (nullptr: off; the stepKernel<.., true> variants only): the caller-facing rows of every env stepped, float32
+    // bit copies of its state after the call (include/megaverse_b200.h has the layout): agents [E*A][16], envs [E][16], objects
+    // [E][MV_MAX_OBJECTS][4], rewards [E][MV_MAX_REWARD][4].  The term* rows (with option final_obs as well) get the state an ending
+    // env's terminal frame shows.
+    float *stAgents, *stEnvs, *stObjects, *stRewards;
+    float *termStAgents, *termStEnvs, *termStObjects, *termStRewards;
 };
 
 // row of the level arrays that holds slot `slot` of env `env`: the env's own ring of slots, or, with a level set, the bank row itself
@@ -892,10 +898,78 @@ __device__ void writeInstances(const WarpShared &S, const MvLevel &L, const MvBo
     (void)no;
 }
 
+// ---------------------------------------------------------------- state tensors (option "state_tensors")
+// One env's rows, from the warp's state and the instance list `inst` that writeInstances has just written (its writes are visible to
+// the warp after a __syncwarp).  An object's position is the translation column of its instance's model matrix, so a carried object is
+// where it is drawn.  `all`: every object and reward row (an episode start, a terminal row); otherwise only the objects writeInstances
+// rewrote (carried, or picked up / put down / pushed in this call) and the rewards collected in this call -- no other row can have changed.
+__device__ float stateRewardValue(const WarpShared &S, const MvLevel &L, int i) {
+    if (!((S.env.reward_alive[i >> 5] >> (i & 31)) & 1u)) return 0.0f;
+    const bool penalty = L.scenario == MV_SCENARIO_COLLECT ? L.reward_voxel[i][3] != 1  // not GREEN
+                                                          : (L.scenario == MV_SCENARIO_HEX_MEMORY && !((L.reward_good[i >> 5] >> (i & 31)) & 1u));
+    return penalty ? -1.0f : 1.0f;
+}
+__device__ void writeStateRows(const WarpShared &S, const MvLevel &L, const MvInstance *inst, int A, bool all, float *ag, float *en, float *ob, float *rw, int lane) {
+    for (int w = lane; w < A * 16; w += 32) {
+        const MvAgent &a = S.agents[w >> 4];
+        const int c = w & 15;
+        float v;
+        if (c < 3) v = a.pos[c];
+        else if (c < 7) v = a.basis[c == 3 ? 0 : (c == 4 ? 2 : (c == 5 ? 6 : 8))];
+        else if (c == 7) v = a.cur_x;
+        else if (c < 11) v = a.hvel[c - 8];
+        else if (c == 11) v = a.vvel;
+        else if (c == 12) v = float(a.was_on_ground);
+        else if (c == 13) v = float(a.was_jumping);
+        else if (c == 14) v = float(a.carrying);
+        else v = a.total_reward;
+        ag[w] = v;
+    }
+    if (lane < 16) {
+        const MvEnvState &e = S.env;
+        const float v[11] = {e.episode_sec, L.episode_len, float(e.num_frames), float(L.scenario), float(L.n_obj), float(L.n_reward), float(e.solved),
+                             float(e.reached_exit), float(e.highest_tower), e.bz_reward, float(e.positive_collected)};
+        en[lane] = lane < 11 ? v[lane] : 0.0f;
+    }
+    auto objectRow = [&](int i, float *row) {
+        const MvObject &o = S.objects[i];
+        const float *m = inst[MV_OBJ_SLOT(o.meta)].model;
+        row[0] = m[12]; row[1] = m[13]; row[2] = m[14]; row[3] = float(o.parent);
+    };
+    auto rewardRow = [&](int i, float *row) {
+        row[0] = L.reward_root[i][12]; row[1] = L.reward_root[i][13]; row[2] = L.reward_root[i][14]; row[3] = stateRewardValue(S, L, i);
+    };
+    if (all) {
+        for (int i = lane; i < MV_MAX_OBJECTS; i += 32) {
+            float4 *row = reinterpret_cast<float4 *>(ob) + i;
+            if (i < L.n_obj) { float r[4]; objectRow(i, r); *row = make_float4(r[0], r[1], r[2], r[3]); }
+            else *row = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        }
+        for (int i = lane; i < MV_MAX_REWARD; i += 32) {
+            float4 *row = reinterpret_cast<float4 *>(rw) + i;
+            if (i < L.n_reward) { float r[4]; rewardRow(i, r); *row = make_float4(r[0], r[1], r[2], r[3]); }
+            else *row = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        }
+        return;
+    }
+    for (int idx = lane; idx < A + S.nDirty; idx += 32) {
+        const int i = idx < A ? S.agents[idx].carrying : S.objDirty[idx - A];
+        if (i < 0) continue;
+        float r[4]; objectRow(i, r);
+        reinterpret_cast<float4 *>(ob)[i] = make_float4(r[0], r[1], r[2], r[3]);
+    }
+    for (int i = lane; i < L.n_reward; i += 32) {
+        if (!((S.rewardDirty[i >> 5] >> (i & 31)) & 1u)) continue;
+        float r[4]; rewardRow(i, r);
+        reinterpret_cast<float4 *>(rw)[i] = make_float4(r[0], r[1], r[2], r[3]);
+    }
+}
+
 // ---------------------------------------------------------------- the kernel
 // kLevelSet: the level-set variant (StepParams::levelSet > 0).  A template parameter, not a run-time branch, so that the default
-// variant is the code it was before level sets existed
-template <bool kLevelSet> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
+// variant is the code it was before level sets existed.  kState: the state-tensor variant (StepParams::stAgents set), a template
+// parameter for the same reason
+template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     extern __shared__ __align__(128) unsigned char smemRaw[];
     const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slotInGrid = blockIdx.x * (blockDim.x >> 5) + warpInBlock;
@@ -1507,6 +1581,11 @@ template <bool kLevelSet> __global__ void __launch_bounds__(128) stepKernel(Step
         __syncwarp();
         writeInstances(S, *L, statics, P.deco + levelRow<kLevelSet>(P, env, slot) * P.decoCap, tInst, tCounts, tViews, A, /*writeStatic=*/false, lane);
         __syncwarp();
+        if (kState && P.termStAgents) {  // the state this terminal frame shows: after the ending tick, before the flip
+            writeStateRows(S, *L, tInst, A, /*all=*/true, P.termStAgents + size_t(env) * A * 16, P.termStEnvs + size_t(env) * 16,
+                           P.termStObjects + size_t(env) * MV_MAX_OBJECTS * 4, P.termStRewards + size_t(env) * MV_MAX_REWARD * 4, lane);
+            __syncwarp();
+        }
     }
 
     if (resetNow) {
@@ -1560,6 +1639,11 @@ template <bool kLevelSet> __global__ void __launch_bounds__(128) stepKernel(Step
     writeInstances(S, *L, statics, P.deco + levelRow<kLevelSet>(P, env, slot) * P.decoCap, P.instances + size_t(env) * P.instStride, P.instCounts + size_t(env) * 8, P.views + size_t(env) * A * 16, A, resetNow, lane);
 
     MV_PROBE(7);  // instance list + views
+    if (kState) {  // the rows of the state the returned frame shows: after an end, the new episode's first
+        __syncwarp();
+        writeStateRows(S, *L, P.instances + size_t(env) * P.instStride, A, resetNow, P.stAgents + size_t(env) * A * 16, P.stEnvs + size_t(env) * 16,
+                       P.stObjects + size_t(env) * MV_MAX_OBJECTS * 4, P.stRewards + size_t(env) * MV_MAX_REWARD * 4, lane);
+    }
 
     // ---- commit env + agents
     {

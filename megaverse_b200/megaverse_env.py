@@ -70,7 +70,7 @@ class MegaverseEnv(Env):
     SKIP_UNFIT_LEVELS = False
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
-                 action_repeat=1, segmentation=False, num_levels=None, start_level=0):
+                 action_repeat=1, segmentation=False, num_levels=None, start_level=0, state_tensors=False):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
@@ -81,6 +81,9 @@ class MegaverseEnv(Env):
         # (extension) num_levels=L, start_level=s (Procgen's names): the envs play a fixed set of L levels per scenario, the first levels of
         # the generators seeded s .. s + L - 1, kept on the GPU (option "level_set").  level_ids() tells which level each env is on,
         # set_next_levels() chooses an env's next one, and the infos of done agents carry 'level', the level the finished episode was played on
+        # (extension) state_tensors=True: state_tensors() gives the state behind the current frames (agents, envs, objects, rewards; option
+        # "state_tensors"), and with final_observation=True the infos of done agents carry 'final_state', the agent's row of the state the
+        # episode ended on
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -117,6 +120,9 @@ class MegaverseEnv(Env):
         self.segmentation_enabled = bool(segmentation)
         if self.segmentation_enabled:
             self.env.set_option("segmentation", 1)
+        self.state_tensors_enabled = bool(state_tensors)
+        if self.state_tensors_enabled:
+            self.env.set_option("state_tensors", 1)
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
         self.num_levels = None if num_levels is None else int(num_levels)
@@ -156,6 +162,12 @@ class MegaverseEnv(Env):
         drawable behind each pixel of the current frame, 0 where nothing was drawn.  Views of engine memory, valid until the next step."""
         seg = self.env.get_segmentation()
         return [seg[i] for i in range(self.num_agents)]
+
+    def state_tensors(self):
+        """(extension, state_tensors=True) {"agents": float32[num_agents, 16], "envs": float32[num_envs, 16], "objects": float32[num_envs, 128, 4],
+        "rewards": float32[num_envs, 128, 4]}: the state the current observations show, rows as in include/megaverse_b200.h.  Views of engine
+        memory, valid until the next step."""
+        return self.env.get_state_tensors()
 
     def check_faults(self):
         """raise if the engine latched a fault bit (one pinned-memory read, no device round trip)"""
@@ -203,6 +215,7 @@ class MegaverseEnv(Env):
         if self.final_observation:
             reasons = self.env.get_done_reasons()
             final = self.env.get_final_observations()
+            final_state = self.env.get_final_state_tensors()['agents'] if self.state_tensors_enabled else None
         dones, infos = [], []
         for env_i in range(self.num_envs):
             done = bool(env_dones[env_i])
@@ -219,6 +232,8 @@ class MegaverseEnv(Env):
                         infos[view]['final_observation'] = np.ascontiguousarray(np.transpose(final[view, :, :, :3], (2, 0, 1)))
                         infos[view]['terminated'] = int(reasons[env_i]) == 2
                         infos[view]['truncated'] = int(reasons[env_i]) in (1, 3)
+                        if final_state is not None:
+                            infos[view]['final_state'] = final_state[view].copy()
             else:
                 infos.extend([{} for _ in range(self.num_agents_per_env)])
 
