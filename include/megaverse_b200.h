@@ -290,6 +290,41 @@ int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth);
  * valid until the next mv_draw_hires / mv_close */
 int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out);
 int mv_sync(mv_handle h);
+/* Spectator cameras: draw chosen envs from caller-placed viewpoints with the step's rasteriser.  Camera c of n draws the instance list of env
+ * envs[c] through the view matrix views16[c * 16 .. c * 16 + 16) (column-major, world to camera, the convention of mv_debug_get_view: the
+ * camera looks down -z with y up; megaverse_b200/cameras.py builds them) into frame c: RGBA uint8[n][h][w][4], and on request view-space
+ * depth float[n][h][w] and segmentation uint16[n][h][w] (MV_SEG_* << 8 | index).  The projection is the agents' at that size (100 degree
+ * horizontal field of view); sizes follow mv_draw_hires: multiples of 32 x 4 up to 768 x 4096.  Neither option "depth" nor option
+ * "segmentation" is needed.
+ * Both calls draw the instance lists of the last completed step -- the state the observations show -- after active-set steps, restarts,
+ * state loads, in mixed and level-set engines alike; camera c is drawn exactly as an agent view with the same matrix and size would be
+ * (an agent's own matrix at the engine's size gives the step's frame, byte for byte, at 768 x 432 mv_draw_hires').  Neither call changes
+ * any other output or any state a later step reads.
+ * mv_draw_cameras: synchronous and host-facing.  envs and views16 are host tables; the frames land in engine-owned buffers (HBM and pinned
+ * twins, grown on demand and kept: w * h * (4 + 4 + 2) B per camera each with depth and segmentation, 3.3 MB at 768 x 432), valid until the
+ * next mv_draw_cameras or mv_close.  Any out pointer may be NULL; *depth / *seg are NULL when not requested.
+ * mv_draw_cameras_device: asynchronous.  d_envs (int32[n]), d_views16 (float[n][16]) and the outputs (d_obs required, d_depth and d_seg
+ * optional) are the caller's, in device memory.  Enqueued on the engine stream (mv_stream): between mv_step_device* calls it sees exactly
+ * the state of the step before it; it does not drain the asynchronous ring.  An entry of d_envs outside [0, num_envs) draws an all-zero frame
+ * (colour and alpha, depth, segmentation) and reads nothing.
+ * Range counter: the integer set-up is exact while snapped window coordinates stay below 2^30.5 sub-pixels and corner differences below
+ * 2^31.  Agent eyes stay inside by measurement; a caller-placed camera close to a large surface that crosses its camera plane far
+ * off-axis may not.  Every camera launch counts the projected triangles (once per camera) that leave that range: a non-zero count means
+ * some pixels of that launch may be wrong.  The host call returns it in *out_of_range; the device call gives in *d_out_of_range the
+ * engine's uint32 counter, which holds the last camera launch's count in stream order.
+ * Errors: MV_ERR_ARG for a null handle, n < 0, a null table (or, device call, a null d_obs) with n > 0, an env out of range in a host
+ * table, a bad size; MV_ERR_STATE before mv_reset or with an mv_step_begin outstanding.  A rejected call changes nothing. */
+int mv_draw_cameras(mv_handle h, const int32_t *envs, const float *views16, int n, int w, int hgt, int want_depth, int want_seg, const uint8_t **obs,
+                    const float **depth, const uint16_t **seg, uint32_t *out_of_range);
+int mv_draw_cameras_device(mv_handle h, const int32_t *d_envs, const float *d_views16, int n, int w, int hgt, uint8_t *d_obs, float *d_depth,
+                           uint16_t *d_seg, uint32_t **d_out_of_range);
+/* float[N][16] view matrices of the last step (view env*A + agent), in HBM, written by the step kernel in stream order: what chase cameras
+ * are built from without leaving the device */
+int mv_views_device(mv_handle h, float **d_views);
+/* out6 = float[num_envs][6]: {min x, y, z, max x, y, z}, the world-space bounding box of each env's live level (static boxes, decorations,
+ * terrain slabs), from the host mirrors: valid after host-facing calls and after mv_sync.  With a level set the bank row of the retired level
+ * id.  MV_ERR_ARG for a null pointer, MV_ERR_STATE before mv_reset. */
+int mv_level_bounds(mv_handle h, float *out6);
 /* after mv_step_device steps: waits, then copies the device obs (and depth and segmentation, when enabled) into the host buffers that
  * mv_obs_host / mv_depth_host / mv_segmentation_host return */
 int mv_fetch_obs(mv_handle h);
@@ -419,6 +454,10 @@ int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, 
  * from the start of the call and cover the whole call: with option "action_repeat" 1..4 and 12 are those of the last tick it ran, 5 ends
  * the tick loop */
 int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable);
+/* the cost-ordered raster queue as it stands (waits for the stream): the per-item costs of the last cost-ordered launch (N * H / 4 words,
+ * N * bands of them used), the env order of the next one (num_envs words), the exit counter (one word).  Returns the number of words, or
+ * minus that number when cap is smaller */
+int mv_debug_view_order(mv_handle h, uint32_t *out, int cap);
 /* rasteriser launch shape: out4 = {persistent grid size, CTAs per SM, dynamic shared memory per CTA in bytes, row bands per view} */
 int mv_debug_raster_config(mv_handle h, int32_t *out4);
 /* current size of the per-level static-box arrays (option "static_cap" at start, grows on demand) */

@@ -47,7 +47,8 @@ def lib():
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
                      "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device",
-                     "mv_segmentation_host", "mv_segmentation_device", "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device"):
+                     "mv_segmentation_host", "mv_segmentation_device", "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device",
+                     "mv_views_device"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
         L.mv_get_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(ci)]
         L.mv_set_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci]
@@ -74,6 +75,10 @@ def lib():
         L.mv_level_set_pick.restype = C.c_uint32
         for name in ("mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device"):
             getattr(L, name).argtypes = [vp] + [C.POINTER(vp)] * 4
+        L.mv_draw_cameras.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint32)]
+        L.mv_draw_cameras_device.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, vp, C.POINTER(vp)]
+        L.mv_level_bounds.argtypes = [vp, vp]
+        L.mv_debug_view_order.argtypes = [vp, vp, ci]
         _lib = L
     return _lib
 
@@ -89,9 +94,23 @@ EXPORTS = [
     "mv_final_depth_device", "mv_last_final_ms", "mv_segmentation_host", "mv_segmentation_device", "mv_step_envs", "mv_step_device_active",
     "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device", "mv_set_next_levels", "mv_level_set_pick",
     "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
+    "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
+
+
+class CameraFrames(tuple):
+    """what Engine.draw_cameras returns: (obs uint8[n,h,w,4], depth float32[n,h,w] or None, seg uint16[n,h,w] or None, out_of_range)"""
+    __slots__ = ()
+
+    def __new__(cls, obs, depth, seg, out_of_range):
+        return tuple.__new__(cls, (obs, depth, seg, out_of_range))
+
+    obs = property(lambda self: self[0])
+    depth = property(lambda self: self[1])
+    seg = property(lambda self: self[2])
+    out_of_range = property(lambda self: self[3])
 
 
 class Engine:
@@ -205,6 +224,45 @@ class Engine:
         n = self.N * h * w * 4
         return np.frombuffer((C.c_char * n).from_address(p.value), dtype=np.uint8).reshape(self.N, h, w, 4)
 
+    def draw_cameras(self, envs, views16, w, h, depth=False, seg=False):
+        """spectator cameras (mv_draw_cameras): camera c draws env envs[c] through the view matrix views16[c] (16 float32, column-major;
+        megaverse_b200.cameras builds them) at w x h from the last step's scene.  Returns CameraFrames(obs uint8[n,h,w,4], depth float32[n,h,w]
+        or None, seg uint16[n,h,w] or None, out_of_range): copies, plus the number of triangles whose window coordinates left the range the
+        rasteriser is exact in (0 means every pixel is exact)."""
+        e = np.ascontiguousarray(envs, dtype=np.int32).reshape(-1)
+        v = np.ascontiguousarray(views16, dtype=np.float32).reshape(-1)
+        assert v.size == 16 * e.size
+        n = e.size
+        po, pd, ps, wide = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint32()
+        self._ck(lib().mv_draw_cameras(self._h, e.ctypes.data if n else None, v.ctypes.data if n else None, n, int(w), int(h), int(bool(depth)),
+                                       int(bool(seg)), C.byref(po), C.byref(pd), C.byref(ps), C.byref(wide)))
+
+        def grab(ptr, shape, dtype):
+            size = int(np.prod(shape)) * np.dtype(dtype).itemsize
+            if size == 0:
+                return np.zeros(shape, dtype=dtype)
+            return np.frombuffer((C.c_char * size).from_address(ptr.value), dtype=dtype).reshape(shape).copy()
+
+        obs = grab(po, (n, h, w, 4), np.uint8)
+        dep = grab(pd, (n, h, w), np.float32) if depth else None
+        sg = grab(ps, (n, h, w), np.uint16) if seg else None
+        return CameraFrames(obs, dep, sg, int(wide.value))
+
+    def draw_cameras_device(self, d_envs_ptr, d_views_ptr, n, w, h, d_obs_ptr, d_depth_ptr=None, d_seg_ptr=None):
+        """asynchronous spectator cameras (mv_draw_cameras_device) on the engine stream: device int32[n] env table, float32[n,16] views and
+        the caller's output buffers (uint8[n,h,w,4], optional float32[n,h,w] depth and uint16[n,h,w] segmentation).  An env outside
+        [0, E) gives an all-zero frame.  Returns the device address of the engine's uint32 out-of-range counter of this launch."""
+        p = [C.c_void_p(x) if x else None for x in (d_envs_ptr, d_views_ptr, d_obs_ptr, d_depth_ptr, d_seg_ptr)]
+        ctr = C.c_void_p()
+        self._ck(lib().mv_draw_cameras_device(self._h, p[0], p[1], int(n), int(w), int(h), p[2], p[3], p[4], C.byref(ctr)))
+        return ctr.value
+
+    def level_bounds(self):
+        """float32[E,6]: {min x, y, z, max x, y, z} of each env's live level (mv_level_bounds), valid after host-facing calls and sync()"""
+        out = np.zeros((self.E, 6), dtype=np.float32)
+        self._ck(lib().mv_level_bounds(self._h, out.ctypes.data))
+        return out
+
     def device_array(self, what="obs"):
         """zero-copy handle on an engine-owned device tensor for any consumer of the CUDA array interface
         (`torch.as_tensor(eng.device_array("obs"), device="cuda")`, CuPy, Numba): "obs" uint8[N,h,w,4], "depth" float32[N,h,w],
@@ -213,11 +271,13 @@ class Engine:
         "segmentation" uint16[N,h,w] (MV_SEG_* << 8 | index), with option state_tensors "state_agents" float32[N,16], "state_envs"
         float32[E,16], "state_objects" / "state_rewards" float32[E,128,4] and, with option final_obs too, the terminal rows "final_state_agents",
         ... (state_tensors()), and with option level_set "level_ids" int32[E] (the level each env is on) and
-        "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream).  Valid in the engine stream's order (mv_stream) until mv_close."""
+        "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream), and "views"
+        float32[N,16] (the last step's view matrices, column-major: chase cameras on the device).  Valid in the engine stream's order (mv_stream)
+        until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
                   "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
-                  "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4")}
+                  "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4"), "views": ((self.N, 16), "<f4")}
         for prefix in ("state_", "final_state_"):
             for k, shp in self._state_shapes().items():
                 shapes[prefix + k] = (shp, "<f4")
@@ -434,6 +494,14 @@ class Engine:
         out = np.zeros(16, dtype=np.float32)
         self._ck(lib().mv_debug_get_view(self._h, env, agent, out.ctypes.data))
         return out
+
+    def view_order(self):
+        """uint32 words of the cost-ordered raster queue (mv_debug_view_order): item costs, the next launch's env order, the exit counter"""
+        out = np.zeros(self.N * (self.h // 4) + self.E + 1, dtype=np.uint32)
+        n = lib().mv_debug_view_order(self._h, out.ctypes.data, out.size)
+        if n < 0:
+            self._ck(n)
+        return out[:n].copy()
 
     def warp_agent(self, env, agent, pos, basis):
         """test hook (mv_debug_warp_agent): set the agent's position and basis rows, zero its velocities; drawn by the next step"""

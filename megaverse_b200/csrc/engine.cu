@@ -185,6 +185,18 @@ static mvr::ViewParams frameParams(int W, int H, int bands, int bandRows, unsign
 // differences <= 2^30.67; at 1024 the differences reach 2^31.08.
 constexpr int kMaxRasterWidth = 768;
 
+// Frames drawn beside the step's own (mv_draw_hires, the camera launches, mv_debug_render_instances_ex's default): row bands of about a
+// hundred 32x4 tiles each, so that a large frame keeps every CTA of the persistent grid busy
+static int hiresBandRows(int w) { return std::max(1, 96 / (w / 32)) * 4; }
+// the size rule of those frames: multiples of 32 x 4, at most kMaxRasterWidth x 4096
+static bool hiresSizeOk(int w, int hgt) { return w >= 32 && hgt >= 4 && w % 32 == 0 && hgt % 4 == 0 && w <= kMaxRasterWidth && hgt <= 4096; }
+// a device buffer of at least `count` elements, reallocated (contents lost) only when it is smaller
+template <typename B> static cudaError_t ensureCapacity(B &b, size_t count) {
+    if (b.p && b.n >= count) return cudaSuccess;
+    b.free();
+    return b.alloc(count);
+}
+
 // the raster kernel variant of a launch: the items it draws, whether it writes segmentation (never with terminal frames), the shading mode
 using ViewKernel = void (*)(mvr::ViewParams);
 static ViewKernel viewKernelOf(mvr::Items items, bool seg, bool fast) {
@@ -195,6 +207,9 @@ static ViewKernel viewKernelOf(mvr::Items items, bool seg, bool fast) {
     case Items::Active:
         if (seg) return fast ? viewKernel<true, Items::Active, true> : viewKernel<false, Items::Active, true>;
         return fast ? viewKernel<true, Items::Active> : viewKernel<false, Items::Active>;
+    case Items::Cameras:
+        if (seg) return fast ? viewKernel<true, Items::Cameras, true> : viewKernel<false, Items::Cameras, true>;
+        return fast ? viewKernel<true, Items::Cameras> : viewKernel<false, Items::Cameras>;
     default:
         if (seg) return fast ? viewKernel<true, Items::All, true> : viewKernel<false, Items::All, true>;
         return fast ? viewKernel<true> : viewKernel<false>;
@@ -313,6 +328,21 @@ struct mv_engine {
         DevBuf<unsigned long long> spill;
         void free() { d_obs.free(); h_obs.free(); spill.free(); W = H = 0; }
     } hires;
+    // camera launches (mv_draw_cameras[_device]): the host call's tables and output buffers, grown on demand and kept; the spill slab and
+    // the out-of-range counter serve both calls
+    struct Cameras {
+        DevBuf<int32_t> d_env; DevBuf<float> d_views;
+        DevBuf<uint8_t> d_obs; DevBuf<float> d_depth; DevBuf<uint16_t> d_seg;
+        PinBuf<uint8_t> h_obs; PinBuf<float> h_depth; PinBuf<uint16_t> h_seg;
+        DevBuf<unsigned long long> spill;
+        DevBuf<uint32_t> d_range;  // [1] triangles of the last camera launch outside the integer set-up's exact range
+        PinBuf<uint32_t> h_range;
+        void free() {
+            d_env.free(); d_views.free(); d_obs.free(); d_depth.free(); d_seg.free(); h_obs.free(); h_depth.free(); h_seg.free(); spill.free();
+            d_range.free(); h_range.free();
+        }
+    } cams;
+    int cameraGrid = 0;  // persistent grid of the camera variants
     DevBuf<MvDeco> d_deco;         // [E][D][decoCap]
     PinBuf<MvDeco> h_deco;
     int decoCap = 1, instCap = MV_DYN_INSTANCES + MV_INITIAL_STATIC_CAP + 1;
@@ -689,7 +719,7 @@ struct mv_engine {
     }
     // CTAs of a launch: the persistent grid of the kernel variant, at most option raster_grid, at most one per work item
     int rasterGridFor(const mvr::ViewParams &vp) const {
-        const int full = vp.envMask ? maskedGrid : rasterGrid;
+        const int full = vp.camEnv ? cameraGrid : (vp.envMask ? maskedGrid : rasterGrid);
         return std::min(rasterGridCap > 0 ? std::min(full, rasterGridCap) : full, vp.N * vp.bands);
     }
     // One persistent launch over all (view, band) items.  Every CTA makes exactly one failing claim when the queue is empty, so the
@@ -781,28 +811,25 @@ struct mv_engine {
     // the last step -- the same kernel over row bands of the large frame.  Result in hires.h_obs, uint8[N][h][w][4].
     int drawHires(int w, int hgt) {
         if (!didReset) { setError("mv_draw_hires before mv_reset"); return MV_ERR_STATE; }
-        if (w < 32 || hgt < 4 || (w % 32) || (hgt % 4) || w > kMaxRasterWidth || hgt > 4096) {
+        if (!hiresSizeOk(w, hgt)) {
             setError("hi-res size must be a multiple of 32 x 4, at most 768 x 4096");
             return MV_ERR_ARG;
         }
         int rc = drain();
         if (rc) return rc;
-        // bands of about a hundred 32x4 tiles each
-        const int rowsPerBand = std::max(1, 96 / (w / 32)) * 4;
-        const int bands = (hgt + rowsPerBand - 1) / rowsPerBand;
         if (hires.W != w || hires.H != hgt) {
             hires.free();
             const size_t px = size_t(N) * w * hgt * 4;
-            if (hires.d_obs.alloc(px) != cudaSuccess || hires.h_obs.alloc(px) != cudaSuccess || hires.spill.alloc(size_t(rasterGrid) * w * rowsPerBand) != cudaSuccess) {
+            if (hires.d_obs.alloc(px) != cudaSuccess || hires.h_obs.alloc(px) != cudaSuccess) {
                 hires.free();
                 setError("hi-res buffers: allocation failed");
                 return MV_ERR_CUDA;
             }
             hires.W = w; hires.H = hgt;
         }
-        MvConsts k;
-        fillConsts(k, w, hgt);
-        mvr::ViewParams vp = frameParams(w, hgt, bands, rowsPerBand, hires.spill.p, triCap, k);
+        mvr::ViewParams vp;
+        rc = bandedFrame(w, hgt, rasterGrid, hires.spill, vp);
+        if (rc) { hires.free(); return rc; }
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         vp.obs = hires.d_obs.p;
         vp.viewBase = 0; vp.N = N;
@@ -811,6 +838,100 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(hires.h_obs.p, hires.d_obs.p, size_t(N) * w * hgt * 4, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaStreamSynchronize(stream));
         return MV_OK;
+    }
+    // The frame part of a launch at w x h beside the step's own (mv_draw_hires, cameras) by a grid of `grid` CTAs: the hi-res band rule,
+    // the projection of that size, and a spill slab of one band per CTA in `spill` (grown when it is too small)
+    int bandedFrame(int w, int hgt, int grid, DevBuf<unsigned long long> &spill, mvr::ViewParams &vp) {
+        const int rowsPerBand = hiresBandRows(w);
+        const int bands = (hgt + rowsPerBand - 1) / rowsPerBand;
+        if (ensureCapacity(spill, size_t(grid) * w * rowsPerBand) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
+        MvConsts k;
+        fillConsts(k, w, hgt);
+        vp = frameParams(w, hgt, bands, rowsPerBand, spill.p, triCap, k);
+        return MV_OK;
+    }
+    // One camera launch on the stream: camera c of n draws env dEnv[c] (an all-zero frame outside [0, E)) through the view matrix
+    // dViews[c * 16 ..] into frame c of obs / depth / seg (depth and seg may be null) at w x h, from the instance lists of the last step.
+    // Stream-ordered, no ready stamps, no costs: the next step's cost-ordered queue does not see it.  The out-of-range counter is zeroed
+    // first and counts this launch only.
+    int launchCameras(const int32_t *dEnv, const float *dViews, int n, int w, int hgt, uint8_t *obs, float *depth, uint16_t *seg) {
+        if (ensureCapacity(cams.d_range, 1) != cudaSuccess) { setError("camera counter allocation failed"); return MV_ERR_CUDA; }
+        MV_CUDA(cudaMemsetAsync(cams.d_range.p, 0, sizeof(uint32_t), stream));
+        if (n == 0) return MV_OK;
+        mvr::ViewParams vp;
+        const int rc = bandedFrame(w, hgt, cameraGrid, cams.spill, vp);
+        if (rc) return rc;
+        vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = dViews;
+        vp.obs = obs; vp.depth = depth; vp.seg = seg;
+        vp.viewBase = 0; vp.N = n;
+        vp.camEnv = dEnv; vp.numEnvs = E; vp.rangeCount = cams.d_range.p;
+        return launchView(vp, false, mvr::Items::Cameras);
+    }
+    // the host-facing camera call: tables up, draw into the engine's buffers, copy into their pinned twins, wait
+    int drawCameras(const int32_t *envs, const float *views, int n, int w, int hgt, bool depth, bool seg) {
+        int rc = drain();
+        if (rc) return rc;
+        const size_t px = size_t(n) * size_t(w) * size_t(hgt);
+        const bool ok = ensureCapacity(cams.d_env, size_t(n)) == cudaSuccess && ensureCapacity(cams.d_views, size_t(n) * 16) == cudaSuccess &&
+                        ensureCapacity(cams.d_obs, px * 4) == cudaSuccess && ensureCapacity(cams.h_obs, px * 4) == cudaSuccess &&
+                        (!depth || (ensureCapacity(cams.d_depth, px) == cudaSuccess && ensureCapacity(cams.h_depth, px) == cudaSuccess)) &&
+                        (!seg || (ensureCapacity(cams.d_seg, px) == cudaSuccess && ensureCapacity(cams.h_seg, px) == cudaSuccess)) &&
+                        ensureCapacity(cams.h_range, 1) == cudaSuccess;
+        if (!ok) { setError("camera buffers: allocation failed"); return MV_ERR_CUDA; }
+        if (n > 0) {
+            MV_CUDA(cudaMemcpyAsync(cams.d_env.p, envs, sizeof(int32_t) * size_t(n), cudaMemcpyHostToDevice, stream));
+            MV_CUDA(cudaMemcpyAsync(cams.d_views.p, views, sizeof(float) * 16 * size_t(n), cudaMemcpyHostToDevice, stream));
+        }
+        rc = launchCameras(cams.d_env.p, cams.d_views.p, n, w, hgt, cams.d_obs.p, depth ? cams.d_depth.p : nullptr, seg ? cams.d_seg.p : nullptr);
+        if (rc) return rc;
+        if (n > 0) {
+            MV_CUDA(cudaMemcpyAsync(cams.h_obs.p, cams.d_obs.p, px * 4, cudaMemcpyDeviceToHost, stream));
+            if (depth) MV_CUDA(cudaMemcpyAsync(cams.h_depth.p, cams.d_depth.p, px * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            if (seg) MV_CUDA(cudaMemcpyAsync(cams.h_seg.p, cams.d_seg.p, px * sizeof(uint16_t), cudaMemcpyDeviceToHost, stream));
+        }
+        MV_CUDA(cudaMemcpyAsync(cams.h_range.p, cams.d_range.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        MV_CUDA(cudaStreamSynchronize(stream));
+        return MV_OK;
+    }
+    // world-space box {min x, y, z, max x, y, z} of env e's live level from the host mirrors: static boxes (rotated ones by their extent
+    // about y), decorations (a unit mesh's reach along each column, the capsule's y doubled) and terrain slabs
+    void levelBounds(int e, float *out6) const {
+        const size_t row = liveRow(e);
+        const MvLevel &L = h_levels.p[row];
+        float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+        auto add = [&](const float c[3], const float r[3]) {
+            for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], c[a] - r[a]); hi[a] = std::max(hi[a], c[a] + r[a]); }
+        };
+        const MvBox *st = h_statics.p + row * size_t(staticCap);
+        const float *rot = h_staticRot.p + row * size_t(staticCap) * 2;
+        for (int i = 0; i < L.n_static; ++i) {
+            float r[3] = {st[i].h[0], st[i].h[1], st[i].h[2]};
+            if (st[i].flags & MV_ROTATED) {
+                const float ax = std::fabs(rot[2 * i]), az = std::fabs(rot[2 * i + 1]);
+                r[0] = ax * st[i].h[0] + az * st[i].h[2];
+                r[2] = az * st[i].h[0] + ax * st[i].h[2];
+            }
+            add(st[i].c, r);
+        }
+        const MvDeco *dc = h_deco.p + row * size_t(decoCap);
+        for (int i = 0; i < L.n_deco; ++i) {
+            const float *m = dc[i].model;
+            const float ys = dc[i].mesh == 1 ? 2.0f : 1.0f;
+            const float c[3] = {m[12], m[13], m[14]};
+            float r[3];
+            for (int a = 0; a < 3; ++a) r[a] = std::fabs(m[a]) + ys * std::fabs(m[4 + a]) + std::fabs(m[8 + a]);
+            add(c, r);
+        }
+        for (int i = 0; i < L.n_terrain; ++i) {
+            const int32_t *bb = L.terrain[i].bb;
+            const float c[3] = {0.5f * float(bb[0] + bb[3]), float(bb[1]) + 0.025f, 0.5f * float(bb[2] + bb[5])};
+            const float r[3] = {0.5f * float(bb[3] - bb[0]), 0.025f, 0.5f * float(bb[5] - bb[2])};
+            add(c, r);
+        }
+        for (int a = 0; a < 3; ++a) {
+            out6[a] = lo[a] <= hi[a] ? lo[a] : 0.0f;
+            out6[3 + a] = lo[a] <= hi[a] ? hi[a] : 0.0f;
+        }
     }
     // shared-memory carve-up, occupancy and the per-CTA spill slabs for the current triangle-list capacity / band count
     int configureRaster() {
@@ -837,6 +958,15 @@ struct mv_engine {
             maskedPerSM = v ? std::min(maskedPerSM, perSM) : perSM;
         }
         maskedGrid = numSMs * std::max(1, std::min(maskedPerSM, rasterCtasPerSM));  // shares d_spill, sized by rasterGrid
+        int cameraPerSM = 0;
+        for (int v = 0; v < 4; ++v) {  // the camera variants size their own grid (and spill slab) from their own occupancy
+            const void *fn = reinterpret_cast<const void *>(viewKernelOf(mvr::Items::Cameras, v >= 2, v & 1));
+            MV_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, maxOptin));
+            int perSM = 0;
+            MV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fn, mvr::kThreads, rasterSmem));
+            cameraPerSM = v ? std::min(cameraPerSM, perSM) : perSM;
+        }
+        cameraGrid = numSMs * std::max(1, std::min(cameraPerSM, rasterCtasPerSM));
         bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
         d_spill.free();
         if (d_spill.alloc(size_t(rasterGrid) * W * bandRows) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
@@ -1262,7 +1392,7 @@ struct mv_engine {
         h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free(); h_active.free(); d_active.free();
         d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
         d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_seg.free(); d_faults.free();
-        hires.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free();
+        hires.free(); cams.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free();
         h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free(); h_seg.free();
         h_faults.free(); h_faultWord.free();
         d_doneReasons.free(); h_doneReasons.free();
@@ -1752,6 +1882,53 @@ int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out) {
     const int rc = h->drawHires(w, hgt);
     if (rc) return rc;
     if (out) *out = h->hires.h_obs.p;
+    return MV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ spectator cameras
+// the checks both camera calls share: state first (nothing may change on a refused call), then the arguments
+static int cameraCall(mv_handle h, const void *envs, const void *views, int n, int w, int hgt, const char *fn) {
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    if (h->hostStepPending) { h->setError(std::string(fn) + ": mv_step_begin is outstanding, call mv_step_end first"); return MV_ERR_STATE; }
+    if (n < 0 || (n > 0 && (!envs || !views))) { h->setError(std::string(fn) + ": bad env / view tables"); return MV_ERR_ARG; }
+    if (!hiresSizeOk(w, hgt)) { h->setError(std::string(fn) + ": camera frames must be a multiple of 32 x 4, at most 768 x 4096"); return MV_ERR_ARG; }
+    return MV_OK;
+}
+
+int mv_draw_cameras(mv_handle h, const int32_t *envs, const float *views16, int n, int w, int hgt, int want_depth, int want_seg, const uint8_t **obs,
+                    const float **depth, const uint16_t **seg, uint32_t *out_of_range) {
+    MV_ON_DEVICE(h)
+    int rc = cameraCall(h, envs, views16, n, w, hgt, "mv_draw_cameras");
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i)
+        if (envs[i] < 0 || envs[i] >= h->E) { h->setError("mv_draw_cameras: env " + std::to_string(envs[i]) + " out of range"); return MV_ERR_ARG; }
+    rc = h->drawCameras(envs, views16, n, w, hgt, want_depth != 0, want_seg != 0);
+    if (rc) return rc;
+    if (obs) *obs = h->cams.h_obs.p;
+    if (depth) *depth = want_depth ? h->cams.h_depth.p : nullptr;
+    if (seg) *seg = want_seg ? h->cams.h_seg.p : nullptr;
+    if (out_of_range) *out_of_range = *h->cams.h_range.p;
+    return MV_OK;
+}
+
+int mv_draw_cameras_device(mv_handle h, const int32_t *d_envs, const float *d_views16, int n, int w, int hgt, uint8_t *d_obs, float *d_depth,
+                           uint16_t *d_seg, uint32_t **d_out_of_range) {
+    MV_ON_DEVICE(h)
+    const int rc = cameraCall(h, d_envs, d_views16, n, w, hgt, "mv_draw_cameras_device");
+    if (rc) return rc;
+    if (n > 0 && !d_obs) { h->setError("mv_draw_cameras_device: null obs buffer"); return MV_ERR_ARG; }
+    const int rcl = h->launchCameras(d_envs, d_views16, n, w, hgt, d_obs, d_depth, d_seg);
+    if (rcl) return rcl;
+    if (d_out_of_range) *d_out_of_range = h->cams.d_range.p;
+    return MV_OK;
+}
+
+int mv_views_device(mv_handle h, float **d_views) { if (!h || !d_views) return MV_ERR_ARG; *d_views = h->d_views.p; return MV_OK; }
+
+int mv_level_bounds(mv_handle h, float *out6) {
+    if (!h || !out6) return MV_ERR_ARG;
+    if (!h->didReset) { h->setError("mv_level_bounds before mv_reset"); return MV_ERR_STATE; }
+    for (int e = 0; e < h->E; ++e) h->levelBounds(e, out6 + size_t(e) * 6);
     return MV_OK;
 }
 
@@ -2297,6 +2474,18 @@ int mv_debug_get_view(mv_handle h, int env, int agent, float *out16) {
     return MV_OK;
 }
 
+int mv_debug_view_order(mv_handle h, uint32_t *out, int cap) {
+    if (!h || !out) return MV_ERR_ARG;
+    MV_ON_DEVICE(h)
+    const size_t words = h->costItems() + size_t(h->E) + 1;
+    if (size_t(cap) < words) return -int(words);
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMemcpy(out, h->d_viewCost.p, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost) != cudaSuccess) {
+        h->setError("mv_debug_view_order: copy failed");
+        return MV_ERR_CUDA;
+    }
+    return int(words);
+}
+
 int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]) {
     MV_ON_DEVICE(h)
     int rc = statesCallState(h, "mv_debug_warp_agent");
@@ -2323,7 +2512,7 @@ int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n
     if (triCap < 32 || triCap > mvr::kMaxTriCap) return MV_ERR_ARG;
     // row bands: opts[3] of them (the last one may be shorter), or 0 = the rule of mv_draw_hires (bands of about a hundred tiles)
     int bandRows;
-    if (opts[3] == 0) bandRows = std::max(1, 96 / (w / 32)) * 4;
+    if (opts[3] == 0) bandRows = hiresBandRows(w);
     else if (opts[3] > 0 && opts[3] <= h / 4) bandRows = ((h / 4 + opts[3] - 1) / opts[3]) * 4;
     else return MV_ERR_ARG;
     const int bands = (h + bandRows - 1) / bandRows;

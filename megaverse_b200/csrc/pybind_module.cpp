@@ -280,6 +280,45 @@ public:
         check(mv_set_next_levels(h__, envs.data(), levels.data(), int(envs.size())));
     }
 
+    // (extension) spectator cameras (mv_draw_cameras): camera c draws env envs[c] through the view matrix views[c] (float32 [n,16] or
+    // [n,4,4] as stored, column-major) at w x h.  Returns (rgba uint8 [n,h,w,4], depth float32 [n,h,w] or None, seg uint16 [n,h,w] or None,
+    // out-of-range triangle count), copies the caller keeps
+    py::tuple drawCameras(const std::vector<int32_t> &envs, py::array_t<float, py::array::c_style | py::array::forcecast> views, int w, int h,
+                          bool depth, bool seg) {
+        alive();
+        const int n = int(envs.size());
+        if (views.size() != py::ssize_t(n) * 16) throw std::invalid_argument("draw_cameras: views must hold 16 floats per env");
+        const uint8_t *o = nullptr;
+        const float *d = nullptr;
+        const uint16_t *sg = nullptr;
+        uint32_t wide = 0;
+        int rc;
+        { py::gil_scoped_release nogil; rc = mv_draw_cameras(h__, envs.data(), views.data(), n, w, h, depth, seg, &o, &d, &sg, &wide); }
+        check(rc);
+        const size_t px = size_t(n) * size_t(w) * size_t(h);
+        py::array_t<uint8_t> rgba({n, h, w, 4});
+        if (px) std::memcpy(rgba.mutable_data(), o, px * 4);
+        py::object dep = py::none(), sgo = py::none();
+        if (depth) { py::array_t<float> a({n, h, w}); if (px) std::memcpy(a.mutable_data(), d, px * sizeof(float)); dep = a; }
+        if (seg) { py::array_t<uint16_t> a({n, h, w}); if (px) std::memcpy(a.mutable_data(), sg, px * sizeof(uint16_t)); sgo = a; }
+        return py::make_tuple(rgba, dep, sgo, wide);
+    }
+    // (extension) float32 [N,16] view matrices of the last step (mv_debug_get_view per view: waits for the stream)
+    py::array_t<float> getViews() {
+        alive();
+        const int N = int(masks_.size());
+        py::array_t<float> out({N, 16});
+        for (int v = 0; v < N; ++v) check(mv_debug_get_view(h__, v / numAgentsPerEnv_, v % numAgentsPerEnv_, out.mutable_data() + size_t(v) * 16));
+        return out;
+    }
+    // (extension) float32 [E,6] world-space bounding box {min xyz, max xyz} of each env's live level (mv_level_bounds)
+    py::array_t<float> levelBounds() {
+        alive();
+        py::array_t<float> out({numEnvs_, 6});
+        check(mv_level_bounds(h__, out.mutable_data()));
+        return out;
+    }
+
     void close() {
         if (h__) { mv_close(h__); h__ = nullptr; }
     }
@@ -344,5 +383,11 @@ PYBIND11_MODULE(megaverse, m) {
         .def("get_final_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(true); },
              "the terminal rows (options state_tensors and final_obs): the state each env's last episode ended on, same dict")
         .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),
-             "step the listed envs only: the others run nothing, report reward 0 and done 0, and keep their observations");
+             "step the listed envs only: the others run nothing, report reward 0 and done 0, and keep their observations")
+        .def("draw_cameras", &MegaverseGym::drawCameras, py::arg("envs"), py::arg("views"), py::arg("w"), py::arg("h"), py::arg("depth") = false,
+             py::arg("seg") = false,
+             "spectator cameras: camera c draws env envs[c] through views[c] (16 floats, column-major) at w x h from the last step's scene; "
+             "returns (rgba uint8[n,h,w,4], depth float32[n,h,w] or None, seg uint16[n,h,w] or None, out-of-range triangle count)")
+        .def("get_views", &MegaverseGym::getViews, "float32[N,16] view matrices of the last step (view env*A + agent)")
+        .def("level_bounds", &MegaverseGym::levelBounds, "float32[num_envs,6] {min xyz, max xyz} of each env's live level");
 }

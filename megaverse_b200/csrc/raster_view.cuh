@@ -125,6 +125,13 @@ struct ViewParams {
     // masked launches only (Items::Ended and Items::Active): the items of env e of this launch's views (viewBase / A + e) are skipped where
     // envMask[e] is 0
     const uint8_t *envMask;
+    // camera launches only (Items::Cameras; viewBase 0, N cameras): work item c * bands + band draws camera c -- the instance list and
+    // counts of env camEnv[c] (an all-zero frame when it is outside [0, numEnvs)), the view matrix views[c * 16 ..], frame c of obs /
+    // depth / seg.  Band 0 of each camera adds the triangles whose snapped corners leave the range the integer set-up is exact in to
+    // *rangeCount (snapOutOfRange).  New fields go here, at the end: the other variants keep their parameter offsets and their code
+    const int32_t *camEnv;
+    uint32_t *rangeCount;
+    int numEnvs;
 };
 
 struct SmemLayout { uint32_t stage, cover, shade, xf, off, frag, small, meshV, meshI, clip, slow, sched, misc, total; };
@@ -249,6 +256,17 @@ __device__ __forceinline__ ScreenVert projectVert(const ClipVert &v, float hw, f
     o.sz = v.cz * r;
     return o;
 }
+// Does a projected triangle leave the range the integer set-up is exact in (engine.cu, kMaxRasterWidth): a snapped coordinate with
+// |s| >= 2^30.5 sub-pixels (a saturated snap included), or two corners 2^31 sub-pixels or more apart on one axis?  Agent eyes stay inside
+// by measurement; the camera launches check every triangle they project.
+__device__ __forceinline__ bool snapOutOfRange(const ScreenVert &a, const ScreenVert &b, const ScreenVert &c) {
+    constexpr long long kSnapMax = 1518500249ll;  // floor(2^30.5)
+    const long long x0 = a.sx, x1 = b.sx, x2 = c.sx, y0 = a.sy, y1 = b.sy, y2 = c.sy;
+    const long long ax = max(llabs(x0), max(llabs(x1), llabs(x2))), ay = max(llabs(y0), max(llabs(y1), llabs(y2)));
+    const long long dx = max(x0, max(x1, x2)) - min(x0, min(x1, x2)), dy = max(y0, max(y1, y2)) - min(y0, min(y1, y2));
+    return ax > kSnapMax || ay > kSnapMax || dx >= (1ll << 31) || dy >= (1ll << 31);
+}
+
 // winding, pixel box: does the projected triangle touch a pixel centre of this band at all?
 struct TriBox { long long area2; uint32_t bx, by; };
 __device__ __forceinline__ bool triBox(const SetupCtx &cx, const ScreenVert &a, const ScreenVert &b, const ScreenVert &c, TriBox &o) {
@@ -344,10 +362,12 @@ enum SetupResult { kSetupDone = 0, kSetupFull = 1, kSetupClip = 2 };  // appende
 // One item: a box face -- four vertices, triangles (0,1,2) and (0,2,3) (Magnum cubeSolid index pattern), nTri = 2 -- or a mesh
 // triangle (nTri = 1, v3 repeats v2).  v0..v3 carry positions only; vp0..vp3 = the mesh vertices (six floats each) for the normals,
 // which are only computed for what survives the screen-space tests.  One copy of the set-up code serves both (code size: the kernel's
-// hot loops have to stay inside the instruction cache).
-template <bool FAST>
+// hot loops have to stay inside the instruction cache).  RANGE (camera launches): once the item is done, its projected triangles that
+// snapOutOfRange flags are added to *rangeCount when that is set.
+template <bool FAST, bool RANGE = false>
 __device__ __forceinline__ SetupResult setupItem(const SetupCtx &cx, ClipVert &v0, ClipVert &v1, ClipVert &v2, ClipVert &v3, int nTri, const float nm[9], const float *vp0,
-                                                 const float *vp1, const float *vp2, const float *vp3, int color, uint32_t keyBase) {
+                                                 const float *vp1, const float *vp2, const float *vp3, int color, uint32_t keyBase,
+                                                 uint32_t *rangeCount = nullptr) {
     if (sideOutcode(v0) & sideOutcode(v1) & sideOutcode(v2) & sideOutcode(v3)) return kSetupDone;
     if (!(insideNearFar(v0) && insideNearFar(v1) && insideNearFar(v2) && insideNearFar(v3))) {
         // wholly behind the near plane or wholly beyond the far plane: clipping would leave nothing
@@ -362,9 +382,17 @@ __device__ __forceinline__ SetupResult setupItem(const SetupCtx &cx, ClipVert &v
     TriBox b0, b1;
     const bool vis0 = triBox(cx, s0, s1, s2, b0), vis1 = nTri == 2 && triBox(cx, s0, s2, s3, b1);
     const int n = (vis0 ? 1 : 0) + (vis1 ? 1 : 0);
-    if (!n) return kSetupDone;
+    auto countWide = [&] {
+        const uint32_t wide = (snapOutOfRange(s0, s1, s2) ? 1u : 0u) + (nTri == 2 && snapOutOfRange(s0, s2, s3) ? 1u : 0u);
+        if (wide && rangeCount) atomicAdd(rangeCount, wide);
+    };
+    if (!n) {
+        if (RANGE) countWide();
+        return kSetupDone;
+    }
     int slot = reserveTris(cx, n);
     if (slot < 0) return kSetupFull;
+    if (RANGE) countWide();
     vertNormal(v0, nm, vp0); vertNormal(v1, nm, vp1); vertNormal(v2, nm, vp2); vertNormal(v3, nm, vp3);
 #pragma unroll 1
     for (int t = 0; t < 2; ++t) {
@@ -812,7 +840,8 @@ __device__ MV_TILE_INLINE void tilePass(const ViewParams &P, int count, unsigned
 // Which items a launch draws: every item, in natural or cost order (All); the items of the envs whose P.envMask byte is set, in natural order
 // (Ended: the terminal frames of the envs that ended); or those of the envs P.envMask names, in cost order when P.viewCost is set (Active: the
 // live frames of a step with an active set).  Ended and Active differ only in the claim, so that the terminal-frame launch keeps its code.
-enum class Items { All, Ended, Active };
+// Cameras: every item in natural order, each view a caller's camera (ViewParams::camEnv): no ready stamps, no costs, `order` untouched.
+enum class Items { All, Ended, Active, Cameras };
 
 // Next work item of the CTA (called by one thread): an index into [0, total), or >= total when the queue is empty.  Natural order: the
 // claim itself; cost-ordered: the view the previous launch's sort put at that position.  Masked: claims of unmasked envs are passed over, so
@@ -850,6 +879,7 @@ template <Items ITEMS> __device__ __forceinline__ uint32_t claimWork(const ViewP
 // ITEMS: which work items the launch draws (Items: every item, the terminal frames of option "final_obs", or the active envs' live frames)
 // SEG: P.seg is set (option "segmentation"); never with Items::Ended
 template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void MV_VIEW_BOUNDS viewKernel(const __grid_constant__ ViewParams P) {
+    constexpr bool CAM = ITEMS == Items::Cameras;
     unsigned char *smem = g_viewSmem;
     const SmemLayout L = smemLayout(P.triCap);
     MvInstance *stage = reinterpret_cast<MvInstance *>(smem + L.stage);
@@ -903,7 +933,8 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
         if (claim >= total) break;
         const int vrel = int(claim / uint32_t(bands)), band = int(claim - uint32_t(vrel) * uint32_t(bands));
         const int view = P.viewBase + vrel;
-        const int env = view / P.A;
+        const int env = CAM ? P.camEnv[vrel] : view / P.A;
+        const bool live = !CAM || (env >= 0 && env < P.numEnvs);  // a camera of no env reads nothing and draws an all-zero frame
         const int rowLo = band * P.bandRows, rowHi = min(P.H, rowLo + P.bandRows) - 1;
         const int bandTiles = tilesX * ((rowHi - rowLo + 1) >> 2);
         const MvInstance *inst = P.instances + size_t(env) * size_t(P.instStride);
@@ -932,7 +963,7 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
         __syncthreads();
         if (!prefetched) {
             if (tid < 16) M.view[tid] = __ldcg(P.views + size_t(view) * 16 + tid);
-            else if (tid < 24) M.counts[tid - 16] = __ldcg(P.instCounts + env * 8 + (tid - 16));
+            else if (tid < 24) M.counts[tid - 16] = live ? __ldcg(P.instCounts + env * 8 + (tid - 16)) : 0;
             __syncthreads();
         }
         const int nInst = M.counts[1];
@@ -1102,7 +1133,8 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
                         if (!facesAway) {
 #pragma unroll
                             for (int k = 0; k < 4; ++k) vertPosition(cvt[k], mv, vpn[k], P.p00, P.p11, P.p22, P.p32);
-                            res = setupItem<FAST>(cx, cvt[0], cvt[1], cvt[2], cvt[3], nTri, nm, vpn[0], vpn[1], vpn[2], vpn[3], color, keyBase);
+                            res = setupItem<FAST, CAM>(cx, cvt[0], cvt[1], cvt[2], cvt[3], nTri, nm, vpn[0], vpn[1], vpn[2], vpn[3], color, keyBase,
+                                                       CAM && band == 0 ? P.rangeCount : nullptr);
                         }
                         pending = res == kSetupFull;
                         if (res == kSetupClip) {
@@ -1162,13 +1194,14 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
                         // its key (coplanar and disjoint, they never tie on a pixel)
                         const int t = lane / 3, k = lane - t * 3 + 1;
                         const ClipVert *pp = t ? poly1 : poly0;
-                        bool vis = false;
+                        bool vis = false, wide = false;
                         TriBox tb;
                         ScreenVert sa, sb, sc;
                         if (lane < 6 && k + 1 < (t ? n1 : n0)) {
                             const float hw = float(P.W) * 0.5f, hh = float(P.H) * 0.5f;
                             sa = projectVert(pp[0], hw, hh); sb = projectVert(pp[k], hw, hh); sc = projectVert(pp[k + 1], hw, hh);
                             vis = triBox(cx, sa, sb, sc, tb);
+                            if (CAM) wide = snapOutOfRange(sa, sb, sc);
                         }
                         const unsigned vm = __ballot_sync(0xffffffffu, vis);
                         bool done = true;
@@ -1181,6 +1214,10 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
                         }
                         if (done) { if (lane == 0) slowList[sidx] = uint16_t(e | 0x8000); }
                         else slowFull = true;
+                        if (CAM && done && band == 0 && P.rangeCount) {
+                            const unsigned wm = __ballot_sync(0xffffffffu, wide);
+                            if (lane == 0 && wm) atomicAdd(P.rangeCount, uint32_t(__popc(wm)));
+                        }
                         __syncwarp();  // the scratch polygons are rewritten by the warp's next entry
                     }
                     if (!__syncthreads_or((pending || slowFull) ? 1 : 0)) break;
@@ -1205,7 +1242,8 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
             const uint32_t nc = claimWork<ITEMS>(P, total);
             int pre = 0;
             if (nc < total) {
-                const int nview = P.viewBase + int(nc / uint32_t(bands)), nenv = nview / P.A;
+                const int nview = P.viewBase + int(nc / uint32_t(bands)), nenv = CAM ? P.camEnv[nview] : nview / P.A;
+                const bool nlive = !CAM || (nenv >= 0 && nenv < P.numEnvs);
                 bool ready = true;
                 if (P.ready) {
                     uint32_t v;
@@ -1219,7 +1257,7 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
 #pragma unroll
                     for (int q = 0; q < 16; ++q) vm[q] = __ldcg(P.views + size_t(nview) * 16 + q);
 #pragma unroll
-                    for (int q = 0; q < 8; ++q) cn[q] = __ldcg(P.instCounts + nenv * 8 + q);
+                    for (int q = 0; q < 8; ++q) cn[q] = nlive ? __ldcg(P.instCounts + nenv * 8 + q) : 0;
 #pragma unroll
                     for (int q = 0; q < 16; ++q) M.view[q] = vm[q];
 #pragma unroll
@@ -1234,7 +1272,17 @@ template <bool FAST, Items ITEMS = Items::All, bool SEG = false> __global__ void
             }
             M.claim = nc; M.prefetched = pre;
         }
-        tilePass<FAST, SEG>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, true);
+        if (live) {
+            tilePass<FAST, SEG>(P, min(M.nTris, M.nValid), spill, view, rowLo, bandTiles, batch, true);
+        } else {  // a camera of no env: zero colour (alpha included), zero depth, zero segmentation over the band
+            const size_t px0 = (size_t(view) * P.H + size_t(rowLo)) * P.W;
+            for (int q = tid; q < ((rowHi - rowLo + 1) * P.W) >> 2; q += kThreads) {
+                const size_t p = px0 + size_t(q) * 4;
+                *reinterpret_cast<uint4 *>(P.obs + p * 4) = make_uint4(0u, 0u, 0u, 0u);
+                if (P.depth) *reinterpret_cast<float4 *>(P.depth + p) = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (SEG) *reinterpret_cast<uint2 *>(P.seg + p) = make_uint2(0u, 0u);
+            }
+        }
         __syncthreads();
         if (P.viewCost && tid == 0) P.viewCost[claim] = uint32_t(min((unsigned long long)clock64() - M.itemStart, 0xffffffffull * 16ull) >> 4);
         if (P.stats && tid < 8) {

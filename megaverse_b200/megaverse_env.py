@@ -5,6 +5,7 @@ unchanged.  The per-agent pybind loops of the reference (megaverse_env.py:121-16
 the values returned are the same lists."""
 import numpy as np
 
+from .cameras import chase_views, overview_views
 from .gym_shim import Box, Discrete, Env, Tuple
 
 # the product fails loudly when its native extension is missing
@@ -266,6 +267,26 @@ class MegaverseEnv(Env):
             except Exception:  # noqa: BLE001  (headless boxes)
                 pass
         return obs_final
+
+    def render_cameras(self, envs, views, w=768, h=432):
+        """(extension) spectator cameras: camera c draws env envs[c] of the current scene through the view matrix views[c] (16 float32,
+        column-major, megaverse_b200.cameras) at w x h (multiples of 32 x 4, at most 768 x 4096).  Returns RGB uint8 [len(envs), h, w, 3], a
+        copy; render() is unchanged"""
+        frames = self.env.draw_cameras([int(e) for e in envs], np.asarray(views, dtype=np.float32).reshape(-1, 16), int(w), int(h))[0]
+        return np.ascontiguousarray(frames[:, :, :, :3])
+
+    def overview(self, envs, w=768, h=432):
+        """(extension) RGB uint8 [len(envs), h, w, 3]: each listed env's whole level seen from above and in front (cameras.overview_views of
+        its bounding box)"""
+        envs = [int(e) for e in envs]
+        return self.render_cameras(envs, overview_views(self.env.level_bounds()[envs], w, h), w, h)
+
+    def chase(self, agents, w=768, h=432):
+        """(extension) RGB uint8 [len(agents), h, w, 3]: a third-person camera behind and above each listed agent (index env *
+        num_agents_per_env + agent, as in observations()), cameras.chase_views of its own view matrix"""
+        agents = [int(a) for a in agents]
+        views = chase_views(self.env.get_views()[agents])
+        return self.render_cameras([a // self.num_agents_per_env for a in agents], views, w, h)
 
     def get_default_reward_shaping(self, actor_idx=None):
         """env 0's default scheme; with actor_idx, the default of that actor's scenario (they differ in a mixed batch)"""
