@@ -184,6 +184,36 @@ int mv_state_tensors_host(mv_handle h, const float **agents, const float **envs,
 int mv_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards);
 int mv_final_state_tensors_host(mv_handle h, const float **agents, const float **envs, const float **objects, const float **rewards);
 int mv_final_state_tensors_device(mv_handle h, float **agents, float **envs, float **objects, float **rewards);
+/* Ray sensors: every agent casts the same fan of n rays against its env's drawn scene, and each ray reports the distance to the first
+ * surface it meets and what that surface is.
+ * mv_set_rays, before the first reset (MV_ERR_STATE after it): dirs3 = float[n][3], directions in CAMERA space, the frame of the agent's
+ * view matrix (x right, y up, -z forward); n = 0 turns the rays off (the default), else 1..MV_MAX_RAYS; max_dist finite and > 0.  A
+ * direction that is zero or not finite, n out of range or a bad max_dist is MV_ERR_ARG and changes nothing.  Each direction is used
+ * exactly as given, and a distance counts multiples of its length: unit vectors give world units.  One fan for every agent of the engine,
+ * in single-scenario and mixed engines alike (megaverse_b200/rays.py builds fans and rings).
+ * What a ray hits: every entry of the env's instance list that the rasteriser draws (the same rows and counts), meshes as drawn (boxes are
+ * the cube [-1, 1]^3), front faces only -- a ray that starts inside a box or a closed mesh does not hit it -- except the agent's own body,
+ * eyes and HUD bar (tag MV_SEG_AGENT << 8 | own index).  The hit is the nearest; on an exact tie the later entry in draw order wins, as
+ * the rasteriser's LESS_OR_EQUAL does.  The arithmetic is defined operation by operation in DESIGN.md section 3 ("Ray sensors"), so that
+ * a CPU restatement gives the same bits.
+ * Outputs, ray r of view env*A + agent at [view][r]: dist float[N][n], the hit's parameter t along the direction (0: no hit within
+ * max_dist); tag uint16[N][n], the hit drawable's MV_SEG_* class << 8 | index (0: no hit) -- the conventions of depth and segmentation.
+ * Rays always describe the scene the current frames show: every call that draws the step's frames writes them (mv_step,
+ * mv_step_begin/end, mv_step_envs, mv_step_device[_ends|_active], mv_reset, mv_reset_envs, mv_states_load's redraw), after the last tick
+ * with action_repeat; inactive envs keep theirs.  With option final_obs as well, an env that ends in a step gets terminal rays, cast from
+ * the terminal rows its terminal frame is drawn from; other terminal rows are left alone.
+ * Delivery: host-facing calls return with both arrays in pinned host memory (mv_rays_host; one copy on the step's stream);
+ * mv_step_device* leaves them in HBM (mv_rays_device) in stream order, and mv_fetch_obs copies them down.  Nothing else changes: obs,
+ * depth, segmentation, rewards, dones, reasons, true objectives, terminal frames and state tensors are byte-identical with rays on and off.
+ * Cost: one launch per drawing call (two with terminal rays); 6 B per ray per view in HBM and again pinned, twice that with final_obs.
+ * The getters take NULL out pointers; MV_ERR_ARG for a null handle and while the rays (or, for the terminal rays, option final_obs) are
+ * off; MV_ERR_STATE before mv_reset. */
+#define MV_MAX_RAYS 256
+int mv_set_rays(mv_handle h, const float *dirs3, int n, float max_dist);
+int mv_rays_host(mv_handle h, const float **dist, const uint16_t **tag);
+int mv_rays_device(mv_handle h, float **dist, uint16_t **tag);
+int mv_final_rays_host(mv_handle h, const float **dist, const uint16_t **tag);
+int mv_final_rays_device(mv_handle h, float **dist, uint16_t **tag);
 
 /* MegaverseGym::getRewardShaping / setRewardShaping (megaverse.cpp:214-222).  get: fills up to cap entries, returns the
  * number of keys in *n.  Key strings are owned by the engine. */
@@ -413,6 +443,10 @@ int mv_last_kernel_ms(mv_handle h, float *out2);
 /* device time of the last step's terminal-frame launch (option "final_obs") in milliseconds, CUDA events; 0 when the step had none or
  * carried no timing events (mv_step_device with option overlap 1).  With it, mv_last_kernel_ms [1] is the step's own raster launch. */
 int mv_last_final_ms(mv_handle h, float *out);
+/* device time of the last call's ray launches (mv_set_rays: the live rays and, with final_obs, the terminal ones) in milliseconds, CUDA
+ * events; 0 when the call cast none or carried no timing events.  They run after the call's raster launches, and mv_last_kernel_ms and
+ * mv_last_final_ms leave them out. */
+int mv_last_rays_ms(mv_handle h, float *out);
 
 /* MegaverseGym::close (megaverse.cpp:224-243) */
 int mv_close(mv_handle h);

@@ -43,8 +43,9 @@ def build_lib(force=False, verbose=False):
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     extra = os.environ.get("MV_NVCC_EXTRA", "").split()  # developer switches, e.g. -DMV_KCC_COUNTERS
-    # state_copy.cu is a module of its own: NVVM optimises per module, so the engine's kernels do not see it
-    cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB] + [os.path.join(CSRC, f) for f in ("engine.cu", "state_copy.cu", "levelgen.cpp")]
+    # state_copy.cu and ray_kernel.cu are modules of their own: NVVM optimises per module, so the engine's kernels do not see them
+    srcs = ("engine.cu", "state_copy.cu", "ray_kernel.cu", "levelgen.cpp")
+    cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB] + [os.path.join(CSRC, f) for f in srcs]
     subprocess.check_call(cmd, cwd=CSRC)
     return LIB
 

@@ -57,6 +57,10 @@ def lib():
         L.mv_kernel_launches.argtypes = [vp, C.POINTER(C.c_int64)]
         L.mv_last_kernel_ms.argtypes = [vp, C.POINTER(cf)]
         L.mv_last_final_ms.argtypes = [vp, C.POINTER(cf)]
+        L.mv_last_rays_ms.argtypes = [vp, C.POINTER(cf)]
+        L.mv_set_rays.argtypes = [vp, vp, ci, cf]
+        for name in ("mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device"):
+            getattr(L, name).argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
         for name in ("mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances"):
             getattr(L, name).argtypes = [vp, ci, vp, ci]
         L.mv_debug_get_view.argtypes = [vp, ci, ci, vp]
@@ -95,6 +99,7 @@ EXPORTS = [
     "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device", "mv_set_next_levels", "mv_level_set_pick",
     "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
     "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
+    "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -134,6 +139,7 @@ class Engine:
         if rc != MV_OK:
             raise MegaverseError(rc, (L.mv_last_error(None) or b"").decode())
         self.E, self.A, self.N, self.w, self.h = num_envs, num_agents, num_envs * num_agents, w, h
+        self.num_rays = 0  # set_rays
         if depth:
             self._ck(L.mv_set_option(self._h, b"depth", 1))
         if segmentation:
@@ -272,8 +278,9 @@ class Engine:
         float32[E,16], "state_objects" / "state_rewards" float32[E,128,4] and, with option final_obs too, the terminal rows "final_state_agents",
         ... (state_tensors()), and with option level_set "level_ids" int32[E] (the level each env is on) and
         "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream), and "views"
-        float32[N,16] (the last step's view matrices, column-major: chase cameras on the device).  Valid in the engine stream's order (mv_stream)
-        until mv_close."""
+        float32[N,16] (the last step's view matrices, column-major: chase cameras on the device), and with rays (set_rays) "rays_dist"
+        float32[N,R] / "rays_tag" uint16[N,R] and, with option final_obs too, "final_rays_dist" / "final_rays_tag".  Valid in the engine
+        stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
                   "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
@@ -281,8 +288,13 @@ class Engine:
         for prefix in ("state_", "final_state_"):
             for k, shp in self._state_shapes().items():
                 shapes[prefix + k] = (shp, "<f4")
+        for prefix in ("", "final_"):
+            shapes[prefix + "rays_dist"] = ((self.N, self.num_rays), "<f4")
+            shapes[prefix + "rays_tag"] = ((self.N, self.num_rays), "<u2")
         shape, typestr = shapes[what]
-        if what.startswith(("state_", "final_state_")):
+        if what.endswith(("rays_dist", "rays_tag")):
+            ptr = self._ray_ptrs("mv_%srays_device" % ("final_" if what.startswith("final_") else ""))[0 if what.endswith("dist") else 1]
+        elif what.startswith(("state_", "final_state_")):
             ptr = self._state_ptrs("mv_%s_tensors_device" % what.rsplit("_", 1)[0])[what.rsplit("_", 1)[1]]
         else:
             ptr = self.device_ptr(what)
@@ -361,6 +373,39 @@ class Engine:
     def final_state_tensors(self):
         """options state_tensors and final_obs: the same dict of terminal rows, the state each env's last episode ended on"""
         return self._state_views("mv_final_state_tensors_host")
+
+    def set_rays(self, directions, max_distance):
+        """ray sensors (mv_set_rays, before the first reset): directions float32[R,3] in camera space (x right, y up, -z forward; rays.fan /
+        rays.ring build them), R in 0..MV_MAX_RAYS (0 turns them off); a hit distance counts multiples of a direction's length"""
+        d = np.ascontiguousarray(directions, dtype=np.float32).reshape(-1, 3)
+        self._ck(lib().mv_set_rays(self._h, d.ctypes.data if len(d) else None, len(d), float(max_distance)))
+        self.num_rays = len(d)
+
+    def _ray_ptrs(self, fn):
+        dist, tag = C.c_void_p(), C.c_void_p()
+        self._ck(getattr(lib(), fn)(self._h, C.byref(dist), C.byref(tag)))
+        return dist.value, tag.value
+
+    def _ray_views(self, fn):
+        dist, tag = self._ray_ptrs(fn)
+        n = self.N * self.num_rays
+        return (np.frombuffer((C.c_char * (n * 4)).from_address(dist), dtype=np.float32).reshape(self.N, self.num_rays),
+                np.frombuffer((C.c_char * (n * 2)).from_address(tag), dtype=np.uint16).reshape(self.N, self.num_rays))
+
+    def rays(self):
+        """(dist float32[N,R], tag uint16[N,R]) of the rays set by set_rays: views of the engine's pinned arrays after the last host-facing
+        call (or fetch_obs).  Ray r of view env*A + agent: the distance to the first front face it meets (0: none within the maximum) and
+        that drawable's MV_SEG_* class << 8 | index (0: none)"""
+        return self._ray_views("mv_rays_host")
+
+    def final_rays(self):
+        """rays and option final_obs: the same pair cast from the terminal rows, the scene each env's last episode ended on"""
+        return self._ray_views("mv_final_rays_host")
+
+    def last_rays_ms(self):
+        out = C.c_float()
+        self._ck(lib().mv_last_rays_ms(self._h, C.byref(out)))
+        return out.value
 
     def final_obs(self):
         """uint8[N,h,w,4] terminal frames (option final_obs): views of env e hold the frame its last episode ended on"""

@@ -35,6 +35,7 @@
 #include "level_set.h"
 #include "levelgen.hpp"
 #include "raster_view.cuh"
+#include "ray_kernel.h"
 #include "state_copy.h"
 #include "step_kernel.cuh"
 
@@ -444,6 +445,41 @@ struct mv_engine {
         return MV_OK;
     }
 
+    // ray sensors (mv_set_rays, allocated at the first reset): dist float[N][R] and tag uint16[N][R] in HBM, each followed with option
+    // final_obs by the terminal rays of the same shape.  Every call that draws the step's frames casts them behind its raster launches
+    // (castRays); a host-facing call then copies both blocks into their pinned twins on the stream
+    int nRays = 0;
+    float rayMaxDist = 0.0f;
+    std::vector<float> rayDirs;     // [nRays][3] camera space, as the caller gave them
+    DevBuf<float> d_rayDirs, d_rayDist;
+    DevBuf<uint16_t> d_rayTag;
+    PinBuf<float> h_rayDist;
+    PinBuf<uint16_t> h_rayTag;
+    cudaEvent_t evRays = nullptr;   // before a timed call's ray launches (readKernelTimes)
+    bool lastHadRays = false;
+    float lastRaysMs = 0.0f;
+    size_t rayCount() const { return size_t(N) * size_t(nRays); }
+    size_t rayBlock() const { return rayCount() * (wantFinal ? 2 : 1); }
+    // one ray launch: the live rays of the envs `mask` names (every env when null), or the terminal rays of the envs that ended (d_dones)
+    // from their terminal rows
+    int castRays(bool terminal, const uint8_t *mask) {
+        mvray::RayParams rp;
+        rp.instances = terminal ? d_termInst.p : d_inst.p; rp.instCounts = terminal ? d_termCounts.p : d_instCounts.p;
+        rp.views = terminal ? d_termViews.p : d_views.p;
+        rp.dirs = d_rayDirs.p; rp.envMask = terminal ? d_dones.p : mask;
+        rp.dist = d_rayDist.p + (terminal ? rayCount() : 0); rp.tag = d_rayTag.p + (terminal ? rayCount() : 0);
+        rp.instStride = instCap; rp.E = E; rp.A = A; rp.R = nRays; rp.maxDist = rayMaxDist;
+        MV_CUDA(mvray::castRays(rp, stream));
+        launches += 1;
+        return MV_OK;
+    }
+    // both blocks (live and terminal rays) into their pinned twins, in stream order
+    int downloadRays(cudaStream_t s) {
+        MV_CUDA(cudaMemcpyAsync(h_rayDist.p, d_rayDist.p, sizeof(float) * rayBlock(), cudaMemcpyDeviceToHost, s));
+        MV_CUDA(cudaMemcpyAsync(h_rayTag.p, d_rayTag.p, sizeof(uint16_t) * rayBlock(), cudaMemcpyDeviceToHost, s));
+        return MV_OK;
+    }
+
     // ------------------------------------------------------------------ level generation scheduling
     // generate the level for episode `serial` of env e into staging slot s, after every job scheduled for the env before
     void scheduleGen(int e, int s, int serial) {
@@ -697,13 +733,20 @@ struct mv_engine {
             if (timed) MV_CUDA(cudaEventRecord(evFinal, stream));
             if (const int rc = launchFinal(!async)) return rc;
         }
-        return endTimes(dep ? Timed::Union : Timed::Split, timed, final);
+        if (nRays) {  // behind every raster launch of the call: the rays of the stepped envs, then the terminal rays of those that ended
+            if (timed) MV_CUDA(cudaEventRecord(evRays, stream));
+            if (const int rc = castRays(false, sp.active)) return rc;
+            if (final) { if (const int rc = castRays(true, nullptr)) return rc; }
+        }
+        if (const int rc = endTimes(dep ? Timed::Union : Timed::Split, timed, final, nRays > 0)) return rc;
+        return (nRays && !async) ? downloadRays(stream) : MV_OK;
     }
     // the last event of a call (ev[2], only when `timed`) and what its events bracket, for readKernelTimes
-    int endTimes(Timed kind, bool timed = true, bool hadFinal = false) {
+    int endTimes(Timed kind, bool timed = true, bool hadFinal = false, bool hadRays = false) {
         if (timed) MV_CUDA(cudaEventRecord(ev[2], stream));
         timedAs = kind;
         lastHadFinal = timed && hadFinal;
+        lastHadRays = timed && hadRays;
         return MV_OK;
     }
     // the masked raster launch over the terminal rows: every (view, band) item of an env whose d_dones byte is set, into the final-frame
@@ -997,13 +1040,15 @@ struct mv_engine {
     // (the dependent launch) only their union is meaningful: {-1, whole call}
     void readKernelTimes() {
         if (cudaEventQuery(ev[2]) != cudaSuccess) return;
-        lastMs[0] = -1.0f; lastMs[1] = 0.0f; lastFinalMs = 0.0f;
+        lastMs[0] = -1.0f; lastMs[1] = 0.0f; lastFinalMs = 0.0f; lastRaysMs = 0.0f;
+        const cudaEvent_t end = lastHadRays ? evRays : ev[2];  // the ray launches come last and are timed on their own
         switch (timedAs) {
-        case Timed::Union: cudaEventElapsedTime(&lastMs[1], ev[0], ev[2]); break;
-        case Timed::Split: cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], lastHadFinal ? evFinal : ev[2]); break;
-        case Timed::FirstOnly: cudaEventElapsedTime(&lastMs[0], ev[0], ev[2]); break;
+        case Timed::Union: cudaEventElapsedTime(&lastMs[1], ev[0], end); break;
+        case Timed::Split: cudaEventElapsedTime(&lastMs[0], ev[0], ev[1]); cudaEventElapsedTime(&lastMs[1], ev[1], lastHadFinal ? evFinal : end); break;
+        case Timed::FirstOnly: cudaEventElapsedTime(&lastMs[0], ev[0], end); break;
         }
-        if (lastHadFinal) cudaEventElapsedTime(&lastFinalMs, evFinal, ev[2]);
+        if (lastHadFinal) cudaEventElapsedTime(&lastFinalMs, evFinal, end);
+        if (lastHadRays) cudaEventElapsedTime(&lastRaysMs, evRays, ev[2]);
     }
 
     int finishStep(bool copyObs, bool wait = true) {
@@ -1210,8 +1255,13 @@ struct mv_engine {
         if (toStore) return endTimes(Timed::FirstOnly);
         if (const int rc = downloadState()) return rc;  // the loaded rows, while the views are drawn again
         MV_CUDA(cudaEventRecord(ev[1], stream));
-        const int rc = launchRaster(false, nullptr);
-        return rc ? rc : endTimes(Timed::Split);
+        int rc = launchRaster(false, nullptr);
+        if (!rc && nRays) {  // the loaded envs' rays, behind the redraw (no terminal rays: the store keeps no terminal rows)
+            MV_CUDA(cudaEventRecord(evRays, stream));
+            rc = castRays(false, nullptr);
+        }
+        if (!rc) rc = endTimes(Timed::Split, true, false, nRays > 0);
+        return (rc || !nRays) ? rc : downloadRays(stream);
     }
     // a state load or an env restart ends like a host-facing step: `launch` enqueues its kernel with every view drawn again behind it
     // (the views it did not change yield the same bytes), `whileDrawing` is the host's part, run while the device works, and frames and
@@ -1399,6 +1449,8 @@ struct mv_engine {
         d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
         d_state.free(); h_state.free();
         if (evState) { cudaEventDestroy(evState); evState = nullptr; }
+        d_rayDirs.free(); d_rayDist.free(); d_rayTag.free(); h_rayDist.free(); h_rayTag.free();
+        if (evRays) { cudaEventDestroy(evRays); evRays = nullptr; }
         for (auto &e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
         if (evFinal) { cudaEventDestroy(evFinal); evFinal = nullptr; }
         for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); p.levelIds.free(); }
@@ -1769,6 +1821,20 @@ int mv_reset(mv_handle h) {
             }
             std::memset(h->h_state.p, 0, sizeof(float) * n);
         }
+        if (h->nRays) {  // the fan, and the live and terminal rays: zero until cast
+            const size_t n = h->rayBlock();
+            if (h->d_rayDirs.alloc(size_t(h->nRays) * 3) != cudaSuccess || h->d_rayDist.alloc(n) != cudaSuccess || h->d_rayTag.alloc(n) != cudaSuccess ||
+                h->h_rayDist.alloc(n) != cudaSuccess || h->h_rayTag.alloc(n) != cudaSuccess ||
+                cudaMemcpy(h->d_rayDirs.p, h->rayDirs.data(), sizeof(float) * h->rayDirs.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemset(h->d_rayDist.p, 0, sizeof(float) * n) != cudaSuccess || cudaMemset(h->d_rayTag.p, 0, sizeof(uint16_t) * n) != cudaSuccess ||
+                cudaEventCreate(&h->evRays) != cudaSuccess) {
+                h->d_rayDirs.free(); h->d_rayDist.free(); h->d_rayTag.free(); h->h_rayDist.free(); h->h_rayTag.free();
+                h->setError("rays: allocation failed");
+                return MV_ERR_CUDA;
+            }
+            std::memset(h->h_rayDist.p, 0, sizeof(float) * n);
+            std::memset(h->h_rayTag.p, 0, sizeof(uint16_t) * n);
+        }
         if (h->levelSet) h->scheduleBank();
         else regenerateNext(h);
         h->didReset = true;
@@ -2095,6 +2161,8 @@ int mv_fetch_obs(mv_handle h) {
         h->setError("state tensor download failed");
         return MV_ERR_CUDA;
     }
+    // the rays (live and terminal): always current in HBM
+    if (h->nRays && h->didReset && h->downloadRays(h->stream) != MV_OK) { h->setError("ray download failed"); return MV_ERR_CUDA; }
     // after a zero-copy host-facing step the host buffer holds the newer frames: no copy.  Rows copied from a caller's tensor are not the
     // engine's to vouch for: the next step with an active set draws every view again
     if (h->deviceObsFresh) {
@@ -2204,6 +2272,54 @@ int mv_final_state_tensors_device(mv_handle h, float **agents, float **envs, flo
     if (rc == MV_OK) stateTensorOuts(h, h->d_state.p, true, agents, envs, objects, rewards);
     return rc;
 }
+int mv_set_rays(mv_handle h, const float *dirs3, int n, float max_dist) {
+    if (!h) return MV_ERR_ARG;
+    if (h->didReset) { h->setError("mv_set_rays must be called before the first reset"); return MV_ERR_STATE; }
+    if (n < 0 || n > MV_MAX_RAYS) { h->setError("mv_set_rays: n out of range [0, MV_MAX_RAYS]"); return MV_ERR_ARG; }
+    if (n > 0 && !dirs3) { h->setError("mv_set_rays: null directions"); return MV_ERR_ARG; }
+    if (!std::isfinite(max_dist) || !(max_dist > 0.0f)) { h->setError("mv_set_rays: max_dist must be finite and > 0"); return MV_ERR_ARG; }
+    for (int i = 0; i < n; ++i) {
+        const float *d = dirs3 + 3 * i;
+        if (!std::isfinite(d[0]) || !std::isfinite(d[1]) || !std::isfinite(d[2]) || (d[0] == 0.0f && d[1] == 0.0f && d[2] == 0.0f)) {
+            h->setError("mv_set_rays: direction " + std::to_string(i) + " is zero or not finite");
+            return MV_ERR_ARG;
+        }
+    }
+    h->rayDirs.assign(dirs3, dirs3 + 3 * size_t(n));
+    h->nRays = n;
+    h->rayMaxDist = max_dist;
+    return MV_OK;
+}
+// the rays are on (and, for the terminal rays, option final_obs) and the engine reset
+static int rayCall(mv_handle h, bool terminal, const char *fn) {
+    if (!h) return MV_ERR_ARG;
+    if (!h->nRays || (terminal && !h->wantFinal)) {
+        h->setError(std::string(fn) + (terminal ? ": the rays or option final_obs are off" : ": the rays are off"));
+        return MV_ERR_ARG;
+    }
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+int mv_rays_host(mv_handle h, const float **dist, const uint16_t **tag) {
+    const int rc = rayCall(h, false, "mv_rays_host");
+    if (rc == MV_OK) { if (dist) *dist = h->h_rayDist.p; if (tag) *tag = h->h_rayTag.p; }
+    return rc;
+}
+int mv_rays_device(mv_handle h, float **dist, uint16_t **tag) {
+    const int rc = rayCall(h, false, "mv_rays_device");
+    if (rc == MV_OK) { if (dist) *dist = h->d_rayDist.p; if (tag) *tag = h->d_rayTag.p; }
+    return rc;
+}
+int mv_final_rays_host(mv_handle h, const float **dist, const uint16_t **tag) {
+    const int rc = rayCall(h, true, "mv_final_rays_host");
+    if (rc == MV_OK) { if (dist) *dist = h->h_rayDist.p + h->rayCount(); if (tag) *tag = h->h_rayTag.p + h->rayCount(); }
+    return rc;
+}
+int mv_final_rays_device(mv_handle h, float **dist, uint16_t **tag) {
+    const int rc = rayCall(h, true, "mv_final_rays_device");
+    if (rc == MV_OK) { if (dist) *dist = h->d_rayDist.p + h->rayCount(); if (tag) *tag = h->d_rayTag.p + h->rayCount(); }
+    return rc;
+}
 int mv_set_obs_buffer(mv_handle h, uint8_t *d_obs, float *d_depth) {
     MV_ON_DEVICE(h)
     // the pointer is a launch parameter: steps already enqueued keep writing the previous buffer, the next step writes the new one.  No
@@ -2299,6 +2415,7 @@ int mv_fault_word(mv_handle h, int32_t *out) {  // no device round trip: the ste
 int mv_kernel_launches(mv_handle h, int64_t *out) { if (!h || !out) return MV_ERR_ARG; *out = h->launches; return MV_OK; }
 int mv_last_kernel_ms(mv_handle h, float *out2) { if (!h || !out2) return MV_ERR_ARG; out2[0] = h->lastMs[0]; out2[1] = h->lastMs[1]; return MV_OK; }
 int mv_last_final_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_ARG; *out = h->lastFinalMs; return MV_OK; }
+int mv_last_rays_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_ARG; *out = h->lastRaysMs; return MV_OK; }
 
 int mv_close(mv_handle h) {
     if (!h) return MV_ERR_ARG;

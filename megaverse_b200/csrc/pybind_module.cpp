@@ -274,6 +274,23 @@ public:
         d["rewards"] = py::array_t<float>({numEnvs_, MV_STATE_REWARD_ROWS, 4}, p[3], py::none{});
         return d;
     }
+    // (extension) ray sensors (mv_set_rays): directions float32 [R,3] in camera space, before the first reset
+    void setRays(py::array_t<float, py::array::c_style | py::array::forcecast> dirs, float maxDist) {
+        alive();
+        if (dirs.size() % 3 != 0) throw std::invalid_argument("set_rays: directions must hold 3 floats per ray");
+        const int n = int(dirs.size() / 3);
+        check(mv_set_rays(h__, n ? dirs.data() : nullptr, n, maxDist));
+        numRays_ = n;
+    }
+    // (dist float32 [N,R], tag uint16 [N,R]), views of the engine's pinned rays; the terminal rays with option final_obs as well
+    py::tuple getRays(bool terminal) {
+        alive();
+        const float *d = nullptr;
+        const uint16_t *t = nullptr;
+        check(terminal ? mv_final_rays_host(h__, &d, &t) : mv_rays_host(h__, &d, &t));
+        const int N = int(masks_.size());
+        return py::make_tuple(py::array_t<float>({N, numRays_}, d, py::none{}), py::array_t<uint16_t>({N, numRays_}, t, py::none{}));
+    }
     void setNextLevels(const std::vector<int32_t> &envs, const std::vector<int32_t> &levels) {
         alive();
         if (envs.size() != levels.size()) throw std::invalid_argument("set_next_levels: envs and levels differ in length");
@@ -327,6 +344,7 @@ private:
     mv_handle h__ = nullptr;
     int numEnvs_, numAgentsPerEnv_, w_, h_;
     int renderW_ = 768, renderH_ = 432;
+    int numRays_ = 0;
     const uint8_t *hires_ = nullptr;
     std::vector<int32_t> masks_;
 };
@@ -380,6 +398,12 @@ PYBIND11_MODULE(megaverse, m) {
              "(option level_set) env envs[i] plays level levels[i] in its next episode, once; followed by reset_envs(envs) it starts them on those levels now")
         .def("get_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(false); },
              "dict of float32 views (option state_tensors): agents [N,16], envs [E,16], objects [E,128,4], rewards [E,128,4]")
+        .def("set_rays", &MegaverseGym::setRays, py::arg("directions"), py::arg("max_distance"),
+             "ray sensors, before the first reset: float32 [R,3] camera-space directions (x right, y up, -z forward), R in 0..256")
+        .def("get_rays", [](MegaverseGym &g) { return g.getRays(false); },
+             "(dist float32 [N,R], tag uint16 [N,R]): distance to the first front face along each ray (0: none) and its MV_SEG_* << 8 | index")
+        .def("get_final_rays", [](MegaverseGym &g) { return g.getRays(true); },
+             "the terminal rays (rays and option final_obs): cast from the scene each env's last episode ended on, same pair")
         .def("get_final_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(true); },
              "the terminal rows (options state_tensors and final_obs): the state each env's last episode ended on, same dict")
         .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),

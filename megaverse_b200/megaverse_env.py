@@ -71,7 +71,8 @@ class MegaverseEnv(Env):
     SKIP_UNFIT_LEVELS = False
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
-                 action_repeat=1, segmentation=False, num_levels=None, start_level=0, state_tensors=False):
+                 action_repeat=1, segmentation=False, num_levels=None, start_level=0, state_tensors=False,
+                 ray_directions=None, ray_max_distance=120.0):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
@@ -85,6 +86,10 @@ class MegaverseEnv(Env):
         # (extension) state_tensors=True: state_tensors() gives the state behind the current frames (agents, envs, objects, rewards; option
         # "state_tensors"), and with final_observation=True the infos of done agents carry 'final_state', the agent's row of the state the
         # episode ended on
+        # (extension) ray_directions=float32 [R, 3] (camera space: x right, y up, -z forward; megaverse_b200.rays builds fans and rings):
+        # every agent casts these rays against its env's drawn scene, up to ray_max_distance; ray_observations() gives each ray's hit
+        # distance and segmentation tag, and with final_observation=True the infos of done agents carry 'final_rays', the agent's rays
+        # cast from the scene the episode ended on.  step()'s return values do not change
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -124,6 +129,11 @@ class MegaverseEnv(Env):
         self.state_tensors_enabled = bool(state_tensors)
         if self.state_tensors_enabled:
             self.env.set_option("state_tensors", 1)
+        self.num_rays = 0
+        if ray_directions is not None:
+            dirs = np.ascontiguousarray(ray_directions, dtype=np.float32).reshape(-1, 3)
+            self.env.set_rays(dirs, float(ray_max_distance))
+            self.num_rays = len(dirs)
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
         self.num_levels = None if num_levels is None else int(num_levels)
@@ -169,6 +179,12 @@ class MegaverseEnv(Env):
         "rewards": float32[num_envs, 128, 4]}: the state the current observations show, rows as in include/megaverse_b200.h.  Views of engine
         memory, valid until the next step."""
         return self.env.get_state_tensors()
+
+    def ray_observations(self):
+        """(extension, ray_directions given) (dist float32[num_agents, R], tag uint16[num_agents, R]) for the current observations: the
+        distance along each ray to the first front face it meets (0: none within ray_max_distance) and that drawable's MV_SEG_* class << 8 |
+        index (0: none).  Views of engine memory, valid until the next step."""
+        return self.env.get_rays()
 
     def check_faults(self):
         """raise if the engine latched a fault bit (one pinned-memory read, no device round trip)"""
@@ -217,6 +233,7 @@ class MegaverseEnv(Env):
             reasons = self.env.get_done_reasons()
             final = self.env.get_final_observations()
             final_state = self.env.get_final_state_tensors()['agents'] if self.state_tensors_enabled else None
+            final_rays = self.env.get_final_rays() if self.num_rays else None
         dones, infos = [], []
         for env_i in range(self.num_envs):
             done = bool(env_dones[env_i])
@@ -235,6 +252,8 @@ class MegaverseEnv(Env):
                         infos[view]['truncated'] = int(reasons[env_i]) in (1, 3)
                         if final_state is not None:
                             infos[view]['final_state'] = final_state[view].copy()
+                        if final_rays is not None:
+                            infos[view]['final_rays'] = (final_rays[0][view].copy(), final_rays[1][view].copy())
             else:
                 infos.extend([{} for _ in range(self.num_agents_per_env)])
 
