@@ -477,6 +477,17 @@ int mv_debug_render_instances(const float *view16, const float *inst18, int n, i
  * a null view, instance, opts or rgba pointer or any value outside these ranges. */
 int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n, int w, int h, const int *opts, uint8_t *rgba, float *depth,
                                  uint16_t *seg, unsigned long long *stats);
+/* Cast rays over caller-supplied scenes through the engine's ray launch (the one every drawing step enqueues): E envs of A agents in
+ * one launch.  views16 = float[E*A][16] world-to-camera matrices; inst18 = float[E][stride][18] rows (mesh, colour, 16 model floats
+ * column-major) and tags = int32[E][stride], the segmentation tag of each row (the rays skip the rows tagged MV_SEG_AGENT << 8 | agent
+ * of the casting agent); counts = int32[E], the rows of each env cast against (the rest are not read); dirs3 = float[R][3] camera-space
+ * directions, used as given; env_mask = uint8[E] or NULL: envs whose byte is 0 are not cast.  dist float[E*A][R] and tag uint16[E*A][R]
+ * are in/out: uploaded first, so the rows of envs not cast come back as the caller filled them.  Host pointers; synchronous.
+ * MV_ERR_ARG for a null pointer (env_mask apart), E outside 1..65536, A outside 1..MV_MAX_AGENTS, R outside 1..MV_MAX_RAYS, stride
+ * outside 1..65536 or E * stride above 2^22, a count outside 0..stride, a cast row's mesh not one of 0..4, or max_dist not finite and
+ * > 0; MV_ERR_CUDA when the device fails. */
+int mv_debug_cast_rays(const float *views16, const float *inst18, const int32_t *tags, const int32_t *counts, int E, int A, int stride,
+                       const float *dirs3, int R, float max_dist, const uint8_t *env_mask, float *dist, uint16_t *tag);
 /* host-only (no CUDA needed): run the level generator for the env RNG stream seeded with env_seed and dump the level of
  * episode `episode` (mv_debug_get_level layout, followed by each agent's 9 spawn-basis floats as bit patterns) */
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *param_keys,

@@ -67,6 +67,7 @@ def lib():
         L.mv_debug_warp_agent.argtypes = [vp, ci, ci, vp, vp]
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
         L.mv_debug_render_instances_ex.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, vp, vp]
+        L.mv_debug_cast_rays.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, ci, cf, vp, vp, vp]
         L.mv_debug_bzset.argtypes = [vp, ci, vp, ci]
         L.mv_debug_generate_level.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp, ci]
         L.mv_states_create.argtypes = [vp, ci, C.POINTER(ci)]
@@ -99,7 +100,7 @@ EXPORTS = [
     "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device", "mv_set_next_levels", "mv_level_set_pick",
     "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
     "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
-    "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms",
+    "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms", "mv_debug_cast_rays",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -581,6 +582,31 @@ def render_instances(view16, inst18, w, h, want_depth=False, fast=None, segmenta
             raise MegaverseError(rc, "mv_debug_render_instances_ex failed")
         out += ([seg] if segmentation else []) + ([st] if stats else [])
     return tuple(out) if len(out) > 1 else rgba
+
+
+def cast_rays(views, inst18, tags, counts, dirs, max_dist, env_mask=None, dist=None, tag=None):
+    """debug: cast rays over caller-supplied scenes through the engine's ray launch (mv_debug_cast_rays).  views float32[E, A, 16],
+    inst18 float32[E, stride, 18], tags int32[E, stride], counts int32[E], dirs float32[R, 3]; env_mask uint8[E] or None.  dist / tag
+    (float32 / uint16 [E * A, R]) are what the launch starts from (zeros when None): rows of envs the mask leaves out come back as given.
+    Returns (dist, tag)."""
+    views = np.ascontiguousarray(views, dtype=np.float32)
+    E, A = views.shape[0], views.shape[1]
+    views = views.reshape(E * A, 16)
+    inst18 = np.ascontiguousarray(inst18, dtype=np.float32)
+    stride = inst18.shape[1]
+    tags = np.ascontiguousarray(tags, dtype=np.int32)
+    counts = np.ascontiguousarray(counts, dtype=np.int32)
+    dirs = np.ascontiguousarray(dirs, dtype=np.float32).reshape(-1, 3)
+    assert inst18.shape == (E, stride, 18) and tags.shape == (E, stride) and counts.shape == (E,)
+    R = dirs.shape[0]
+    dist = np.zeros((E * A, R), dtype=np.float32) if dist is None else np.array(dist, dtype=np.float32).reshape(E * A, R)
+    tag = np.zeros((E * A, R), dtype=np.uint16) if tag is None else np.array(tag, dtype=np.uint16).reshape(E * A, R)
+    mask = None if env_mask is None else np.ascontiguousarray(env_mask, dtype=np.uint8).reshape(E)
+    rc = lib().mv_debug_cast_rays(views.ctypes.data, inst18.ctypes.data, tags.ctypes.data, counts.ctypes.data, E, A, stride, dirs.ctypes.data, R,
+                                  float(max_dist), None if mask is None else mask.ctypes.data, dist.ctypes.data, tag.ctypes.data)
+    if rc != MV_OK:
+        raise MegaverseError(rc, "mv_debug_cast_rays failed")
+    return dist, tag
 
 
 def generate_level(scenario, num_agents, env_seed, episode, params=None):

@@ -2695,6 +2695,53 @@ int mv_debug_render_instances(const float *view16, const float *inst18, int n, i
     return mv_debug_render_instances_ex(view16, inst18, n, w, h, opts, rgba, depth, nullptr, nullptr);
 }
 
+int mv_debug_cast_rays(const float *views16, const float *inst18, const int32_t *tags, const int32_t *counts, int E, int A, int stride,
+                       const float *dirs3, int R, float max_dist, const uint8_t *env_mask, float *dist, uint16_t *tag) {
+    if (!views16 || !inst18 || !tags || !counts || !dirs3 || !dist || !tag) return MV_ERR_ARG;
+    if (E < 1 || E > 65536 || A < 1 || A > MV_MAX_AGENTS || R < 1 || R > MV_MAX_RAYS || stride < 1 || stride > 65536) return MV_ERR_ARG;
+    if (size_t(E) * size_t(stride) > (size_t(1) << 22) || !std::isfinite(max_dist) || !(max_dist > 0.0f)) return MV_ERR_ARG;
+    // the engine's layouts: rows [E][stride] (the entries below the env's count are cast, the rest are not read), counts [E][8] with the
+    // number drawn in [1]
+    std::vector<MvInstance> inst(size_t(E) * size_t(stride));
+    std::vector<int32_t> cnt(size_t(E) * 8, 0);
+    for (int e = 0; e < E; ++e) {
+        if (counts[e] < 0 || counts[e] > stride) return MV_ERR_ARG;
+        cnt[size_t(e) * 8 + 1] = counts[e];
+        for (int i = 0; i < counts[e]; ++i) {
+            const size_t r = size_t(e) * size_t(stride) + size_t(i);
+            const float mesh = inst18[r * 18];
+            if (!(mesh >= 0.0f && mesh <= 4.0f) || mesh != std::floor(mesh)) return MV_ERR_ARG;
+            MvInstance &d = inst[r];
+            d.mesh = int(mesh); d.color = 0;
+            std::memcpy(d.model, inst18 + r * 18 + 2, 64);
+            d.pad[0] = tags[r]; d.pad[1] = 0;
+        }
+    }
+    const size_t nv = size_t(E) * size_t(A), nr = nv * size_t(R);
+    MvInstance *dInst = nullptr; int32_t *dCnt = nullptr; float *dViews = nullptr, *dDirs = nullptr, *dDist = nullptr; uint8_t *dMask = nullptr;
+    uint16_t *dTag = nullptr;
+    bool ok = cudaMalloc(&dInst, sizeof(MvInstance) * inst.size()) == cudaSuccess && cudaMalloc(&dCnt, sizeof(int32_t) * cnt.size()) == cudaSuccess &&
+              cudaMalloc(&dViews, nv * 64) == cudaSuccess && cudaMalloc(&dDirs, size_t(R) * 12) == cudaSuccess &&
+              cudaMalloc(&dDist, nr * 4) == cudaSuccess && cudaMalloc(&dTag, nr * 2) == cudaSuccess &&
+              (!env_mask || cudaMalloc(&dMask, size_t(E)) == cudaSuccess);
+    ok = ok && cudaMemcpy(dInst, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dCnt, cnt.data(), sizeof(int32_t) * cnt.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dViews, views16, nv * 64, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dDirs, dirs3, size_t(R) * 12, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dDist, dist, nr * 4, cudaMemcpyHostToDevice) == cudaSuccess && cudaMemcpy(dTag, tag, nr * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
+         (!env_mask || cudaMemcpy(dMask, env_mask, size_t(E), cudaMemcpyHostToDevice) == cudaSuccess);
+    if (ok) {
+        // the engine's launch (Engine::castRays), on the legacy stream
+        mvray::RayParams rp;
+        rp.instances = dInst; rp.instCounts = dCnt; rp.views = dViews; rp.dirs = dDirs; rp.envMask = dMask;
+        rp.dist = dDist; rp.tag = dTag; rp.instStride = stride; rp.E = E; rp.A = A; rp.R = R; rp.maxDist = max_dist;
+        ok = mvray::castRays(rp, nullptr) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess &&
+             cudaMemcpy(dist, dDist, nr * 4, cudaMemcpyDeviceToHost) == cudaSuccess && cudaMemcpy(tag, dTag, nr * 2, cudaMemcpyDeviceToHost) == cudaSuccess;
+    }
+    cudaFree(dInst); cudaFree(dCnt); cudaFree(dViews); cudaFree(dDirs); cudaFree(dDist); cudaFree(dTag); cudaFree(dMask);
+    return ok ? MV_OK : MV_ERR_CUDA;
+}
+
 // host-only (no CUDA): run the product's level generator for env stream `env_seed` and dump episode `episode`'s level in
 // the mv_debug_get_level layout.  Lets the CPU test-suite compare level generation with the oracle without a GPU.
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys, const float *vals, int nparams,

@@ -7,6 +7,7 @@
 namespace {
 
 constexpr float kBoundMargin = 1.0f / 64.0f;  // the prefilter's margin, as in csrc/ray_kernel.cu (it changes no result)
+constexpr float kEdgeTol = 1.0f / 262144.0f;   // the widening of the barycentric bounds per object unit of |o - p0|, as in csrc/ray_kernel.cu
 
 Vec3 cross3(Vec3 a, Vec3 b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
 
@@ -46,19 +47,24 @@ void slab(Vec3 o, Vec3 v, Vec3 h, float &tin, float &tout) {
     }
 }
 
-bool triHit(Vec3 o, Vec3 v, Vec3 p0, Vec3 p1, Vec3 p2, float &t) {
+// s = -1 for a mirrored model: the faces counted are those clockwise seen from the origin.  0: no hit; 1: a hit within the exact bounds;
+// 2: within the bounds widened by tol only (a fallback, see castFan)
+int triHit(Vec3 o, Vec3 v, Vec3 p0, Vec3 p1, Vec3 p2, float s, float &t) {
     const Vec3 e1 = p1 - p0, e2 = p2 - p0;
     const Vec3 pv = cross3(v, e2);
-    const float det = dot(e1, pv);
-    if (!(det > 0.0f)) return false;
+    const float det = s * dot(e1, pv);
+    if (!(det > 0.0f)) return 0;
     const Vec3 tv = o - p0;
-    const float u = dot(tv, pv);
-    if (u < 0.0f || u > det) return false;
+    float a = 1.0f;
+    a += std::fabs(tv.x); a += std::fabs(tv.y); a += std::fabs(tv.z);
+    const float tol = det * (a * kEdgeTol);
+    const float u = s * dot(tv, pv);
+    if (u < -tol || u > det + tol) return 0;
     const Vec3 qv = cross3(tv, e1);
-    const float w = dot(v, qv);
-    if (w < 0.0f || u + w > det) return false;
-    t = dot(e2, qv) / det;
-    return true;
+    const float w = s * dot(v, qv);
+    if (w < -tol || u + w > det + tol) return 0;
+    t = s * dot(e2, qv) / det;
+    return u < 0.0f || u > det || w < 0.0f || u + w > det ? 2 : 1;
 }
 
 Vec3 vertex(const MeshRef &m, int i) { return {bitsToFloat(m.vtx[i][0]), bitsToFloat(m.vtx[i][1]), bitsToFloat(m.vtx[i][2])}; }
@@ -69,9 +75,10 @@ void castFan(const Mat4 &view, const std::vector<Instance> &inst, const std::vec
     const Mat4 cam = inverted(view);
     const int own = agent < 0 ? -1 : (SEG_AGENT << 8 | agent);
     std::vector<Mat4> inv(inst.size());
-    std::vector<bool> finite(inst.size());
+    std::vector<bool> finite(inst.size()), mirrored(inst.size());
     for (size_t i = 0; i < inst.size(); ++i) {
         inv[i] = inverted(inst[i].model);
+        mirrored[i] = det4(inst[i].model) < 0.0f;
         bool f = true;
         for (int col = 0; col < 4; ++col)
             for (int row = 0; row < 3; ++row) f = f && std::isfinite(inv[i].c[col][row]);
@@ -88,20 +95,33 @@ void castFan(const Mat4 &view, const std::vector<Instance> &inst, const std::vec
             float tin, tout;
             if (inst[i].mesh == MESH_BOX) {
                 slab(o, v, {1.0f, 1.0f, 1.0f}, tin, tout);
-                if (tin > 0.0f && tin <= tout && tin <= best) { best = tin; bestTag = tags[i]; }
+                const float th = mirrored[i] ? tout : tin;  // a mirrored box shows its far faces
+                if (th > 0.0f && tin <= tout && th <= best) { best = th; bestTag = tags[i]; }
                 continue;
             }
             const float ys = inst[i].mesh == MESH_CAPSULE ? 2.0f : 1.0f;
             slab(o, v, {1.0f + kBoundMargin, ys + kBoundMargin, 1.0f + kBoundMargin}, tin, tout);
             if (!(tin <= tout && tout > 0.0f)) continue;
             const MeshRef m = meshRef(inst[i].mesh);
+            const float s = mirrored[i] ? -1.0f : 1.0f;
+            // hits within the exact bounds count as they are; a hit within the widened bounds only counts when no triangle of the
+            // instance is hit within the exact ones, so the widening closes the cracks between its faces and moves no exact hit
+            float wide = best;
+            bool exact = false, widened = false, nearer = false;
             for (int k = 0; k + 2 < m.ni; k += 3) {
                 float t;
-                if (triHit(o, v, vertex(m, m.idx[k]), vertex(m, m.idx[k + 1]), vertex(m, m.idx[k + 2]), t) && t > 0.0f && t <= best) {
-                    best = t;
-                    bestTag = tags[i];
+                const int h = triHit(o, v, vertex(m, m.idx[k]), vertex(m, m.idx[k + 1]), vertex(m, m.idx[k + 2]), s, t);
+                if (!h || !(t > 0.0f)) continue;
+                if (h == 1) {
+                    exact = true;
+                    if (t <= best) { best = t; nearer = true; }
+                } else if (t <= wide) {
+                    wide = t;
+                    widened = true;
                 }
             }
+            if (!exact && widened) { best = wide; nearer = true; }
+            if (nearer) bestTag = tags[i];
         }
         dist[r] = bestTag >= 0 ? best : 0.0f;
         tag[r] = uint16_t(bestTag >= 0 ? bestTag : 0);
