@@ -488,6 +488,21 @@ int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n
  * > 0; MV_ERR_CUDA when the device fails. */
 int mv_debug_cast_rays(const float *views16, const float *inst18, const int32_t *tags, const int32_t *counts, int E, int A, int stride,
                        const float *dirs3, int R, float max_dist, const uint8_t *env_mask, float *dist, uint16_t *tag);
+/* Run chosen contact cases through the step kernel's own collision code: the per-step candidate gather and culling envelope, then one
+ * character-controller query, one warp per case (synchronous, host pointers).  A case is a collider set in collider order -- statics
+ * [0, n_static_pre), the objects, statics [n_static_pre, n_static), the A agents' capsules -- and one query by agent `agent`.
+ *   hdr8     int32[n][8]   {n_static_pre, n_static, n_obj, A, mode (0 sweep, 1 recover, 2 controller step), agent, 0, 0}
+ *   boxes10  float[n][2 * MV_MAX_OBJECTS][10]  rows [0, n_static) the statics, rows MV_MAX_OBJECTS + [0, n_obj) the objects:
+ *            centre[3], half extents[3], solid (statics) / enabled (objects) 0|1, rotated about Y 0|1 (statics only), local x axis (ax, az)
+ *   agents3  float[n][MV_MAX_AGENTS][3]  capsule centres; the querying agent's own is where its envelope is centred (mode 2: the query's)
+ *   query20  float[n][20]  sweep: from[3], to[3], filterDir[3], minSlopeDot; recover: point[3]; step: pos[3], hvel[3], vvel, voff, stepOff,
+ *            jumpSpeed, jumpAxis[3], wasOnGround 0|1, wasJumping 0|1, dt > 0, maxSlopeCos
+ * out_i8 int32[n][8] = {candidates, fault bits (MV_FAULT_CAND_OVERFLOW, MV_FAULT_ENVELOPE), hit / penetrated / wasOnGround, winning collider
+ * index (-1 for none), winning feature (sweep: 0..22 for boxes, 0 for capsules; else -1), wasJumping, 0, 0}; out_f16 float[n][16] = sweep:
+ * fraction, normal[3]; recover: delta[3]; step: pos[3], hvel[3], vvel, voff, stepOff, jumpSpeed; the rest 0.  MV_ERR_ARG, before any device
+ * work, for a null pointer, n outside 1..65536, counts above MV_MAX_OBJECTS / MV_MAX_AGENTS, a bad mode or agent, a negative half
+ * extent, a flag not 0 or 1, a rotated object, dt <= 0 or any non-finite float that the case uses; MV_ERR_CUDA when the device fails. */
+int mv_debug_kcc(const int32_t *hdr8, const float *boxes10, const float *agents3, const float *query20, int n, int32_t *out_i8, float *out_f16);
 /* host-only (no CUDA needed): run the level generator for the env RNG stream seeded with env_seed and dump the level of
  * episode `episode` (mv_debug_get_level layout, followed by each agent's 9 spawn-basis floats as bit patterns) */
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *param_keys,

@@ -14,6 +14,8 @@ MV_OK, MV_ERR_ARG, MV_ERR_CUDA, MV_ERR_CAPACITY, MV_ERR_STATE = 0, -1, -2, -3, -
 MV_END_NONE, MV_END_TIME, MV_END_SOLVED, MV_END_REQUESTED = 0, 1, 2, 3  # done_reasons(): why an episode ended
 # segmentation(): a pixel is class << 8 | index of the drawable behind it, 0 where nothing was drawn
 MV_SEG_NONE, MV_SEG_STATIC, MV_SEG_TERRAIN, MV_SEG_OBJECT, MV_SEG_AGENT, MV_SEG_REWARD = 0, 1, 2, 3, 4, 5
+MAX_OBJECTS, MAX_AGENTS, MAX_CAND = 128, 8, 96  # MV_MAX_OBJECTS, MV_MAX_AGENTS, MV_MAX_CAND (csrc/mv_types.h)
+MV_FAULT_ENVELOPE, MV_FAULT_CAND_OVERFLOW = 16, 32
 
 
 class MegaverseError(RuntimeError):
@@ -68,6 +70,7 @@ def lib():
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
         L.mv_debug_render_instances_ex.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, vp, vp]
         L.mv_debug_cast_rays.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, ci, cf, vp, vp, vp]
+        L.mv_debug_kcc.argtypes = [vp, vp, vp, vp, ci, vp, vp]
         L.mv_debug_bzset.argtypes = [vp, ci, vp, ci]
         L.mv_debug_generate_level.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp, ci]
         L.mv_states_create.argtypes = [vp, ci, C.POINTER(ci)]
@@ -101,6 +104,7 @@ EXPORTS = [
     "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
     "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
     "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms", "mv_debug_cast_rays",
+    "mv_debug_kcc",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -607,6 +611,24 @@ def cast_rays(views, inst18, tags, counts, dirs, max_dist, env_mask=None, dist=N
     if rc != MV_OK:
         raise MegaverseError(rc, "mv_debug_cast_rays failed")
     return dist, tag
+
+
+def kcc_cases(hdr, boxes, agents, query):
+    """debug: contact cases through the step kernel's candidate gather, sweep, recovery and controller step (mv_debug_kcc).  hdr int32[n, 8],
+    boxes float32[n, 2 * MAX_OBJECTS, 10], agents float32[n, MAX_AGENTS, 3], query float32[n, 20] in the layouts the header documents.
+    Returns (out_i int32[n, 8], out_f float32[n, 16])."""
+    hdr = np.ascontiguousarray(hdr, dtype=np.int32)
+    n = hdr.shape[0]
+    boxes = np.ascontiguousarray(boxes, dtype=np.float32)
+    agents = np.ascontiguousarray(agents, dtype=np.float32)
+    query = np.ascontiguousarray(query, dtype=np.float32)
+    assert hdr.shape == (n, 8) and boxes.shape == (n, 2 * MAX_OBJECTS, 10) and agents.shape == (n, MAX_AGENTS, 3) and query.shape == (n, 20)
+    out_i = np.zeros((n, 8), dtype=np.int32)
+    out_f = np.zeros((n, 16), dtype=np.float32)
+    rc = lib().mv_debug_kcc(hdr.ctypes.data, boxes.ctypes.data, agents.ctypes.data, query.ctypes.data, n, out_i.ctypes.data, out_f.ctypes.data)
+    if rc != MV_OK:
+        raise MegaverseError(rc, "mv_debug_kcc failed")
+    return out_i, out_f
 
 
 def generate_level(scenario, num_agents, env_seed, episode, params=None):

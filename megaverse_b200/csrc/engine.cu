@@ -2742,6 +2742,69 @@ int mv_debug_cast_rays(const float *views16, const float *inst18, const int32_t 
     return ok ? MV_OK : MV_ERR_CUDA;
 }
 
+int mv_debug_kcc(const int32_t *hdr8, const float *boxes10, const float *agents3, const float *query20, int n, int32_t *out_i8, float *out_f16) {
+    if (!hdr8 || !boxes10 || !agents3 || !query20 || !out_i8 || !out_f16 || n < 1 || n > 65536) return MV_ERR_ARG;
+    std::vector<MvBox> statics(size_t(n) * MV_MAX_OBJECTS);
+    std::vector<float> rot(size_t(n) * MV_MAX_OBJECTS * 2, 0.0f);
+    std::vector<MvObject> objects(size_t(n) * MV_MAX_OBJECTS);
+    std::memset(statics.data(), 0, statics.size() * sizeof(MvBox));
+    std::memset(objects.data(), 0, objects.size() * sizeof(MvObject));
+    auto finite = [](const float *p, int k) { for (int j = 0; j < k; ++j) if (!std::isfinite(p[j])) return false; return true; };
+    auto flag = [](float v) { return v == 0.0f || v == 1.0f; };
+    for (int c = 0; c < n; ++c) {
+        const int32_t *hd = hdr8 + size_t(c) * 8;
+        const int nsPre = hd[0], ns = hd[1], no = hd[2], A = hd[3], mode = hd[4], agent = hd[5];
+        if (ns < 0 || ns > MV_MAX_OBJECTS || nsPre < 0 || nsPre > ns || no < 0 || no > MV_MAX_OBJECTS || A < 1 || A > MV_MAX_AGENTS) return MV_ERR_ARG;
+        if (mode < mvk::kKccSweep || mode > mvk::kKccStep || agent < 0 || agent >= A) return MV_ERR_ARG;
+        const float *q = query20 + size_t(c) * 20;
+        const int nq = mode == mvk::kKccSweep ? 10 : mode == mvk::kKccRecover ? 3 : 17;
+        if (!finite(q, nq) || !finite(agents3 + size_t(c) * MV_MAX_AGENTS * 3, A * 3)) return MV_ERR_ARG;
+        if (mode == mvk::kKccStep && (!flag(q[13]) || !flag(q[14]) || !(q[15] > 0.0f))) return MV_ERR_ARG;
+        for (int j = 0; j < ns + no; ++j) {
+            const bool isStatic = j < ns;
+            const float *b = boxes10 + (size_t(c) * 2 * MV_MAX_OBJECTS + (isStatic ? j : MV_MAX_OBJECTS + j - ns)) * 10;
+            if (!finite(b, 10) || !flag(b[6]) || !flag(b[7]) || b[3] < 0.0f || b[4] < 0.0f || b[5] < 0.0f) return MV_ERR_ARG;
+            if (isStatic) {
+                MvBox &d = statics[size_t(c) * MV_MAX_OBJECTS + j];
+                std::memcpy(d.c, b, 12); std::memcpy(d.h, b + 3, 12);
+                d.flags = (b[6] != 0.0f ? MV_SOLID : 0) | (b[7] != 0.0f ? MV_ROTATED : 0);
+                rot[(size_t(c) * MV_MAX_OBJECTS + j) * 2] = b[8]; rot[(size_t(c) * MV_MAX_OBJECTS + j) * 2 + 1] = b[9];
+            } else {
+                if (b[7] != 0.0f) return MV_ERR_ARG;  // objects are axis-aligned
+                MvObject &d = objects[size_t(c) * MV_MAX_OBJECTS + j - ns];
+                std::memcpy(d.col_c, b, 12); std::memcpy(d.col_h, b + 3, 12);
+                d.enabled = b[6] != 0.0f;
+            }
+        }
+    }
+    int32_t *dHdr = nullptr, *dOutI = nullptr; MvBox *dStatics = nullptr; MvObject *dObjects = nullptr;
+    float *dRot = nullptr, *dAgents = nullptr, *dQuery = nullptr, *dOutF = nullptr;
+    const size_t nA = size_t(n) * MV_MAX_AGENTS * 3;
+    bool ok = cudaMalloc(&dHdr, size_t(n) * 32) == cudaSuccess && cudaMalloc(&dStatics, statics.size() * sizeof(MvBox)) == cudaSuccess &&
+              cudaMalloc(&dRot, rot.size() * 4) == cudaSuccess && cudaMalloc(&dObjects, objects.size() * sizeof(MvObject)) == cudaSuccess &&
+              cudaMalloc(&dAgents, nA * 4) == cudaSuccess && cudaMalloc(&dQuery, size_t(n) * 80) == cudaSuccess &&
+              cudaMalloc(&dOutI, size_t(n) * 32) == cudaSuccess && cudaMalloc(&dOutF, size_t(n) * 64) == cudaSuccess;
+    ok = ok && cudaMemcpy(dHdr, hdr8, size_t(n) * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dStatics, statics.data(), statics.size() * sizeof(MvBox), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dRot, rot.data(), rot.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dObjects, objects.data(), objects.size() * sizeof(MvObject), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dAgents, agents3, nA * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dQuery, query20, size_t(n) * 80, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (ok) {
+        mvk::KccCaseParams kp;
+        kp.hdr = dHdr; kp.statics = dStatics; kp.staticRot = dRot; kp.objects = dObjects; kp.agentPos = dAgents; kp.query = dQuery;
+        kp.outI = dOutI; kp.outF = dOutF;
+        const int smem = int(sizeof(mvk::WarpShared));
+        ok = cudaFuncSetAttribute(mvk::kccCaseKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess;
+        if (ok) mvk::kccCaseKernel<<<n, 32, smem>>>(kp);
+        ok = ok && cudaGetLastError() == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess &&
+             cudaMemcpy(out_i8, dOutI, size_t(n) * 32, cudaMemcpyDeviceToHost) == cudaSuccess &&
+             cudaMemcpy(out_f16, dOutF, size_t(n) * 64, cudaMemcpyDeviceToHost) == cudaSuccess;
+    }
+    cudaFree(dHdr); cudaFree(dStatics); cudaFree(dRot); cudaFree(dObjects); cudaFree(dAgents); cudaFree(dQuery); cudaFree(dOutI); cudaFree(dOutF);
+    return ok ? MV_OK : MV_ERR_CUDA;
+}
+
 // host-only (no CUDA): run the product's level generator for env stream `env_seed` and dump episode `episode`'s level in
 // the mv_debug_get_level layout.  Lets the CPU test-suite compare level generation with the oracle without a GPU.
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys, const float *vals, int nparams,

@@ -19,6 +19,8 @@
 // (min hit fraction, lowest collider index on ties).  Static colliders and movable-object records are staged into shared
 // memory with one TMA bulk copy each (cp.async.bulk + mbarrier).  Lane 0 commits state changes.
 #pragma once
+#include <type_traits>
+
 #include "bzset.h"
 #include "dev_math.cuh"
 #include "level_set.h"
@@ -331,16 +333,19 @@ struct ColliderView {
 };
 
 struct SweepHit { bool hit; float fraction; V3 normal; };
+struct SweepReport : SweepHit { int slot, feature; };  // mv_debug_kcc: the winner's candidate slot and its feature f (0 for capsules)
 
 // KinematicClosestNotMeConvexResultCallback over this agent's candidates.  Lanes first cull candidates against the swept
 // bounds (the broadphase), then the warp tests (surviving candidate, boundary feature) pairs in parallel; each
 // candidate's closest feature is found with a packed shared-memory atomicMin (t bits | feature), its lane re-evaluates
 // that one feature for the exact fraction and normal, applies the callback's slope filter, and a shuffle reduction picks
-// the closest candidate (ties: lowest collider index, i.e. the order a serial scan would have kept).
-__device__ SweepHit warpSweep(const ColliderView &cv, int self, V3 from, V3 to, V3 filterDir, float minSlopeDot, int lane) {
+// the closest candidate (ties: lowest collider index, i.e. the order a serial scan would have kept).  kReport (mv_debug_kcc only) also
+// returns the winner's slot and feature.
+template <bool kReport = false>
+__device__ std::conditional_t<kReport, SweepReport, SweepHit> warpSweep(const ColliderView &cv, int self, V3 from, V3 to, V3 filterDir, float minSlopeDot, int lane) {
     const V3 d = to - from;
     float bt = 1.0f;
-    int bi = 0x7fffffff;
+    int bi = 0x7fffffff, bf = 0;
     V3 bn = v3(0, 0, 0);
     WarpShared &S = *const_cast<WarpShared *>(cv.S);
     const float lx = from.x < to.x ? from.x : to.x, hx = from.x < to.x ? to.x : from.x;
@@ -399,7 +404,10 @@ __device__ SweepHit warpSweep(const ColliderView &cv, int self, V3 from, V3 to, 
                     rayRoundedBoxFeature(cv.toLocal(j, kind, from - c), cv.toLocal(j, kind, d), v3(h.x, h.y + kCapsuleHalfHeight, h.z), rhoBox, int(key & 31u), t, nn);
                     nn = cv.toWorld(j, kind, nn);
                 } else rayCapsule(from - c, d, 2.0f * kCapsuleHalfHeight, rhoCap, t, nn);
-                if (t < bt && !(dot(filterDir, nn) < minSlopeDot)) { bt = t; bi = j; bn = nn; }
+                if (t < bt && !(dot(filterDir, nn) < minSlopeDot)) {
+                    bt = t; bi = j; bn = nn;
+                    if constexpr (kReport) bf = int(key & 31u);
+                }
             }
         }
         __syncwarp();
@@ -409,17 +417,24 @@ __device__ SweepHit warpSweep(const ColliderView &cv, int self, V3 from, V3 to, 
         const float ot = __shfl_xor_sync(FULL, bt, off);
         const int oi = __shfl_xor_sync(FULL, bi, off);
         const float ox = __shfl_xor_sync(FULL, bn.x, off), oy = __shfl_xor_sync(FULL, bn.y, off), oz = __shfl_xor_sync(FULL, bn.z, off);
+        if constexpr (kReport) {
+            const int of = __shfl_xor_sync(FULL, bf, off);
+            if (ot < bt || (ot == bt && oi < bi)) bf = of;
+        }
         if (ot < bt || (ot == bt && oi < bi)) { bt = ot; bi = oi; bn = v3(ox, oy, oz); }
     }
-    SweepHit r;
+    std::conditional_t<kReport, SweepReport, SweepHit> r;
     r.hit = bi != 0x7fffffff;
     r.fraction = r.hit ? bt : 1.0f;
     r.normal = bn;
+    if constexpr (kReport) { r.slot = bi; r.feature = bf; }
     return r;
 }
 
-// first collider (index order) penetrating deeper than maxPenetrationDepth; returns push-out delta
-__device__ bool warpRecover(const ColliderView &cv, int self, V3 p, V3 &delta, int lane) {
+// first collider (index order) penetrating deeper than maxPenetrationDepth; returns push-out delta (and, when slotOut is given, that
+// collider's candidate slot: mv_debug_kcc only)
+template <bool kReport = false>
+__device__ bool warpRecover(const ColliderView &cv, int self, V3 p, V3 &delta, int lane, int *slotOut = nullptr) {
     for (int base = 0; base < cv.nc; base += 32) {
         const int j = base + lane;
         bool pen = false;
@@ -437,6 +452,7 @@ __device__ bool warpRecover(const ColliderView &cv, int self, V3 p, V3 &delta, i
         if (m) {
             const int src = __ffs(m) - 1;
             delta = v3(__shfl_sync(FULL, dl.x, src), __shfl_sync(FULL, dl.y, src), __shfl_sync(FULL, dl.z, src));
+            if constexpr (kReport) *slotOut = base + src;
             return true;
         }
     }
@@ -596,6 +612,68 @@ __device__ void kccPlayerStep(Kcc &k, const ColliderView &cv, int self, float dt
 #ifdef MV_KCC_COUNTERS
 #undef warpSweep
 #endif
+
+// ---------------------------------------------------------------- per-step collision candidates
+// The box an agent at p can move in within one step (0.2 step-up + jump, <= 55/15 fall, <= 5 push-outs): colliders whose bounds miss it
+// are left out of the step's sweeps and recoveries.  An agent that ends the step within 0.5 of its faces sets MV_FAULT_ENVELOPE.
+__device__ __forceinline__ V3 envelopeLo(V3 p) { return v3(p.x - 3.0f, p.y - 6.0f, p.z - 3.0f); }
+__device__ __forceinline__ V3 envelopeHi(V3 p) { return v3(p.x + 3.0f, p.y + 3.0f, p.z + 3.0f); }
+__device__ __forceinline__ bool leftEnvelope(V3 envLo, V3 envHi, V3 p) {
+    return p.x < envLo.x + 0.5f || p.x > envHi.x - 0.5f || p.y < envLo.y + 0.5f || p.y > envHi.y - 0.5f || p.z < envLo.z + 0.5f || p.z > envHi.z - 0.5f;
+}
+
+// Agent i's candidate colliders for the whole step into S.cand, in ascending collider order: everything whose bounds (grown by the
+// capsule) reach the envelope [envLo, envHi].  Statics come from global memory, objects and agents from S.  Returns the count, at most
+// MV_MAX_CAND; more sets MV_FAULT_CAND_OVERFLOW in S.env.faults.  slotCollider, when given, receives each slot's collider index.
+__device__ __forceinline__ int gatherCandidates(WarpShared &S, const MvBox *statics, const float *staticRot, int nsPre, int ns, int no, int A, int i,
+                                                V3 envLo, V3 envHi, int lane, int16_t *slotCollider = nullptr) {
+    int nc = 0;
+    const int n = ns + no + A;
+    for (int base = 0; base < n; base += 32) {
+        const int ci = base + lane;
+        bool keep = false;
+        int kind = 0, agentIdx = 0;
+        float rax = 1.0f, raz = 0.0f;
+        V3 c = v3(0, 0, 0), h = v3(0, 0, 0);
+        // collider order (= the reference's creation order, which decides ties): the first nsPre static boxes,
+        // the movable objects, the remaining static boxes, the agents
+        if (ci < nsPre || (ci >= nsPre + no && ci < ns + no)) {
+            const int si = ci < nsPre ? ci : ci - no;
+            const MvBox &sb = statics[si];  // global memory (L2 resident): scanned once per agent per step
+            if (sb.flags & MV_SOLID) {
+                keep = true; c = v3(sb.c[0], sb.c[1], sb.c[2]); h = v3(sb.h[0], sb.h[1], sb.h[2]);
+                if (sb.flags & MV_ROTATED) { kind = 2; rax = staticRot[size_t(si) * 2]; raz = staticRot[size_t(si) * 2 + 1]; }
+            }
+        } else if (ci < nsPre + no) {
+            const MvObject &ob = S.objects[ci - nsPre];
+            if (ob.enabled) { keep = true; c = v3(ob.col_c[0], ob.col_c[1], ob.col_c[2]); h = v3(ob.col_h[0], ob.col_h[1], ob.col_h[2]); }
+        } else if (ci < n && ci - ns - no != i) {
+            agentIdx = ci - ns - no;
+            const MvAgent &oa = S.agents[agentIdx];
+            keep = true; kind = 1; c = v3(oa.pos[0], oa.pos[1], oa.pos[2]);
+        }
+        if (keep) {
+            // agents may move up to an envelope of their own within this step: give capsules the same slack
+            V3 ext = kind != 1 ? v3(h.x + kCapsuleRadius, h.y + (kCapsuleHalfHeight + kCapsuleRadius), h.z + kCapsuleRadius)
+                               : v3(2.0f * kCapsuleRadius + 3.0f, 2.0f * (kCapsuleHalfHeight + kCapsuleRadius) + 6.0f, 2.0f * kCapsuleRadius + 3.0f);
+            if (kind == 2) { ext.x = (fabsf(rax) * h.x + fabsf(raz) * h.z) + kCapsuleRadius; ext.z = (fabsf(raz) * h.x + fabsf(rax) * h.z) + kCapsuleRadius; }
+            keep = !(envHi.x < c.x - ext.x || envLo.x > c.x + ext.x || envHi.y < c.y - ext.y || envLo.y > c.y + ext.y ||
+                     envHi.z < c.z - ext.z || envLo.z > c.z + ext.z);
+        }
+        const unsigned m = __ballot_sync(FULL, keep);
+        const int slotC = nc + __popc(m & ((1u << lane) - 1u));
+        if (keep && slotC < MV_MAX_CAND) {
+            WarpShared::Cand &cd = S.cand[slotC];
+            cd.c[0] = c.x; cd.c[1] = c.y; cd.c[2] = c.z; cd.h[0] = h.x; cd.h[1] = h.y; cd.h[2] = h.z; cd.kind = kind; cd.agent = agentIdx; cd.ax = rax; cd.az = raz;
+            if (slotCollider) slotCollider[slotC] = int16_t(ci);
+        }
+        nc += __popc(m);
+    }
+    if (nc > MV_MAX_CAND) { nc = MV_MAX_CAND; S.env.faults |= MV_FAULT_CAND_OVERFLOW; }
+    __syncwarp();
+    return nc;
+}
+
 
 // ---------------------------------------------------------------- helpers on shared state
 __device__ __forceinline__ M4 loadM4(const float *p) { M4 m;
@@ -1119,63 +1197,14 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
                 k.jumpAxis = v3(a.jump_axis[0], a.jump_axis[1], a.jump_axis[2]);
                 k.vvel = a.vvel; k.voff = a.voff; k.stepOff = a.step_off; k.jumpSpeed = a.jump_speed;
                 k.wasOnGround = a.was_on_ground != 0; k.wasJumping = a.was_jumping != 0;
-                // candidate colliders of this agent for the whole step: everything whose bounds (grown by the capsule) reach
-                // the envelope the controller can move in within one step (0.2 step-up + jump, <= 55/15 fall, <= 5 push-outs)
-                const V3 envLo = v3(k.pos.x - 3.0f, k.pos.y - 6.0f, k.pos.z - 3.0f), envHi = v3(k.pos.x + 3.0f, k.pos.y + 3.0f, k.pos.z + 3.0f);
-                {
-                    int nc = 0;
-                    const int n = ns + no + A, nsPre = L->n_static_pre;
-                    for (int base = 0; base < n; base += 32) {
-                        const int ci = base + lane;
-                        bool keep = false;
-                        int kind = 0, agentIdx = 0;
-                        float rax = 1.0f, raz = 0.0f;
-                        V3 c = v3(0, 0, 0), h = v3(0, 0, 0);
-                        // collider order (= the reference's creation order, which decides ties): the first nsPre static boxes,
-                        // the movable objects, the remaining static boxes, the agents
-                        if (ci < nsPre || (ci >= nsPre + no && ci < ns + no)) {
-                            const int si = ci < nsPre ? ci : ci - no;
-                            const MvBox &sb = statics[si];  // global memory (L2 resident): scanned once per agent per step
-                            if (sb.flags & MV_SOLID) {
-                                keep = true; c = v3(sb.c[0], sb.c[1], sb.c[2]); h = v3(sb.h[0], sb.h[1], sb.h[2]);
-                                if (sb.flags & MV_ROTATED) { kind = 2; rax = staticRot[size_t(si) * 2]; raz = staticRot[size_t(si) * 2 + 1]; }
-                            }
-                        } else if (ci < nsPre + no) {
-                            const MvObject &ob = S.objects[ci - nsPre];
-                            if (ob.enabled) { keep = true; c = v3(ob.col_c[0], ob.col_c[1], ob.col_c[2]); h = v3(ob.col_h[0], ob.col_h[1], ob.col_h[2]); }
-                        } else if (ci < n && ci - ns - no != i) {
-                            agentIdx = ci - ns - no;
-                            const MvAgent &oa = S.agents[agentIdx];
-                            keep = true; kind = 1; c = v3(oa.pos[0], oa.pos[1], oa.pos[2]);
-                        }
-                        if (keep) {
-                            // agents may move up to an envelope of their own within this step: give capsules the same slack
-                            V3 ext = kind != 1 ? v3(h.x + kCapsuleRadius, h.y + (kCapsuleHalfHeight + kCapsuleRadius), h.z + kCapsuleRadius)
-                                               : v3(2.0f * kCapsuleRadius + 3.0f, 2.0f * (kCapsuleHalfHeight + kCapsuleRadius) + 6.0f, 2.0f * kCapsuleRadius + 3.0f);
-                            if (kind == 2) { ext.x = (fabsf(rax) * h.x + fabsf(raz) * h.z) + kCapsuleRadius; ext.z = (fabsf(raz) * h.x + fabsf(rax) * h.z) + kCapsuleRadius; }
-                            keep = !(envHi.x < c.x - ext.x || envLo.x > c.x + ext.x || envHi.y < c.y - ext.y || envLo.y > c.y + ext.y ||
-                                     envHi.z < c.z - ext.z || envLo.z > c.z + ext.z);
-                        }
-                        const unsigned m = __ballot_sync(FULL, keep);
-                        const int slotC = nc + __popc(m & ((1u << lane) - 1u));
-                        if (keep && slotC < MV_MAX_CAND) {
-                            WarpShared::Cand &cd = S.cand[slotC];
-                            cd.c[0] = c.x; cd.c[1] = c.y; cd.c[2] = c.z; cd.h[0] = h.x; cd.h[1] = h.y; cd.h[2] = h.z; cd.kind = kind; cd.agent = agentIdx; cd.ax = rax; cd.az = raz;
-                        }
-                        nc += __popc(m);
-                    }
-                    if (nc > MV_MAX_CAND) { nc = MV_MAX_CAND; S.env.faults |= MV_FAULT_CAND_OVERFLOW; }
-                    __syncwarp();
-                    cv.nc = nc;
-                }
+                const V3 envLo = envelopeLo(k.pos), envHi = envelopeHi(k.pos);
+                cv.nc = gatherCandidates(S, statics, staticRot, L->n_static_pre, ns, no, A, i, envLo, envHi, lane);
                 if (i == 0) { MV_PROBE(2); if (P.prof && lane == 0) P.prof[size_t(env) * 16 + 12] = uint32_t(cv.nc); }  // candidate list of agent 0
                 kccPlayerStep(k, cv, ns + no + i, dt, P.k.max_slope_cos, lane);
     #ifdef MV_KCC_COUNTERS
                 if (i == 0 && P.prof && lane == 0) { P.prof[size_t(env) * 16 + 9] = k.dbg[0]; P.prof[size_t(env) * 16 + 10] = k.dbg[1]; P.prof[size_t(env) * 16 + 11] = k.dbg[2]; P.prof[size_t(env) * 16 + 13] = k.dbg[3]; }
     #endif
-                if (k.pos.x < envLo.x + 0.5f || k.pos.x > envHi.x - 0.5f || k.pos.y < envLo.y + 0.5f || k.pos.y > envHi.y - 0.5f || k.pos.z < envLo.z + 0.5f ||
-                    k.pos.z > envHi.z - 0.5f)
-                    S.env.faults |= MV_FAULT_ENVELOPE;
+                if (leftEnvelope(envLo, envHi, k.pos)) S.env.faults |= MV_FAULT_ENVELOPE;
                 __syncwarp();
                 if (lane == 0) {
                     a.pos[0] = k.pos.x; a.pos[1] = k.pos.y; a.pos[2] = k.pos.z;
@@ -1668,6 +1697,70 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
         asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
     }
 #undef MV_PROBE
+}
+
+// ---------------------------------------------------------------- mv_debug_kcc: chosen contact cases through the step's own collision code
+// One warp per case: the candidate gather, warpSweep / warpRecover / kccPlayerStep exactly as stepKernel runs them, on a caller-built
+// collider set.  Layouts are those of mv_debug_kcc (include/megaverse_b200.h); the host entry validates them.
+struct KccCaseParams {
+    const int32_t *hdr;      // [n][8] n_static_pre, n_static, n_obj, A, mode, agent
+    const MvBox *statics;    // [n][MV_MAX_OBJECTS]
+    const float *staticRot;  // [n][MV_MAX_OBJECTS][2]
+    const MvObject *objects; // [n][MV_MAX_OBJECTS] col_c, col_h, enabled
+    const float *agentPos;   // [n][MV_MAX_AGENTS][3] (the querying agent's own is its position for the envelope)
+    const float *query;      // [n][20]
+    int32_t *outI;           // [n][8]
+    float *outF;             // [n][16]
+};
+constexpr int kKccSweep = 0, kKccRecover = 1, kKccStep = 2;
+
+__global__ void __launch_bounds__(32) kccCaseKernel(KccCaseParams P) {
+    extern __shared__ __align__(128) unsigned char smemRaw[];
+    WarpShared &S = *reinterpret_cast<WarpShared *>(smemRaw);
+    __shared__ int16_t slotCollider[MV_MAX_CAND];
+    const int cs = blockIdx.x, lane = threadIdx.x;
+    const int32_t *hd = P.hdr + size_t(cs) * 8;
+    const int nsPre = hd[0], ns = hd[1], no = hd[2], A = hd[3], mode = hd[4], i = hd[5];
+    const float *q = P.query + size_t(cs) * 20;
+    for (int o = lane; o < no; o += 32) S.objects[o] = P.objects[size_t(cs) * MV_MAX_OBJECTS + o];
+    for (int a = lane; a < A; a += 32)
+        for (int c = 0; c < 3; ++c) S.agents[a].pos[c] = (mode == kKccStep && a == i) ? q[c] : P.agentPos[(size_t(cs) * MV_MAX_AGENTS + a) * 3 + c];
+    if (lane == 0) S.env.faults = 0;
+    __syncwarp();
+    const V3 self = v3(S.agents[i].pos[0], S.agents[i].pos[1], S.agents[i].pos[2]);
+    const V3 envLo = envelopeLo(self), envHi = envelopeHi(self);
+    ColliderView cv;
+    cv.S = &S; cv.L = nullptr; cv.ns = ns; cv.no = no; cv.A = A;
+    cv.nc = gatherCandidates(S, P.statics + size_t(cs) * MV_MAX_OBJECTS, P.staticRot + size_t(cs) * MV_MAX_OBJECTS * 2, nsPre, ns, no, A, i, envLo, envHi,
+                             lane, slotCollider);
+    int32_t oi[8] = {cv.nc, 0, 0, -1, -1, 0, 0, 0};
+    float of[16] = {};
+    if (mode == kKccSweep) {
+        const SweepReport r = warpSweep<true>(cv, ns + no + i, v3(q[0], q[1], q[2]), v3(q[3], q[4], q[5]), v3(q[6], q[7], q[8]), q[9], lane);
+        oi[2] = r.hit;
+        if (r.hit) { oi[3] = slotCollider[r.slot]; oi[4] = r.feature; }
+        of[0] = r.fraction; of[1] = r.normal.x; of[2] = r.normal.y; of[3] = r.normal.z;
+    } else if (mode == kKccRecover) {
+        V3 delta = v3(0, 0, 0);
+        int slot = -1;
+        oi[2] = warpRecover<true>(cv, ns + no + i, v3(q[0], q[1], q[2]), delta, lane, &slot);
+        if (oi[2]) { oi[3] = slotCollider[slot]; of[0] = delta.x; of[1] = delta.y; of[2] = delta.z; }
+    } else {
+        Kcc k;
+        k.pos = v3(q[0], q[1], q[2]); k.hvel = v3(q[3], q[4], q[5]);
+        k.vvel = q[6]; k.voff = q[7]; k.stepOff = q[8]; k.jumpSpeed = q[9];
+        k.jumpAxis = v3(q[10], q[11], q[12]);
+        k.wasOnGround = q[13] != 0.0f; k.wasJumping = q[14] != 0.0f;
+        kccPlayerStep(k, cv, ns + no + i, q[15], q[16], lane);
+        if (leftEnvelope(envLo, envHi, k.pos)) S.env.faults |= MV_FAULT_ENVELOPE;
+        oi[2] = k.wasOnGround; oi[5] = k.wasJumping;
+        of[0] = k.pos.x; of[1] = k.pos.y; of[2] = k.pos.z; of[3] = k.hvel.x; of[4] = k.hvel.y; of[5] = k.hvel.z;
+        of[6] = k.vvel; of[7] = k.voff; of[8] = k.stepOff; of[9] = k.jumpSpeed;
+    }
+    __syncwarp();
+    oi[1] = S.env.faults;
+    if (lane < 8) P.outI[size_t(cs) * 8 + lane] = oi[lane];
+    if (lane < 16) P.outF[size_t(cs) * 16 + lane] = of[lane];
 }
 
 }  // namespace mvk

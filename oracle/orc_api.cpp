@@ -439,6 +439,71 @@ void orc_scenegraph_case(const float *ps, float angle, const float *pt, const fl
     const Mat4 abs = mul(root, local);
     std::memcpy(out48 + 32, &abs.c[0][0], 64);
 }
+// One mv_debug_kcc case list (same layouts, include/megaverse_b200.h) through the oracle's own queries over the FULL collider list: no
+// envelope, no candidate cap, so out_i8[0] is the number of enabled colliders other than the agent and out_i8[1] is 0.  Arguments are
+// trusted (the tests build them).
+constexpr int kKccMaxObjects = 128, kKccMaxAgents = 8;  // the layouts' row counts: the engine's MV_MAX_OBJECTS and MV_MAX_AGENTS
+void orc_kcc_case(const int32_t *hdr8, const float *boxes10, const float *agents3, const float *query20, int n, int32_t *out_i8, float *out_f16) {
+    for (int cs = 0; cs < n; ++cs) {
+        const int32_t *hd = hdr8 + size_t(cs) * 8;
+        const int nsPre = hd[0], ns = hd[1], no = hd[2], A = hd[3], mode = hd[4], agent = hd[5];
+        const float *q = query20 + size_t(cs) * 20;
+        std::vector<Collider> cols;
+        auto box = [&](int row, bool isStatic) {
+            const float *b = boxes10 + (size_t(cs) * 2 * kKccMaxObjects + size_t(row)) * 10;
+            Collider c;
+            c.c = {b[0], b[1], b[2]}; c.h = {b[3], b[4], b[5]}; c.enabled = b[6] != 0.0f;
+            if (isStatic && b[7] != 0.0f) { c.rotated = true; c.ax = b[8]; c.az = b[9]; }
+            cols.push_back(c);
+        };
+        for (int j = 0; j < nsPre; ++j) box(j, true);
+        for (int j = 0; j < no; ++j) box(kKccMaxObjects + j, false);
+        for (int j = nsPre; j < ns; ++j) box(j, true);
+        for (int a = 0; a < A; ++a) {
+            const float *p = agents3 + (size_t(cs) * kKccMaxAgents + size_t(a)) * 3;
+            Collider c;
+            c.kind = 1; c.c = (mode == 2 && a == agent) ? Vec3{q[0], q[1], q[2]} : Vec3{p[0], p[1], p[2]};
+            cols.push_back(c);
+        }
+        const int self = ns + no + agent;
+        int32_t *oi = out_i8 + size_t(cs) * 8;
+        float *of = out_f16 + size_t(cs) * 16;
+        for (int j = 0; j < 8; ++j) oi[j] = 0;
+        for (int j = 0; j < 16; ++j) of[j] = 0.0f;
+        for (int j = 0; j < int(cols.size()); ++j) oi[0] += j != self && cols[size_t(j)].enabled;
+        oi[3] = oi[4] = -1;
+        if (mode == 0) {
+            const SweepHit r = convexSweep(cols, self, {q[0], q[1], q[2]}, {q[3], q[4], q[5]}, {q[6], q[7], q[8]}, q[9]);
+            oi[2] = r.hit;
+            if (r.hit) { oi[3] = r.index; oi[4] = r.feature; }
+            of[0] = r.fraction; of[1] = r.normal.x; of[2] = r.normal.y; of[3] = r.normal.z;
+        } else if (mode == 1) {
+            KCC k;
+            k.pos = {q[0], q[1], q[2]};
+            int idx = -1;
+            oi[2] = k.recoverFromPenetration(cols, self, &idx);
+            if (oi[2]) {  // the push-out itself, as recoverFromPenetration forms it before adding it to the position
+                Vec3 nrm;
+                const float dist = capsuleDistance(cols[size_t(idx)], {q[0], q[1], q[2]}, nrm);
+                const Vec3 delta = nrm * (-dist);
+                oi[3] = idx; of[0] = delta.x; of[1] = delta.y; of[2] = delta.z;
+            }
+        } else {
+            KCC k;
+            k.pos = {q[0], q[1], q[2]}; k.horizontalVelocity = {q[3], q[4], q[5]};
+            k.verticalVelocity = q[6]; k.verticalOffset = q[7]; k.currentStepOffset = q[8]; k.jumpSpeed = q[9];
+            k.jumpAxis = {q[10], q[11], q[12]};
+            k.wasOnGround = q[13] != 0.0f; k.wasJumping = q[14] != 0.0f;
+            k.maxSlopeCosine = q[16];
+            k.playerStep(cols, self, q[15]);
+            oi[2] = k.wasOnGround; oi[5] = k.wasJumping;
+            of[0] = k.pos.x; of[1] = k.pos.y; of[2] = k.pos.z;
+            of[3] = k.horizontalVelocity.x; of[4] = k.horizontalVelocity.y; of[5] = k.horizontalVelocity.z;
+            of[6] = k.verticalVelocity; of[7] = k.verticalOffset; of[8] = k.currentStepOffset; of[9] = k.jumpSpeed;
+        }
+    }
+}
+
 // colour tables of the restatement, same layout as ref_color_tables (oracle/ref_shim/ref_shim.cpp)
 int orc_color_tables(unsigned *out, int cap) {
     std::vector<unsigned> o{unsigned(numColors), unsigned(numAgentColors), unsigned(numObjectColors), unsigned(numLayoutColors)};

@@ -49,6 +49,7 @@ struct SweepHit {
     float fraction = 1.0f;
     Vec3 normal;
     int index = -1;
+    int feature = -1;  // of the winner: the box feature numbered as the device numbers it (0..2 faces, 3..14 edges, 15..22 corners), 0 for a capsule
 };
 
 // signed distance helper: point o (relative to box centre) vs box half H.  Returns distance (>=0 outside,
@@ -73,16 +74,17 @@ inline float pointBoxDistance(Vec3 o, Vec3 H, Vec3 &n) {
 }
 
 // Ray o + t d, t in [0,1], against the rounded box {p : dist(p, box(H)) <= rho}.  Returns true and the first
-// entry (t, outward normal).  Start inside => t = 0 iff moving into the surface.
-inline bool rayRoundedBox(Vec3 o, Vec3 d, Vec3 H, float rho, float &tOut, Vec3 &nOut) {
+// entry (t, outward normal, and the feature that gave it, 0 for a start inside).  Start inside => t = 0 iff moving into the surface.
+inline bool rayRoundedBox(Vec3 o, Vec3 d, Vec3 H, float rho, float &tOut, Vec3 &nOut, int *fOut = nullptr) {
     Vec3 n0;
     const float d0 = pointBoxDistance(o, H, n0);
     if (d0 - rho <= 0.0f) {
-        if (dot(d, n0) < -kSimdEpsilon) { tOut = 0.0f; nOut = n0; return true; }
+        if (dot(d, n0) < -kSimdEpsilon) { tOut = 0.0f; nOut = n0; if (fOut) *fOut = 0; return true; }
         return false;
     }
     float best = 2.0f;
     Vec3 bestN;
+    int bestF = -1;
     // 6 faces
     for (int i = 0; i < 3; ++i) {
         if (d[i] == 0.0f) continue;
@@ -91,7 +93,7 @@ inline bool rayRoundedBox(Vec3 o, Vec3 d, Vec3 H, float rho, float &tOut, Vec3 &
         if (t < 0.0f || t > 1.0f || t >= best) continue;
         const int j = (i + 1) % 3, k = (i + 2) % 3;
         const float qj = o[j] + t * d[j], qk = o[k] + t * d[k];
-        if (fabsf(qj) <= H[j] && fabsf(qk) <= H[k]) { best = t; bestN = {0, 0, 0}; bestN[i] = s; }
+        if (fabsf(qj) <= H[j] && fabsf(qk) <= H[k]) { best = t; bestN = {0, 0, 0}; bestN[i] = s; bestF = i; }
     }
     // 12 edges: axis k free, signs on i and j
     for (int k = 0; k < 3; ++k) {
@@ -113,6 +115,7 @@ inline bool rayRoundedBox(Vec3 o, Vec3 d, Vec3 H, float rho, float &tOut, Vec3 &
                     bestN = {0, 0, 0};
                     bestN[i] = qi / rho;
                     bestN[j] = qj / rho;
+                    bestF = 3 + 4 * k + (si > 0 ? 2 : 0) + (sj > 0 ? 1 : 0);
                 }
             }
     }
@@ -131,12 +134,16 @@ inline bool rayRoundedBox(Vec3 o, Vec3 d, Vec3 H, float rho, float &tOut, Vec3 &
                         const float t = (-b - sqrtf(disc)) / a;
                         if (t < 0.0f || t > 1.0f || t >= best) continue;
                         const Vec3 q = oc + d * t;
-                        if (sx * q.x >= 0.0f && sy * q.y >= 0.0f && sz * q.z >= 0.0f) { best = t; bestN = q * (1.0f / rho); }
+                        if (sx * q.x >= 0.0f && sy * q.y >= 0.0f && sz * q.z >= 0.0f) {
+                            best = t; bestN = q * (1.0f / rho);
+                            bestF = 15 + (sx > 0 ? 4 : 0) + (sy > 0 ? 2 : 0) + (sz > 0 ? 1 : 0);
+                        }
                     }
     }
     if (best > 1.0f) return false;
     tOut = best;
     nOut = bestN;
+    if (fOut) *fOut = bestF;
     return true;
 }
 
@@ -207,12 +214,13 @@ inline bool sweepBroadphaseMiss(const Collider &c, Vec3 from, Vec3 to) {
     return miss;
 }
 // narrow phase of one sweep: the agent capsule from `from` along d against one collider (see the header comment)
-inline bool sweepNarrow(const Collider &c, Vec3 from, Vec3 d, float &t, Vec3 &n) {
+inline bool sweepNarrow(const Collider &c, Vec3 from, Vec3 d, float &t, Vec3 &n, int *f = nullptr) {
     if (c.kind == 0) {
-        const bool hit = rayRoundedBox(c.toLocal(from - c.c), c.toLocal(d), Vec3{c.h.x, c.h.y + kCapsuleHalfHeight, c.h.z}, kCapsuleRadius - kAllowedCcdPenetration, t, n);
+        const bool hit = rayRoundedBox(c.toLocal(from - c.c), c.toLocal(d), Vec3{c.h.x, c.h.y + kCapsuleHalfHeight, c.h.z}, kCapsuleRadius - kAllowedCcdPenetration, t, n, f);
         if (hit) n = c.toWorld(n);
         return hit;
     }
+    if (f) *f = 0;
     return rayCapsule(from - c.c, d, 2.0f * kCapsuleHalfHeight, 2.0f * kCapsuleRadius - kAllowedCcdPenetration, t, n);
 }
 
@@ -226,13 +234,15 @@ inline SweepHit convexSweep(const std::vector<Collider> &cols, int self, Vec3 fr
         if (sweepBroadphaseMiss(c, from, to)) continue;
         float t;
         Vec3 n;
-        if (!sweepNarrow(c, from, d, t, n)) continue;
+        int f;
+        if (!sweepNarrow(c, from, d, t, n, &f)) continue;
         if (!(t < res.fraction)) continue;             // btCollisionWorld: castResult.m_fraction < m_closestHitFraction
         if (dot(filterDir, n) < minSlopeDot) continue;  // slope filter
         res.hit = true;
         res.fraction = t;
         res.normal = n;
         res.index = i;
+        res.feature = f;
     }
     return res;
 }
@@ -304,7 +314,7 @@ struct KCC {
         verticalVelocity = 0;
     }
 
-    bool recoverFromPenetration(const std::vector<Collider> &cols, int self) {  // :156-221
+    bool recoverFromPenetration(const std::vector<Collider> &cols, int self, int *index = nullptr) {  // :156-221; index: the collider that pushed
         bool penetration = false;
         currentPosition = pos;
         for (int i = 0; i < int(cols.size()) && !penetration; ++i) {
@@ -314,6 +324,7 @@ struct KCC {
             if (dist < -maxPenetrationDepth) {
                 currentPosition += n * (-dist);
                 penetration = true;
+                if (index) *index = i;
             }
         }
         pos = currentPosition;

@@ -36,6 +36,8 @@ def lib():
         L.orc_get_mesh.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.orc_get_reward_shaping.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p, C.POINTER(C.c_float)]
         L.orc_set_reward_shaping.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p, C.c_float]
+        L.orc_kcc_case.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p]
+        L.orc_kcc_case.restype = None
         _LIB = L
     return _LIB
 
@@ -128,6 +130,21 @@ def render_instances(view16, inst18, w, h, want_depth=False):
     depth = np.zeros((h, w), dtype=np.float32)
     lib().orc_render_instances(view16.ctypes.data, inst18.ctypes.data, inst18.shape[0], w, h, rgba.ctypes.data, depth.ctypes.data if want_depth else None)
     return (rgba, depth) if want_depth else rgba
+
+
+def kcc_cases(hdr, boxes, agents, query):
+    """the oracle's convexSweep / recoverFromPenetration / KCC::playerStep over mv_debug_kcc's case layouts, every collider a candidate:
+    (out_i int32[n, 8], out_f float32[n, 16]) as capi.kcc_cases returns them"""
+    hdr = np.ascontiguousarray(hdr, dtype=np.int32)
+    boxes = np.ascontiguousarray(boxes, dtype=np.float32)
+    agents = np.ascontiguousarray(agents, dtype=np.float32)
+    query = np.ascontiguousarray(query, dtype=np.float32)
+    n = hdr.shape[0]
+    assert boxes.shape == (n, 256, 10) and agents.shape == (n, 8, 3) and query.shape == (n, 20)
+    out_i = np.zeros((n, 8), dtype=np.int32)
+    out_f = np.zeros((n, 16), dtype=np.float32)
+    lib().orc_kcc_case(hdr.ctypes.data, boxes.ctypes.data, agents.ctypes.data, query.ctypes.data, n, out_i.ctypes.data, out_f.ctypes.data)
+    return out_i, out_f
 
 
 def mesh(type_):
