@@ -373,10 +373,12 @@ int mv_stream(mv_handle h, void **stream);
  * generates, once, L levels for every distinct scenario name of the engine: level j of a scenario is the first level (episode 0) of a
  * fresh generator of that scenario seeded s + j with the engine's params -- what mv_debug_generate_level(scenario, A, s + j, 0, params)
  * dumps.  Generation runs on the worker pool; "skip_unfit_levels" and generation errors behave as for the streams.  The levels stay in
- * HBM as a bank of immutable rows that the envs share, and every env plays levels of its own scenario's rows only.  At each start of an
+ * HBM as a bank of rows that the envs share (rewritten only by mv_replace_levels, below), and every env plays levels of its own
+ * scenario's rows only.  At each start of an
  * episode (a natural end, a requested end, mv_reset, mv_reset_envs) the step kernel chooses the env's next level j:
  *   1. the env's entry of the next-level array when it is in [0, L): used once, then set back to -1;
- *   2. else mv_level_set_pick(pick seed of the env, index of the new episode, L), a hash: uniform over the set, no state.
+ *   2. else mv_level_set_pick(pick seed of the env, index of the new episode, L), a hash: uniform over the set, no state
+ *      (probed forward past rows being replaced, see mv_replace_levels).
  * mv_seed, mv_seed_env and the seeds of mv_reset_envs set pick seeds (mv_seed: the value it would seed the env's generator with); they
  * never regenerate the bank, and the episode counter keeps counting.  Engines with the same options, seeds and actions play the same
  * level sequences and produce the same bytes.  A second mv_reset keeps the bank and starts every env on its next pick.
@@ -405,6 +407,38 @@ int mv_level_ids_device(mv_handle h, int32_t **d_ids);
 int mv_next_levels_device(mv_handle h, int32_t **d_next);
 int mv_set_next_levels(mv_handle h, const int32_t *envs, const int32_t *levels, int n);
 uint32_t mv_level_set_pick(uint32_t pick_seed, int32_t episode, int32_t count);
+
+/* Replaceable rows: swap chosen rows of the bank for new levels while the envs run (Prioritised Level Replay's buffer, open-ended
+ * procedural training).  Bank row b * L + j is level j (what mv_level_ids reports) of the engine's b-th distinct scenario name in order of
+ * first appearance; for a single-scenario engine, row = j.
+ * mv_replace_levels: row rows[i] is to hold episode 0 of a fresh generator of its block's scenario seeded seeds[i] -- what
+ *   mv_debug_generate_level(scenario, A, seeds[i], 0, params) dumps.  The level is generated on the worker pool beside the device.
+ *   Retiring: from the kernel of the next call that enqueues the step kernel (mv_step, mv_step_envs, mv_step_begin, mv_step_device*,
+ *   mv_reset, mv_reset_envs) on, the row is retiring:
+ *     - the hash pick never lands on it: j = mv_level_set_pick(...) probes forward (j + 1, j + 2, ... mod L) to the first pickable row of
+ *       the env's block;
+ *     - a next-level entry naming it is left in place and honoured at the first end at which the row is pickable again (deferred, not
+ *       dropped, so a replay sampler may point envs at the new level at once);
+ *     - envs already on it keep playing it, bit for bit, until their episode ends.
+ *   Rewrite: at the start of the first later such call at which (a) the newest call the host has retired when the call starts is at or
+ *   after the request's call (for host-facing calls the previous call; in a run of mv_step_device* calls the one three back, whose results
+ *   the previous call published; every call after mv_sync) and (b) that retired call's mv_level_ids show no env on the row.  The rewrite is
+ *   stream-ordered before that call's kernel, and the row is pickable from that kernel on.  The host waits for the worker's level if it
+ *   is not ready, so the rewrite call depends only on the sequence of calls and on the device's results, never on worker timing or thread
+ *   count.  An inactive env holds its row; an end request or mv_reset_envs releases it.
+ *   Nothing changes for an engine that never calls it: with every row pickable the picks are the hash's, and no copy is added.
+ *   Refusals, with nothing changed: MV_ERR_STATE without "level_set", before the first mv_reset or with an outstanding mv_step_begin;
+ *   MV_ERR_ARG for a row out of range, a row listed twice, a row already retiring, or a request that would leave a block with no
+ *   pickable row.  "skip_unfit_levels" and generation errors behave as for the bank (an error is reported by the rewrite call).  A second
+ *   mv_reset keeps the bank, replaced rows included.
+ * mv_level_rows: host arrays [L * blocks], valid like mv_dones: the seed of the level each row holds now (level_set_seed + j before any
+ *   replacement) and whether the row is retiring (1 from mv_replace_levels to the rewrite).  Right after a call that reports env e done,
+ *   the seed of the row e's finished episode was played on is still that episode's: the row cannot be rewritten before a later retired
+ *   call shows the env gone.  MV_ERR_STATE before the first mv_reset.
+ * State store: a saved row records the seed of the bank row the env was on; mv_states_load refuses it (MV_ERR_ARG, naming the row) when
+ *   that bank row now holds another seed or is retiring -- the loaded env would otherwise replay a level other than the one it was saved on. */
+int mv_replace_levels(mv_handle h, const int32_t *rows, const int32_t *seeds, int n);
+int mv_level_rows(mv_handle h, const int32_t **seeds, const uint8_t **retiring);
 
 /* Env state store: save envs mid-episode and rewind or clone them later, on the device.  A store holds `rows` env states; a row is the
  * complete state of one env -- every per-env device array (env, agents, objects, object grid, instance list, views, both level slots,

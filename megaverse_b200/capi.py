@@ -79,6 +79,8 @@ def lib():
         L.mv_states_destroy.argtypes = [vp, ci]
         L.mv_state_row_bytes.argtypes = [vp, C.POINTER(C.c_int64)]
         L.mv_set_next_levels.argtypes = [vp, vp, vp, ci]
+        L.mv_replace_levels.argtypes = [vp, vp, vp, ci]
+        L.mv_level_rows.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
         L.mv_level_set_pick.argtypes = [C.c_uint32, C.c_int32, C.c_int32]
         L.mv_level_set_pick.restype = C.c_uint32
         for name in ("mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device"):
@@ -104,7 +106,7 @@ EXPORTS = [
     "mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device",
     "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
     "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms", "mv_debug_cast_rays",
-    "mv_debug_kcc",
+    "mv_debug_kcc", "mv_replace_levels", "mv_level_rows",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -141,6 +143,9 @@ class Engine:
                 raise MegaverseError(MV_ERR_ARG, "%d scenario names for %d envs" % (len(names), num_envs))
             arr = (C.c_char_p * max(1, num_envs))(*[n.encode() for n in names])
             rc = L.mv_create_mixed(arr, w, h, num_envs, num_agents, num_threads, device, keys, vals, len(params), C.byref(self._h))
+        # level-set blocks: the distinct names in any spelling (the engine lowercases them)
+        self.banks = 1 if isinstance(scenario, str) else len({n.lower() for n in scenario})
+        self.level_set = 0
         if rc != MV_OK:
             raise MegaverseError(rc, (L.mv_last_error(None) or b"").decode())
         self.E, self.A, self.N, self.w, self.h = num_envs, num_agents, num_envs * num_agents, w, h
@@ -161,6 +166,8 @@ class Engine:
 
     def set_option(self, key, value):
         self._ck(lib().mv_set_option(self._h, key.encode(), int(value)))
+        if key == "level_set":
+            self.level_set = int(value)
 
     def seed(self, s):
         self._ck(lib().mv_seed(self._h, int(s)))
@@ -346,6 +353,22 @@ class Engine:
     def level_ids(self):
         """int32[E] (option level_set): the level of the set each env is on after the last call; for an env that just ended, the new episode's"""
         return self._host("mv_level_ids", (self.E,), np.int32)
+
+    def replace_levels(self, rows, seeds):
+        """(option level_set) bank row rows[i] (block * L + level) is to hold the first level of seed seeds[i] (mv_replace_levels): it
+        retires at the next call and is rewritten once a retired call shows no env on it"""
+        r, sd = np.ascontiguousarray(rows, dtype=np.int32), np.ascontiguousarray(seeds, dtype=np.int32)
+        assert r.size == sd.size
+        self._ck(lib().mv_replace_levels(self._h, r.ctypes.data if r.size else None, sd.ctypes.data if sd.size else None, r.size))
+
+    def level_rows(self):
+        """(option level_set) (seeds int32[B], retiring bool[B]) of the bank's rows, copies (mv_level_rows)"""
+        s, r = C.c_void_p(), C.c_void_p()
+        self._ck(lib().mv_level_rows(self._h, C.byref(s), C.byref(r)))
+        B = self.level_set * self.banks
+        seeds = np.ctypeslib.as_array(C.cast(s, C.POINTER(C.c_int32)), (B,)).copy()
+        retiring = np.ctypeslib.as_array(C.cast(r, C.POINTER(C.c_uint8)), (B,)).astype(bool)
+        return seeds, retiring
 
     def set_next_levels(self, envs, levels):
         """(option level_set) env envs[i] plays level levels[i] of the set in its next episode, once (mv_set_next_levels).  Followed by

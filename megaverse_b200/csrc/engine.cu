@@ -21,6 +21,7 @@
 #include <cstring>
 #include <deque>
 #include <functional>
+#include <list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -150,6 +151,7 @@ struct StateStore {
         bool saved = false;
         std::optional<mv::LevelGenerator> gen;  // the env's level stream; empty with a level set (the bank is the engine's, the pick is in MvEnvState)
         std::string scenario;                   // the saved env's scenario name: only an env of the same name may load the row
+        int bankRow = -1, bankSeed = 0;         // level set: the bank row the env was on and the seed of the level it held then
         int slot = 0, episode = 0;
         // the host mirrors of every level slot that the debug dumps and the uploads read, one entry per slot (option "level_slots")
         std::vector<int> words;
@@ -282,6 +284,27 @@ struct mv_engine {
     DevBuf<int32_t> d_bankBase, d_levelIds, d_nextLevels;  // [E] each, see StepParams
     PinBuf<int32_t> h_levelIds;        // [E] level ids of the last retired call, beside h_dones
     PinBuf<int32_t> h_nextLevels;      // [E] staging of mv_set_next_levels
+    // replaceable rows (mv_replace_levels, the header has the rule).  A request makes its row retiring from the next kernel-enqueuing call
+    // on; the level is generated on replacePool into the request's own LevelOut meanwhile and copied into the row's mirrors and uploaded
+    // only at the rewrite, at the start of the first call whose published level ids (those of call publishedCall) are at or after the
+    // request's call and show no env on the row.  No device refcount is needed: from the request's kernel on no flip lands on the row, so
+    // once a retired call shows it empty, no kernel still in flight can put an env back on it
+    struct Replacement {
+        int row = 0, seed = 0;
+        int64_t call = -1;  // the call from whose kernel on the row is retiring (-1: requested since the last call)
+        bool ready = false;
+        std::string error;  // generation failed: reported by the rewrite call
+        mv::LevelOut out;
+    };
+    std::vector<int32_t> rowSeed;      // [levelRows()] the seed of the level each row holds
+    std::vector<uint8_t> rowRetiring;  // [levelRows()] a replacement of the row is pending
+    std::vector<uint8_t> rowPickable;  // [levelRows()] what d_rowPickable holds (0 from a request's call to its rewrite)
+    DevBuf<uint8_t> d_rowPickable;
+    std::list<std::unique_ptr<Replacement>> replacements;  // pending, in request order
+    std::unique_ptr<WorkerPool> replacePool;  // its own pool: the per-call flushUploads never waits for a replacement that is not due
+    std::condition_variable replaceDone;      // with genMutex: a Replacement became ready
+    int64_t stepCalls = 0;                    // kernel-enqueuing calls so far (mv_step*, mv_reset*)
+    int64_t publishedCall = -1;               // the call whose level ids h_levelIds holds
     size_t levelRows() const { return levelSet ? size_t(levelSet) * size_t(numBanks) : size_t(E) * size_t(levelSlots); }
     // the row of the level arrays and their host mirrors that holds what MvEnvState::slot names for env e
     size_t rowOfSlot(int e, int slot) const { return levelSet ? size_t(slot) : size_t(e) * size_t(levelSlots) + size_t(slot); }
@@ -368,7 +391,7 @@ struct mv_engine {
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
     // mv_step_device pipeline: results of step k are consumed by the host while steps k+1, k+2 already run
-    struct Pending { bool valid = false; uint64_t step = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
+    struct Pending { bool valid = false; uint64_t step = 0; int64_t call = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
     std::vector<int64_t> lastAsyncDone;  // [E] asynchronous step index of the env's previous episode end
     bool asyncContractBroken = false;
     Pending ring[3];
@@ -504,43 +527,52 @@ struct mv_engine {
     }
     // worker thread: one level of env e's stream into slot s
     void generateLevel(int e, int s, int serial) { generateInto(gens[size_t(e)], envScenario[size_t(e)], e * levelSlots + s, serial); }
-    // worker thread: level j of the level set of the scenario env `first` runs, into bank row `row` -- the first level of that env's
-    // generator (scenario, agents, params) as constructed and seeded levelSetSeed + j, which is what mv_debug_generate_level(..., 0) dumps
-    void generateBankLevel(int first, int row, int j) {
-        mv::LevelGenerator gen = gens[size_t(first)];
-        gen.restart((unsigned long)(levelSetSeed + j));
-        generateInto(gen, envScenario[size_t(first)], row, 0);
+    // worker thread: a bank level of MV_SCENARIO_* sc -- the first level of `gen` (a copy of the generator, as constructed, of an env of
+    // that scenario) restarted with `seed`, which is what mv_debug_generate_level(..., seed, 0) dumps.  Into bank row `row`, or, for a
+    // replacement, into its own LevelOut until the rewrite (the row's mirrors still hold the level live envs play)
+    void generateBankLevel(mv::LevelGenerator gen, int sc, int row, int seed, Replacement *side = nullptr) {
+        gen.restart((unsigned long)seed);
+        if (!side) { generateInto(gen, sc, row, 0); return; }
+        std::string error;
+        generateOut(gen, sc, 0, side->out, &error);
+        std::lock_guard<std::mutex> lk(genMutex);
+        side->error = error;
+        side->ready = true;
+        replaceDone.notify_all();
+    }
+    // worker thread: the next level of `gen` (of MV_SCENARIO_* sc) into `out`; false on a generation error, which goes to *error when
+    // given, else to genErrors
+    bool generateOut(mv::LevelGenerator &gen, int sc, int serial, mv::LevelOut &out, std::string *error = nullptr) {
+        // the env's own scenario's capacity, not the engine's pitch: a level is accepted exactly as in a single-scenario engine
+        const int cap = mv::gridCapacity(sc);
+        try {
+            if (skipUnfitLevels) {
+                const int skipped = gen.generateFitting(out, serial, cap);
+                if (skipped) levelsSkipped.fetch_add(skipped);
+            } else {
+                gen.generate(out, serial, cap);
+            }
+        } catch (const std::exception &ex) {
+            if (error) { *error = ex.what(); return false; }
+            std::lock_guard<std::mutex> lk(genMutex);
+            genErrors.push_back(ex.what());
+            return false;
+        }
+        int curO = maxObjSeen.load();
+        while (out.level.n_obj > curO && !maxObjSeen.compare_exchange_weak(curO, out.level.n_obj)) {}
+        return true;
     }
     // worker thread: the next level of `gen` (of MV_SCENARIO_* sc) into row `id` of the level arrays
     void generateInto(mv::LevelGenerator &gen, int sc, int id, int serial) {
-        {
-            mv::LevelOut out;
-            // the env's own scenario's capacity, not the engine's pitch: a level is accepted exactly as in a single-scenario engine
-            const int cap = mv::gridCapacity(sc);
-            try {
-                if (skipUnfitLevels) {
-                    const int skipped = gen.generateFitting(out, serial, cap);
-                    if (skipped) levelsSkipped.fetch_add(skipped);
-                } else {
-                    gen.generate(out, serial, cap);
-                }
-            } catch (const std::exception &ex) {
-                std::lock_guard<std::mutex> lk(genMutex);
-                genErrors.push_back(ex.what());
-                return;
-            }
-            {
-                int curO = maxObjSeen.load();
-                while (out.level.n_obj > curO && !maxObjSeen.compare_exchange_weak(curO, out.level.n_obj)) {}
-            }
-            if (int(out.statics.size()) > staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
-                std::lock_guard<std::mutex> lk(genMutex);
-                wantStaticCap = std::max(wantStaticCap, int(out.statics.size()));
-                oversize.emplace_back(id, std::move(out));
-                return;
-            }
-            stageLevel(id, out);
+        mv::LevelOut out;
+        if (!generateOut(gen, sc, serial, out)) return;
+        if (int(out.statics.size()) > staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
+            std::lock_guard<std::mutex> lk(genMutex);
+            wantStaticCap = std::max(wantStaticCap, int(out.statics.size()));
+            oversize.emplace_back(id, std::move(out));
+            return;
         }
+        stageLevel(id, out);
     }
     // worker thread (or flushUploads for parked levels): copy a generated level into the pinned staging mirrors and queue its upload
     void stageLevel(int id, const mv::LevelOut &out) {
@@ -586,15 +618,17 @@ struct mv_engine {
         MV_CUDA(cudaStreamSynchronize(stream));
         DevBuf<MvBox> nStat; DevBuf<float> nRot; DevBuf<MvInstance> nInst; PinBuf<MvBox> hStat; PinBuf<float> hRot;
         const size_t rows = levelRows();
-        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside (with a level set the
-        // only growth is the first reset's, before any store exists)
+        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside (with a level set a
+        // store holds no level, only the instance rows; a replacement can grow the arrays after stores exist)
         struct Repitch { DevBuf<uint8_t> *buf; DevBuf<uint8_t> next; size_t rows, oldPitch, newPitch; };
         std::vector<Repitch> storeGrow;
         for (auto &st : stores) {
-            if (!st || levelSet) continue;
+            if (!st) continue;
             const size_t r = size_t(st->rows);
-            storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * levelSlots, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
-            storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * levelSlots, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
+            if (!levelSet) {
+                storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * levelSlots, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
+                storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * levelSlots, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
+            }
             storeGrow.push_back({&st->slabs[kSlabInst], {}, r, sizeof(MvInstance) * instCap, sizeof(MvInstance) * newInstCap});
         }
         bool storesOk = true;
@@ -690,6 +724,7 @@ struct mv_engine {
         sp.slots = levelSlots;
         sp.levelSet = levelSet; sp.bankBase = d_bankBase.p; sp.nextLevels = d_nextLevels.p; sp.levelIds = d_levelIds.p;
         sp.hostLevelIds = (mirror && levelSet) ? mirror->levelIds.p : nullptr;
+        sp.rowPickable = d_rowPickable.p;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         float *st = wantState ? d_state.p : nullptr, *termSt = wantFinal ? st : nullptr;
@@ -1056,7 +1091,10 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
-        if (levelSet) MV_CUDA(cudaMemcpyAsync(h_levelIds.p, d_levelIds.p, sizeof(int32_t) * E, cudaMemcpyDeviceToHost, stream));
+        if (levelSet) {
+            MV_CUDA(cudaMemcpyAsync(h_levelIds.p, d_levelIds.p, sizeof(int32_t) * E, cudaMemcpyDeviceToHost, stream));
+            publishedCall = stepCalls - 1;  // every call so far is behind this copy
+        }
         if (copyObs && !rasterToHost && sliceCount <= 1) {
             const int rc = downloadViews(0, N, stream);
             if (rc) return rc;
@@ -1087,7 +1125,7 @@ struct mv_engine {
         std::memcpy(h_dones.p, p.dones.p, E);
         std::memcpy(h_doneReasons.p, p.reasons.p, E);
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
-        if (levelSet) std::memcpy(h_levelIds.p, p.levelIds.p, sizeof(int32_t) * E);
+        if (levelSet) { std::memcpy(h_levelIds.p, p.levelIds.p, sizeof(int32_t) * E); publishedCall = p.call; }
         p.valid = false;
         // with two level slots the pre-staged next level of an env is delivered three calls after its episode ended: an env that finishes
         // again sooner flipped to a stale level on the device (MV_FAULT_LEVEL_NOT_READY is latched there as well) -- refuse to go on.  Counted
@@ -1122,10 +1160,12 @@ struct mv_engine {
         if (hostStepPending) { const int rcp = stepEnd(); if (rcp) return rcp; }
         if (asyncContractBroken) { setError("mv_step_device: an episode lasted fewer than 3 steps -- outside the asynchronous call's contract; use mv_step"); return MV_ERR_STATE; }
         Pending &slotP = ring[asyncSteps % 3];
+        int rc = bankCall();
+        if (rc) return rc;
         // levels generated since the previous call go up first (done at step k-3 -> retired at call k-1 -> uploaded ahead
         // of kernel k; that env cannot flip again before step k+1), then step k-2 is retired and its regeneration jobs
         // run on the worker pool while this call's kernels are enqueued
-        int rc = flushUploads();
+        rc = flushUploads();
         if (rc) return rc;
         rc = retire(ring[(asyncSteps + 1) % 3]);
         if (rc) return rc;
@@ -1139,6 +1179,7 @@ struct mv_engine {
         MV_CUDA(cudaEventRecord(slotP.ev, stream));
         slotP.valid = true;
         slotP.step = asyncSteps;
+        slotP.call = stepCalls - 1;
         ++asyncSteps;
         return MV_OK;
     }
@@ -1146,7 +1187,9 @@ struct mv_engine {
     int stepCommon(const int32_t *dActions, bool copyObs, bool split = false, const uint8_t *dActive = nullptr) {
         if (!didReset) { setError("mv_step before mv_reset"); return MV_ERR_STATE; }
         if (hostStepPending) { setError("mv_step_begin is outstanding: call mv_step_end first"); return MV_ERR_STATE; }
-        int rc = drain();
+        int rc = bankCall();
+        if (rc) return rc;
+        rc = drain();
         if (rc) return rc;
         rc = flushUploads();
         if (rc) return rc;
@@ -1283,7 +1326,11 @@ struct mv_engine {
             r.saved = true;
             r.scenario = envScenarioName[size_t(e)];
             r.slot = hostSlot[size_t(e)]; r.episode = hostEpisode[size_t(e)];
-            if (levelSet) continue;  // no generator, no mirrors: the pick seed and the live row travel in MvEnvState
+            if (levelSet) {  // no generator, no mirrors: the pick seed and the live row travel in MvEnvState
+                r.bankRow = int(liveRow(e));
+                r.bankSeed = rowSeed[size_t(r.bankRow)];
+                continue;
+            }
             r.gen = gens[size_t(e)];
             const size_t D = size_t(levelSlots);
             r.words.resize(D); r.level.resize(D); r.statics.resize(D); r.staticRot.resize(D); r.deco.resize(D); r.solid.resize(D);
@@ -1338,7 +1385,9 @@ struct mv_engine {
     // a state load.  A synchronisation point: on return the restarted envs' levels after next are generated and uploaded, so the
     // asynchronous call's three-step rule holds from the next mv_step_device on.
     int resetEnvs(const int32_t *envs, const int32_t *seeds, int n) {
-        int rc = quiesce();
+        int rc = bankCall();
+        if (rc) return rc;
+        rc = quiesce();
         if (rc) return rc;
         if (seeds) {  // the staged slots take the first levels of the new stream, in order, as in a fresh engine; the workers are idle after quiesce
             for (int i = 0; i < n; ++i) {
@@ -1379,7 +1428,7 @@ struct mv_engine {
     }
     // option "level_set": the bank's rows replace the slot rings, and the per-env arrays of the mode appear (or go)
     int allocLevelSet() {
-        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free();
+        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free(); d_rowPickable.free();
         for (auto &p : ring) p.levelIds.free();
         if (const int rc = allocLevelSlots("level_set")) return rc;
         if (!levelSet) return MV_OK;
@@ -1395,18 +1444,79 @@ struct mv_engine {
         MV_CUDA(cudaMemcpy(d_bankBase.p, base.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice));
         MV_CUDA(cudaMemset(d_levelIds.p, 0, sizeof(int32_t) * n));
         MV_CUDA(cudaMemset(d_nextLevels.p, 0xFF, sizeof(int32_t) * n));  // -1: the engine picks
+        rowRetiring.assign(levelRows(), 0);
+        rowPickable.assign(levelRows(), 1);
+        if (d_rowPickable.alloc(levelRows()) != cudaSuccess) { setError("level_set: allocation failed"); return MV_ERR_CUDA; }
+        MV_CUDA(cudaMemset(d_rowPickable.p, 1, levelRows()));
         return MV_OK;
     }
     // first reset with a level set: every level of the bank, on the worker pool; flushUploads then grows the static-box arrays once, to
     // the largest level of the bank, and uploads the rows
     void scheduleBank() {
-        std::vector<int> first(size_t(numBanks), -1);
-        for (int e = E - 1; e >= 0; --e) first[size_t(envBank[size_t(e)])] = e;
+        rowSeed.resize(levelRows());
         for (int b = 0; b < numBanks; ++b)
             for (int j = 0; j < levelSet; ++j) {
-                const int f = first[size_t(b)], row = b * levelSet + j;
-                pool->submit([this, f, row, j] { generateBankLevel(f, row, j); });
+                const int f = bankFirstEnv(b), row = b * levelSet + j, seed = levelSetSeed + j;
+                rowSeed[size_t(row)] = seed;
+                pool->submit([this, f, row, seed] { generateBankLevel(gens[size_t(f)], envScenario[size_t(f)], row, seed); });
             }
+    }
+    int bankFirstEnv(int b) const { return int(std::find(envBank.begin(), envBank.end(), b) - envBank.begin()); }
+
+    // ------------------------------------------------------------------ replaceable rows (mv_replace_levels)
+    // mv_replace_levels after its checks: the rows retire at the next kernel-enqueuing call; their levels are generated meanwhile
+    void replaceLevels(const int32_t *rows, const int32_t *seeds, int n) {
+        if (!replacePool) replacePool = std::make_unique<WorkerPool>(threads);
+        for (int i = 0; i < n; ++i) {
+            auto rep = std::make_unique<Replacement>();
+            rep->row = rows[i]; rep->seed = seeds[i];
+            rowRetiring[size_t(rows[i])] = 1;
+            const int f = bankFirstEnv(rows[i] / levelSet);
+            Replacement *side = rep.get();
+            // the generator is copied here, on the caller's thread: mv_seed and mv_reset_envs may reseed gens[f] while the job runs
+            replacePool->submit([this, gen = gens[size_t(f)], sc = envScenario[size_t(f)], side] { generateBankLevel(gen, sc, side->row, side->seed, side); });
+            replacements.push_back(std::move(rep));
+        }
+    }
+    // the start of every call that enqueues the step kernel: with a level set, the rewrites that are due, then the requests made since the
+    // previous such call become retiring, and the pickable bytes go up in one copy when they changed.  Nothing at all without requests
+    int bankCall() {
+        const int64_t call = stepCalls++;
+        if (!levelSet || replacements.empty()) return MV_OK;
+        std::vector<uint8_t> held(levelRows(), 0);  // rows with an env on them as of call publishedCall
+        for (int e = 0; e < E; ++e) held[size_t(envBank[size_t(e)]) * size_t(levelSet) + size_t(h_levelIds.p[e])] = 1;
+        bool changed = false, staged = false;
+        for (auto it = replacements.begin(); it != replacements.end();) {
+            Replacement &r = **it;
+            if (r.call < 0) {
+                r.call = call;
+                rowPickable[size_t(r.row)] = 0;
+                changed = true;
+            }
+            if (r.call >= call || publishedCall < r.call || held[size_t(r.row)]) { ++it; continue; }
+            {  // due: wait for its level if the worker has not finished it
+                std::unique_lock<std::mutex> lk(genMutex);
+                replaceDone.wait(lk, [&] { return r.ready; });
+            }
+            if (!r.error.empty()) {  // as for the bank: sticky, only mv_close recovers
+                { std::lock_guard<std::mutex> lk(genMutex); genErrors.push_back(r.error); }
+                setError("level generation failed: " + r.error);
+                return MV_ERR_CAPACITY;
+            }
+            if (int(r.out.statics.size()) > staticCap) {
+                if (const int rc = growStatics(int(r.out.statics.size()))) return rc;
+            }
+            stageLevel(r.row, r.out);
+            rowSeed[size_t(r.row)] = r.seed;
+            rowRetiring[size_t(r.row)] = 0;
+            rowPickable[size_t(r.row)] = 1;
+            changed = staged = true;
+            it = replacements.erase(it);
+        }
+        if (staged) { if (const int rc = flushUploads()) return rc; }
+        // pageable source: staged before the call returns, so the vector may change at once
+        if (changed) MV_CUDA(cudaMemcpyAsync(d_rowPickable.p, rowPickable.data(), rowPickable.size(), cudaMemcpyHostToDevice, stream));
+        return MV_OK;
     }
     // mv_set_next_levels: the listed entries of the next-level array, in stream order ahead of the next kernel; runs of consecutive envs
     // go up in one copy
@@ -1436,6 +1546,9 @@ struct mv_engine {
 
     void freeAll() {
         if (pool) { pool->waitAll(); pool.reset(); }
+        replacePool.reset();  // joins its workers after the queue drains: no job outlives `replacements`
+        replacements.clear();
+        d_rowPickable.free();
         for (auto &st : stores) if (st) st->free();
         stores.clear();
         d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free();
@@ -1788,6 +1901,7 @@ int mv_reset(mv_handle h) {
     MV_ON_DEVICE(h)
     ensureMirrors(h);
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
+    if (const int rcb = h->bankCall()) return rcb;
     if (h->didReset) { const int rcd = h->drain(); if (rcd) return rcd; }
     if (!h->didReset) {
         // initial device state: the last slot / episode -1 so that the forced flip lands on (slot 0, episode 0); the first levels go to
@@ -2059,6 +2173,12 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
                         h->envScenarioName[size_t(envs[i])]);
             return MV_ERR_ARG;
         }
+        // level set: the env's bank row must still hold the level the env was saved on, and stay pickable for its next episodes' probes
+        if (r.bankRow >= 0 && (h->rowSeed[size_t(r.bankRow)] != r.bankSeed || h->rowRetiring[size_t(r.bankRow)])) {
+            h->setError("mv_states_load: row " + std::to_string(rows[i]) + " was saved on bank row " + std::to_string(r.bankRow) + " (seed " +
+                        std::to_string(r.bankSeed) + "), which " + (h->rowRetiring[size_t(r.bankRow)] ? "is being replaced" : "now holds seed " + std::to_string(h->rowSeed[size_t(r.bankRow)])));
+            return MV_ERR_ARG;
+        }
     }
     return h->statesLoad(*st, rows, envs, n);
 }
@@ -2144,6 +2264,40 @@ int mv_set_next_levels(mv_handle h, const int32_t *envs, const int32_t *levels, 
     return n ? h->setNextLevels(envs, levels, n) : MV_OK;
 }
 uint32_t mv_level_set_pick(uint32_t pick_seed, int32_t episode, int32_t count) { return mvLevelSetPick(pick_seed, episode, count); }
+
+int mv_replace_levels(mv_handle h, const int32_t *rows, const int32_t *seeds, int n) {
+    if (!h) return MV_ERR_ARG;
+    int rc = levelSetCall(h, "mv_replace_levels");
+    if (rc) return rc;
+    if ((rc = statesCallState(h, "mv_replace_levels"))) return rc;
+    if (n < 0 || (n > 0 && (!rows || !seeds))) { h->setError("mv_replace_levels: bad row / seed arrays"); return MV_ERR_ARG; }
+    const size_t B = h->levelRows();
+    std::vector<uint8_t> asked(B, 0);
+    std::vector<int> pickable(size_t(h->numBanks), 0);
+    for (size_t r = 0; r < B; ++r) pickable[r / size_t(h->levelSet)] += h->rowRetiring[r] ? 0 : 1;
+    for (int i = 0; i < n; ++i) {
+        const int r = rows[i];
+        if (r < 0 || size_t(r) >= B) { h->setError("mv_replace_levels: row " + std::to_string(r) + " is outside the bank of " + std::to_string(B)); return MV_ERR_ARG; }
+        if (asked[size_t(r)]++) { h->setError("mv_replace_levels: row " + std::to_string(r) + " is listed twice"); return MV_ERR_ARG; }
+        if (h->rowRetiring[size_t(r)]) { h->setError("mv_replace_levels: row " + std::to_string(r) + " is already being replaced"); return MV_ERR_ARG; }
+        if (--pickable[size_t(r / h->levelSet)] == 0) {
+            h->setError("mv_replace_levels: row " + std::to_string(r) + " would leave bank " + std::to_string(r / h->levelSet) + " with no pickable row");
+            return MV_ERR_ARG;
+        }
+    }
+    h->replaceLevels(rows, seeds, n);
+    return MV_OK;
+}
+
+int mv_level_rows(mv_handle h, const int32_t **seeds, const uint8_t **retiring) {
+    if (!h || !seeds || !retiring) return MV_ERR_ARG;
+    const int rc = levelSetCall(h, "mv_level_rows");
+    if (rc) return rc;
+    if (!h->didReset) { h->setError("mv_level_rows before mv_reset"); return MV_ERR_STATE; }
+    *seeds = h->rowSeed.data();
+    *retiring = h->rowRetiring.data();
+    return MV_OK;
+}
 
 int mv_fetch_obs(mv_handle h) {
     MV_ON_DEVICE(h)

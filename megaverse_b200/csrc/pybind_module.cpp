@@ -15,10 +15,12 @@
 #include <pybind11/stl.h>
 
 #include <algorithm>
+#include <cctype>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <optional>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -54,6 +56,12 @@ public:
         const int rc = mv_create_mixed(names.data(), w, h, numEnvs, numAgentsPerEnv, numSimulationThreads, device, keys.data(), vals.data(), int(keys.size()), &h__);
         if (rc != MV_OK) throw std::runtime_error(std::string("MegaverseGym: ") + mv_last_error(nullptr));
         masks_.assign(size_t(numEnvs) * numAgentsPerEnv, 0);
+        std::set<std::string> distinct;  // level-set blocks: the engine keeps one per scenario, in any spelling
+        for (auto s : scenarios) {
+            for (char &c : s) c = char(std::tolower(static_cast<unsigned char>(c)));
+            distinct.insert(s);
+        }
+        numBanks_ = int(distinct.size());
     }
     ~MegaverseGym() { close(); }
 
@@ -225,7 +233,11 @@ public:
     uintptr_t obsDevicePtr() { alive(); uint8_t *p; check(mv_obs_device(h__, &p)); return reinterpret_cast<uintptr_t>(p); }
     int faults() { alive(); int32_t f; check(mv_faults(h__, &f)); return f; }
     int faultWord() { alive(); int32_t f; check(mv_fault_word(h__, &f)); return f; }
-    void setOption(const std::string &key, int value) { alive(); check(mv_set_option(h__, key.c_str(), value)); }
+    void setOption(const std::string &key, int value) {
+        alive();
+        check(mv_set_option(h__, key.c_str(), value));
+        if (key == "level_set") levelSet_ = value;
+    }
     int levelsSkipped() { alive(); return mv_levels_skipped(h__); }
     // env state store (include/megaverse_b200.h): save / load copy on the device and wait for it, so they run without the GIL
     int statesCreate(int rows) { alive(); int id = -1; check(mv_states_create(h__, rows, &id)); return id; }
@@ -291,6 +303,21 @@ public:
         const int N = int(masks_.size());
         return py::make_tuple(py::array_t<float>({N, numRays_}, d, py::none{}), py::array_t<uint16_t>({N, numRays_}, t, py::none{}));
     }
+    // (extension, option "level_set") bank row rows[i] (block * L + level) is to hold the first level of seed seeds[i] (mv_replace_levels)
+    void replaceLevels(const std::vector<int32_t> &rows, const std::vector<int32_t> &seeds) {
+        alive();
+        if (rows.size() != seeds.size()) throw std::invalid_argument("replace_levels: rows and seeds differ in length");
+        check(mv_replace_levels(h__, rows.data(), seeds.data(), int(rows.size())));
+    }
+    // (seeds int32 [B], retiring uint8 [B]) of the bank's rows (mv_level_rows), views valid like get_level_ids'
+    py::tuple getLevelRows() {
+        alive();
+        const int32_t *seeds = nullptr;
+        const uint8_t *retiring = nullptr;
+        check(mv_level_rows(h__, &seeds, &retiring));
+        const int B = levelSet_ * numBanks_;
+        return py::make_tuple(py::array_t<int32_t>({B}, seeds, py::none{}), py::array_t<uint8_t>({B}, retiring, py::none{}));
+    }
     void setNextLevels(const std::vector<int32_t> &envs, const std::vector<int32_t> &levels) {
         alive();
         if (envs.size() != levels.size()) throw std::invalid_argument("set_next_levels: envs and levels differ in length");
@@ -345,6 +372,7 @@ private:
     int numEnvs_, numAgentsPerEnv_, w_, h_;
     int renderW_ = 768, renderH_ = 432;
     int numRays_ = 0;
+    int numBanks_ = 1, levelSet_ = 0;
     const uint8_t *hires_ = nullptr;
     std::vector<int32_t> masks_;
 };
@@ -396,6 +424,9 @@ PYBIND11_MODULE(megaverse, m) {
         .def("level_ids", &MegaverseGym::getLevelIds, "int32[num_envs] (option level_set): the level of the set each env is on; after an end, the new episode's")
         .def("set_next_levels", &MegaverseGym::setNextLevels, py::arg("envs"), py::arg("levels"),
              "(option level_set) env envs[i] plays level levels[i] in its next episode, once; followed by reset_envs(envs) it starts them on those levels now")
+        .def("replace_levels", &MegaverseGym::replaceLevels, py::arg("rows"), py::arg("seeds"),
+             "(option level_set) bank row rows[i] is to hold the first level of seed seeds[i]; it retires at the next call and is rewritten once no env is on it")
+        .def("get_level_rows", &MegaverseGym::getLevelRows, "(option level_set) (seeds int32[B], retiring uint8[B]) of the bank's rows")
         .def("get_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(false); },
              "dict of float32 views (option state_tensors): agents [N,16], envs [E,16], objects [E,128,4], rewards [E,128,4]")
         .def("set_rays", &MegaverseGym::setRays, py::arg("directions"), py::arg("max_distance"),

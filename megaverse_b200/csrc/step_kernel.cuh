@@ -100,6 +100,9 @@ struct StepParams {
     // env's terminal frame shows.
     float *stAgents, *stEnvs, *stObjects, *stRewards;
     float *termStAgents, *termStEnvs, *termStObjects, *termStRewards;
+    // level set: [levelSet * banks] 0 for a row being replaced (mv_replace_levels), which no flip may land on; the host keeps at least one
+    // row of every bank pickable.  Last, so that no other field moves
+    const uint8_t *rowPickable;
 };
 
 // row of the level arrays that holds slot `slot` of env `env`: the env's own ring of slots, or, with a level set, the bank row itself
@@ -1621,13 +1624,19 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
         if (kLevelSet) {
             // level set: the next level is a row of the bank, chosen here -- the caller's choice when it names a level of the set (used once),
             // else the hash of the env's pick seed and the new episode's index.  The entry comes from outside the engine: it is bounded
-            // before it indexes anything, and a value out of range is left alone and ignored.  Bank rows are always there: no serial check
+            // before it indexes anything, and a value out of range is left alone and ignored.  Bank rows are always there: no serial check.
+            // A row being replaced is not pickable: an entry naming it stays for a later end, and the hash probes forward to the next row
             if (lane == 0) {
                 S.env.episode_idx += 1;
+                const int base = P.bankBase[env];
                 int j = P.nextLevels[env];
-                if (j >= 0 && j < P.levelSet) P.nextLevels[env] = -1;
-                else j = int(mvLevelSetPick(uint32_t(S.env.pad[0]), S.env.episode_idx, P.levelSet));
-                S.env.slot = P.bankBase[env] + j;
+                if (j >= 0 && j < P.levelSet && P.rowPickable[base + j]) {
+                    P.nextLevels[env] = -1;
+                } else {
+                    j = int(mvLevelSetPick(uint32_t(S.env.pad[0]), S.env.episode_idx, P.levelSet));
+                    for (int k = 0; k < P.levelSet && !P.rowPickable[base + j]; ++k) j = j + 1 == P.levelSet ? 0 : j + 1;
+                }
+                S.env.slot = base + j;
             }
             __syncwarp();
             slot = S.env.slot;

@@ -206,6 +206,41 @@ class MegaverseEnv(Env):
         set_next_levels(envs, levels) followed by reset_envs(envs) starts the listed envs on the listed levels now."""
         self.env.set_next_levels([int(e) for e in envs], [int(j) for j in levels])
 
+    def _level_block(self, scenario):
+        """the bank block of `scenario` (the batch's distinct scenarios in order of first appearance); None names the only one"""
+        if self.num_levels is None:
+            raise ValueError('level replacement needs num_levels')
+        blocks = list(dict.fromkeys(self.scenarios))
+        if scenario is None:
+            if len(blocks) > 1:
+                raise ValueError('a mixed batch needs scenario= to name the block of levels')
+            return 0
+        if scenario.casefold() not in blocks:
+            raise ValueError('scenario %r is not in this batch' % scenario)
+        return blocks.index(scenario.casefold())
+
+    def replace_levels(self, levels, seeds, scenario=None):
+        """(extension, num_levels given) level levels[i] of the set (of `scenario`'s block in a mixed batch) is to become the first level of
+        seed seeds[i].  Envs playing it finish their episodes on the old level; no env starts it from the next call on, and it is rewritten
+        at the start of the first call after a finished call showed no env on it.  Prioritised Level Replay and other curricula use it to
+        add fresh levels to the set and evict others."""
+        levels, seeds = [int(j) for j in levels], [int(s) for s in seeds]
+        if len(levels) != len(seeds):
+            raise ValueError('%d levels and %d seeds' % (len(levels), len(seeds)))
+        b = self._level_block(scenario)
+        for j in levels:
+            if not 0 <= j < self.num_levels:
+                raise ValueError('level %d is outside the set of %d' % (j, self.num_levels))
+        self.env.replace_levels([b * self.num_levels + j for j in levels], seeds)
+
+    def level_seeds(self, scenario=None):
+        """(extension, num_levels given) per level of the set (of `scenario`'s block in a mixed batch), the seed of the level it holds now:
+        start_level + j until replace_levels rewrites it.  After step(), level_seeds()[info['level']] is the seed of the level a finished
+        episode was played on (its level cannot be rewritten before a later call)."""
+        b = self._level_block(scenario)
+        seeds, _ = self.env.get_level_rows()
+        return [int(s) for s in seeds[b * self.num_levels:(b + 1) * self.num_levels]]
+
     def reset(self):
         self.env.reset()
         self.check_faults()
