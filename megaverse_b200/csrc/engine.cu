@@ -29,6 +29,7 @@
 #include <queue>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "../../include/megaverse_b200.h"
@@ -118,18 +119,59 @@ private:
     bool stop_ = false;
 };
 
-template <typename T> struct DevBuf {
+// The owners of the engine's CUDA resources.  Each releases what it holds when it is destroyed or given something else, and moves but
+// never copies, so that every buffer, event and stream has exactly one owner.
+//
+// `count` elements of T in HBM (DevBuf) or in pinned host memory (PinBuf).  alloc first releases what the buffer holds and leaves it
+// empty (p null, n 0) when it fails; free releases it early
+template <typename T, bool Pinned> struct CudaBuf {
     T *p = nullptr;
     size_t n = 0;
-    cudaError_t alloc(size_t count) { n = count; return cudaMalloc(reinterpret_cast<void **>(&p), sizeof(T) * (count ? count : 1)); }
-    void free() { if (p) cudaFree(p); p = nullptr; }
+    CudaBuf() = default;
+    CudaBuf(const CudaBuf &) = delete;
+    CudaBuf &operator=(const CudaBuf &) = delete;
+    CudaBuf(CudaBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+    CudaBuf &operator=(CudaBuf &&o) noexcept {
+        if (this != &o) { free(); p = std::exchange(o.p, nullptr); n = std::exchange(o.n, 0); }
+        return *this;
+    }
+    ~CudaBuf() { free(); }
+    cudaError_t alloc(size_t count) {
+        free();
+        void *q = nullptr;
+        const size_t bytes = sizeof(T) * (count ? count : 1);
+        const cudaError_t err = Pinned ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes);
+        if (err == cudaSuccess) { p = static_cast<T *>(q); n = count; }
+        return err;
+    }
+    void free() {
+        if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); }
+        p = nullptr; n = 0;
+    }
 };
-template <typename T> struct PinBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    cudaError_t alloc(size_t count) { n = count; return cudaMallocHost(reinterpret_cast<void **>(&p), sizeof(T) * (count ? count : 1)); }
-    void free() { if (p) cudaFreeHost(p); p = nullptr; }
+template <typename T> using DevBuf = CudaBuf<T, false>;
+template <typename T> using PinBuf = CudaBuf<T, true>;
+
+// an event or a stream, created with flags; call sites take the raw handle through the conversion
+template <typename H, cudaError_t (*Create)(H *, unsigned int), cudaError_t (*Destroy)(H)> struct CudaHandle {
+    H h = nullptr;
+    CudaHandle() = default;
+    CudaHandle(const CudaHandle &) = delete;
+    CudaHandle &operator=(const CudaHandle &) = delete;
+    CudaHandle(CudaHandle &&o) noexcept : h(std::exchange(o.h, nullptr)) {}
+    CudaHandle &operator=(CudaHandle &&o) noexcept {
+        if (this != &o) { release(); h = std::exchange(o.h, nullptr); }
+        return *this;
+    }
+    ~CudaHandle() { release(); }
+    cudaError_t create(unsigned int flags) { release(); return Create(&h, flags); }
+    operator H() const { return h; }
+
+private:
+    void release() { if (h) Destroy(h); h = nullptr; }
 };
+using CudaEvent = CudaHandle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
+using CudaStream = CudaHandle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
 
 // one per-env device array as the state store sees it: `units` rows per env (the slot count for the arrays that hold the level slots, none
 // of them with a level set) of unitBytes
@@ -162,7 +204,6 @@ struct StateStore {
         std::vector<std::vector<uint32_t>> solid;  // the three bit planes, levelWords words each
     };
     std::vector<HostRow> host;
-    void free() { for (auto &s : slabs) s.free(); for (auto &s : stateSlabs) s.free(); }
 };
 
 }  // namespace
@@ -187,6 +228,8 @@ static mvr::ViewParams frameParams(int W, int H, int bands, int bandRows, unsign
 // corner differences ~ 17 400 (the hex mazes; tests/test_raster_independent.py measures them): at 768 wide |s| <= 2^30.06 and the
 // differences <= 2^30.67; at 1024 the differences reach 2^31.08.
 constexpr int kMaxRasterWidth = 768;
+// triangle-list capacity of one raster CTA (shared memory) unless option tri_cap sets another; larger views are drawn in several batches
+constexpr int kDefaultTriCap = 368;
 
 // Frames drawn beside the step's own (mv_draw_hires, the camera launches, mv_debug_render_instances_ex's default): row bands of about a
 // hundred 32x4 tiles each, so that a large frame keeps every CTA of the persistent grid busy
@@ -234,7 +277,7 @@ struct mv_engine {
 
     // pitch of the per-env grid arrays: the largest dense-grid capacity among the engine's scenarios (one pitch for all envs)
     int gridCells = 0, gridWords = 0;
-    int triCap = 368;              // triangle-list capacity of one raster CTA (shared memory); larger views are drawn in several batches
+    int triCap = kDefaultTriCap;
     std::atomic<int> maxObjSeen{0};
     bool wantDepth = false, obsToHost = true, didReset = false, fastShading = true;
     bool wantSeg = false;          // option "segmentation": the rasteriser also writes each pixel's drawable tag (d_seg / h_seg)
@@ -254,16 +297,16 @@ struct mv_engine {
     bool hostObsFresh = false, ownDeviceObsFresh = false;
     bool ownDeviceBuffers() const { return obsOut == d_obs.p && (!wantDepth || depthOut == d_depth.p); }
     int sliceCount = 1;            // this launch: > 1 = sliced download on copyStream
-    cudaStream_t copyStream = nullptr;
-    std::vector<cudaEvent_t> sliceEv;
+    CudaStream copyStream;
+    std::vector<CudaEvent> sliceEv;
     int numSMs = 132;              // H100 SXM; replaced by the device's count in mv_create
     MvConsts consts{};
 
-    cudaStream_t stream = nullptr;
+    CudaStream stream;
     // kernel times of the last timed call, read by readKernelTimes only.  The call records ev[0] before its first kernel, ev[1] after it
     // when its raster launch is serialised behind it, evFinal before a terminal-frame launch and ev[2] at the end
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-    cudaEvent_t evFinal = nullptr;
+    CudaEvent ev[3];
+    CudaEvent evFinal;
     enum class Timed { Union, Split, FirstOnly } timedAs = Timed::Union;  // no ev[1] (overlapping kernels), ev[1], no raster launch (a save)
     bool lastHadFinal = false;
     float lastMs[2] = {0, 0};
@@ -350,7 +393,6 @@ struct mv_engine {
         int W = 0, H = 0;
         DevBuf<uint8_t> d_obs; PinBuf<uint8_t> h_obs;
         DevBuf<unsigned long long> spill;
-        void free() { d_obs.free(); h_obs.free(); spill.free(); W = H = 0; }
     } hires;
     // camera launches (mv_draw_cameras[_device]): the host call's tables and output buffers, grown on demand and kept; the spill slab and
     // the out-of-range counter serve both calls
@@ -361,10 +403,6 @@ struct mv_engine {
         DevBuf<unsigned long long> spill;
         DevBuf<uint32_t> d_range;  // [1] triangles of the last camera launch outside the integer set-up's exact range
         PinBuf<uint32_t> h_range;
-        void free() {
-            d_env.free(); d_views.free(); d_obs.free(); d_depth.free(); d_seg.free(); h_obs.free(); h_depth.free(); h_seg.free(); spill.free();
-            d_range.free(); h_range.free();
-        }
     } cams;
     int cameraGrid = 0;  // persistent grid of the camera variants
     DevBuf<MvDeco> d_deco;         // [E][D][decoCap]
@@ -391,7 +429,7 @@ struct mv_engine {
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
     // mv_step_device pipeline: results of step k are consumed by the host while steps k+1, k+2 already run
-    struct Pending { bool valid = false; uint64_t step = 0; int64_t call = 0; cudaEvent_t ev = nullptr; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
+    struct Pending { bool valid = false; uint64_t step = 0; int64_t call = 0; CudaEvent ev; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
     std::vector<int64_t> lastAsyncDone;  // [E] asynchronous step index of the env's previous episode end
     bool asyncContractBroken = false;
     Pending ring[3];
@@ -442,7 +480,7 @@ struct mv_engine {
     // on copyStream while the frames are drawn; mv_step_device leaves it in HBM (mv_fetch_obs copies it down).
     bool wantState = false;
     bool stateCopyPending = false;  // this call's block download is on copyStream
-    cudaEvent_t evState = nullptr;  // the step kernel's rows are written: the download may start
+    CudaEvent evState;              // the step kernel's rows are written: the download may start
     DevBuf<float> d_state;
     PinBuf<float> h_state;
     size_t stateFloats() const { return size_t(N) * 16 + size_t(E) * (16 + 4 * MV_MAX_OBJECTS + 4 * MV_MAX_REWARD); }
@@ -478,7 +516,7 @@ struct mv_engine {
     DevBuf<uint16_t> d_rayTag;
     PinBuf<float> h_rayDist;
     PinBuf<uint16_t> h_rayTag;
-    cudaEvent_t evRays = nullptr;   // before a timed call's ray launches (readKernelTimes)
+    CudaEvent evRays;               // before a timed call's ray launches (readKernelTimes)
     bool lastHadRays = false;
     float lastRaysMs = 0.0f;
     size_t rayCount() const { return size_t(N) * size_t(nRays); }
@@ -597,8 +635,6 @@ struct mv_engine {
     // decorations and the three bit planes; and the instance rows, whose pitch staticCap sets as well
     int allocLevelSlots(const char *what) {
         const size_t rows = levelRows(), cap = size_t(staticCap), deco = size_t(decoCap), words = size_t(gridWords) * 3;
-        d_levels.free(); d_statics.free(); d_staticRot.free(); d_deco.free(); d_solid.free(); d_inst.free();
-        h_levels.free(); h_statics.free(); h_staticRot.free(); h_deco.free(); h_solid.free();
         levelWords.assign(rows, 0);
         instCap = MV_DYN_INSTANCES + staticCap + decoCap;
         if (d_levels.alloc(rows) != cudaSuccess || d_statics.alloc(rows * cap) != cudaSuccess || d_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
@@ -635,15 +671,12 @@ struct mv_engine {
         for (auto &g : storeGrow) storesOk = storesOk && g.next.alloc(g.rows * g.newPitch) == cudaSuccess;
         if (!storesOk || nStat.alloc(rows * newCap) != cudaSuccess || nRot.alloc(rows * newCap * 2) != cudaSuccess || nInst.alloc(size_t(E) * newInstCap) != cudaSuccess ||
             hStat.alloc(rows * newCap) != cudaSuccess || hRot.alloc(rows * newCap * 2) != cudaSuccess) {
-            nStat.free(); nRot.free(); nInst.free(); hStat.free(); hRot.free();
-            for (auto &g : storeGrow) g.next.free();
             setError("growing the static-box arrays: allocation failed");
             return MV_ERR_CUDA;
         }
         for (auto &g : storeGrow) {
             MV_CUDA(cudaMemcpy2D(g.next.p, g.newPitch, g.buf->p, g.oldPitch, g.oldPitch, g.rows, cudaMemcpyDeviceToDevice));
-            g.buf->free();
-            *g.buf = g.next;
+            *g.buf = std::move(g.next);
         }
         MV_CUDA(cudaMemcpy2D(nStat.p, sizeof(MvBox) * newCap, d_statics.p, sizeof(MvBox) * staticCap, sizeof(MvBox) * staticCap, rows, cudaMemcpyDeviceToDevice));
         MV_CUDA(cudaMemcpy2D(nRot.p, sizeof(float) * 2 * newCap, d_staticRot.p, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * staticCap, rows, cudaMemcpyDeviceToDevice));
@@ -652,11 +685,9 @@ struct mv_engine {
             std::memcpy(hStat.p + r * newCap, h_statics.p + r * staticCap, sizeof(MvBox) * staticCap);
             std::memcpy(hRot.p + r * newCap * 2, h_staticRot.p + r * staticCap * 2, sizeof(float) * 2 * staticCap);
         }
-        d_statics.free(); d_staticRot.free(); d_inst.free(); h_statics.free(); h_staticRot.free();
-        d_statics = nStat; d_staticRot = nRot; d_inst = nInst; h_statics = hStat; h_staticRot = hRot;
+        d_statics = std::move(nStat); d_staticRot = std::move(nRot); d_inst = std::move(nInst); h_statics = std::move(hStat); h_staticRot = std::move(hRot);
         staticCap = newCap; instCap = newInstCap;
         if (d_termInst.p) {  // no copy: a terminal row is written whole before the launch that reads it
-            d_termInst.free();
             if (d_termInst.alloc(size_t(E) * size_t(instCap)) != cudaSuccess) { setError("growing the terminal instance rows: allocation failed"); return MV_ERR_CUDA; }
         }
         return MV_OK;
@@ -858,7 +889,7 @@ struct mv_engine {
             vp.envMask = mask ? mask + base / A : nullptr;
             const int rc = launchView(vp, dep && si == 0, items);
             if (rc) return rc;
-            while (int(sliceEv.size()) <= si) { cudaEvent_t e2; MV_CUDA(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming)); sliceEv.push_back(e2); }
+            while (int(sliceEv.size()) <= si) { CudaEvent e2; MV_CUDA(e2.create(cudaEventDisableTiming)); sliceEv.push_back(std::move(e2)); }
             MV_CUDA(cudaEventRecord(sliceEv[size_t(si)], stream));
             MV_CUDA(cudaStreamWaitEvent(copyStream, sliceEv[size_t(si)], 0));
             if (const int rcd = downloadViews(base, cnt, copyStream)) return rcd;
@@ -896,10 +927,9 @@ struct mv_engine {
         int rc = drain();
         if (rc) return rc;
         if (hires.W != w || hires.H != hgt) {
-            hires.free();
+            hires = {};  // the old size's buffers go before the new ones are allocated
             const size_t px = size_t(N) * w * hgt * 4;
             if (hires.d_obs.alloc(px) != cudaSuccess || hires.h_obs.alloc(px) != cudaSuccess) {
-                hires.free();
                 setError("hi-res buffers: allocation failed");
                 return MV_ERR_CUDA;
             }
@@ -907,7 +937,7 @@ struct mv_engine {
         }
         mvr::ViewParams vp;
         rc = bandedFrame(w, hgt, rasterGrid, hires.spill, vp);
-        if (rc) { hires.free(); return rc; }
+        if (rc) return rc;
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         vp.obs = hires.d_obs.p;
         vp.viewBase = 0; vp.N = N;
@@ -1046,9 +1076,8 @@ struct mv_engine {
         }
         cameraGrid = numSMs * std::max(1, std::min(cameraPerSM, rasterCtasPerSM));
         bandRows = ((H / 4 + rasterBands - 1) / rasterBands) * 4;
-        d_spill.free();
         if (d_spill.alloc(size_t(rasterGrid) * W * bandRows) != cudaSuccess) { setError("raster spill slab allocation failed"); return MV_ERR_CUDA; }
-        hires.free();  // its spill slab is sized by the grid
+        hires = {};  // its spill slab is sized by the grid
         return MV_OK;
     }
 
@@ -1251,9 +1280,9 @@ struct mv_engine {
         st->rows = rows;
         const auto sl = envSlabs();
         for (int k = 0; k < kSlabCount; ++k)
-            if (st->slabs[k].alloc(size_t(rows) * sl[size_t(k)].rowBytes()) != cudaSuccess) { st->free(); setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
+            if (st->slabs[k].alloc(size_t(rows) * sl[size_t(k)].rowBytes()) != cudaSuccess) { setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
         for (int k = 0; k < 4 && wantState; ++k)
-            if (st->stateSlabs[k].alloc(size_t(rows) * stateRowBytes(k)) != cudaSuccess) { st->free(); setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
+            if (st->stateSlabs[k].alloc(size_t(rows) * stateRowBytes(k)) != cudaSuccess) { setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
         st->host.resize(size_t(rows));
         stores.push_back(std::move(st));
         *id = int(stores.size()) - 1;
@@ -1268,10 +1297,9 @@ struct mv_engine {
     // one copy kernel over all listed rows.  toStore: engine row pairs[i].x -> store row pairs[i].y; else back, and every view is drawn
     // again behind the copy
     int copyStateRows(StateStore &st, const int32_t *from, const int32_t *to, int n, bool toStore) {
-        if (size_t(n) > h_pairs.n) {
+        if (size_t(n) > std::min(h_pairs.n, d_pairs.n)) {
             MV_CUDA(cudaStreamSynchronize(stream));  // the previous upload may still read the pinned pairs
-            h_pairs.free(); d_pairs.free();
-            if (h_pairs.alloc(size_t(n)) != cudaSuccess || d_pairs.alloc(size_t(n)) != cudaSuccess) { h_pairs.free(); d_pairs.free(); setError("state pairs: allocation failed"); return MV_ERR_CUDA; }
+            if (h_pairs.alloc(size_t(n)) != cudaSuccess || d_pairs.alloc(size_t(n)) != cudaSuccess) { setError("state pairs: allocation failed"); return MV_ERR_CUDA; }
         }
         for (int i = 0; i < n; ++i) h_pairs.p[i] = make_int2(from[i], to[i]);
         MV_CUDA(cudaMemcpyAsync(d_pairs.p, h_pairs.p, sizeof(int2) * size_t(n), cudaMemcpyHostToDevice, stream));
@@ -1426,10 +1454,8 @@ struct mv_engine {
         MV_CUDA(cudaStreamSynchronize(stream));  // pageable source
         return MV_OK;
     }
-    // option "level_set": the bank's rows replace the slot rings, and the per-env arrays of the mode appear (or go)
+    // option "level_set": the bank's rows replace the slot rings, and the per-env arrays of the mode appear
     int allocLevelSet() {
-        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free(); d_rowPickable.free();
-        for (auto &p : ring) p.levelIds.free();
         if (const int rc = allocLevelSlots("level_set")) return rc;
         if (!levelSet) return MV_OK;
         const size_t n = size_t(E);
@@ -1544,33 +1570,14 @@ struct mv_engine {
         return MV_OK;
     }
 
-    void freeAll() {
+    // Every member releases what it owns, in reverse order of declaration.  That order alone is not safe: the level workers (pool) write
+    // into the pinned mirrors declared after it, replacePool's jobs into `replacements`, and both streams may still run work that reads or
+    // writes the buffers.  So the workers are joined and the streams drained first.  Runs on the engine's device (mv_close, mv_create).
+    ~mv_engine() {
         if (pool) { pool->waitAll(); pool.reset(); }
         replacePool.reset();  // joins its workers after the queue drains: no job outlives `replacements`
-        replacements.clear();
-        d_rowPickable.free();
-        for (auto &st : stores) if (st) st->free();
-        stores.clear();
-        d_bankBase.free(); d_levelIds.free(); d_nextLevels.free(); h_levelIds.free(); h_nextLevels.free();
-        h_pairs.free(); d_pairs.free(); h_envList.free(); d_envList.free(); h_active.free(); d_active.free();
-        d_levels.free(); d_statics.free(); d_staticRot.free(); h_statics.free(); h_staticRot.free(); d_solid.free(); d_objGrid.free(); d_envs.free(); d_agents.free(); d_objects.free(); d_inst.free(); d_instCounts.free();
-        d_views.free(); d_actions.free(); d_rtable.free(); d_rewards.free(); d_dones.free(); d_trueObj.free(); d_obs.free(); d_depth.free(); d_seg.free(); d_faults.free();
-        hires.free(); cams.free(); d_deco.free(); h_deco.free(); d_prof.free(); d_ready.free(); d_workCounter.free(); d_spill.free(); d_rasterStats.free(); d_viewCost.free();
-        h_levels.free(); h_solid.free(); h_actions.free(); h_rtable.free(); h_rewards.free(); h_dones.free(); h_trueObj.free(); h_obs.free(); h_depth.free(); h_seg.free();
-        h_faults.free(); h_faultWord.free();
-        d_doneReasons.free(); h_doneReasons.free();
-        d_termInst.free(); d_termCounts.free(); d_termViews.free(); d_finalObs.free(); d_finalDepth.free(); h_finalObs.free(); h_finalDepth.free();
-        d_state.free(); h_state.free();
-        if (evState) { cudaEventDestroy(evState); evState = nullptr; }
-        d_rayDirs.free(); d_rayDist.free(); d_rayTag.free(); h_rayDist.free(); h_rayTag.free();
-        if (evRays) { cudaEventDestroy(evRays); evRays = nullptr; }
-        for (auto &e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
-        if (evFinal) { cudaEventDestroy(evFinal); evFinal = nullptr; }
-        for (auto &p : ring) { if (p.ev) { cudaEventDestroy(p.ev); p.ev = nullptr; } p.rewards.free(); p.trueObj.free(); p.dones.free(); p.reasons.free(); p.levelIds.free(); }
-        for (auto &e2 : sliceEv) if (e2) cudaEventDestroy(e2);
-        sliceEv.clear();
-        if (copyStream) { cudaStreamDestroy(copyStream); copyStream = nullptr; }
-        if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
+        if (stream) cudaStreamSynchronize(stream);
+        if (copyStream) cudaStreamSynchronize(copyStream);
     }
 };
 
@@ -1579,16 +1586,14 @@ namespace {
 const uint32_t kPaletteRgb[22] = {0xffdd3c, 0x3bb372, 0x50c878, 0x2eb5d0, 0xadd8e6, 0x3a7fa6, 0x2c3e50, 0xffb400, 0xb3b3b3, 0x555555, 0x222222,
                                   0xffffff, 0xff0000, 0xffa770, 0xd468ee, 0xffe6e6, 0xffffe6, 0xccffcc, 0xe6ecff, 0xd9d9d9, 0xf2e6ff, 0xffebcc};
 
-int uploadPalette(mv_engine *h) {
+cudaError_t uploadPalette() {
     float pal[22][3];
     for (int i = 0; i < 22; ++i) {  // toRgbf: byte / 255 (util/magnum.hpp:25-32)
         pal[i][0] = float((kPaletteRgb[i] >> 16) & 255) / 255.0f;
         pal[i][1] = float((kPaletteRgb[i] >> 8) & 255) / 255.0f;
         pal[i][2] = float(kPaletteRgb[i] & 255) / 255.0f;
     }
-    cudaError_t err = cudaMemcpyToSymbol(mvr::c_palette, pal, sizeof(pal));
-    if (err != cudaSuccess) { h->setError(std::string("palette upload: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
-    return MV_OK;
+    return cudaMemcpyToSymbol(mvr::c_palette, pal, sizeof(pal));
 }
 
 int setKernelAttrs(mv_engine *h) {
@@ -1658,7 +1663,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { g_createError = "no CUDA device: megaverse_b200 has no CPU fallback"; return MV_ERR_CUDA; }
     if (device < 0 || device >= ndev) { g_createError = "bad CUDA device ordinal"; return MV_ERR_ARG; }
     auto *e = new mv_engine;
-    auto fail = [&](int code) { g_createError = e->error; e->freeAll(); delete e; return code; };
+    auto fail = [&](int code) { g_createError = e->error; delete e; return code; };
     DeviceGuard dg__(device);
     if (!dg__.ok) { e->setError("cudaSetDevice failed"); return fail(MV_ERR_CUDA); }
     e->W = w; e->H = h; e->E = num_envs; e->A = num_agents; e->N = num_envs * num_agents; e->device = device;
@@ -1708,9 +1713,9 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
 
     auto ck = [&](cudaError_t err, const char *what) { if (err != cudaSuccess) { e->setError(std::string(what) + ": " + cudaGetErrorString(err)); return false; } return true; };
     const size_t E = size_t(e->E), N = size_t(e->N), px = size_t(w) * h;
-    bool ok = ck(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking), "stream") && ck(cudaStreamCreateWithFlags(&e->copyStream, cudaStreamNonBlocking), "copy stream");
-    for (auto &evx : e->ev) ok = ok && ck(cudaEventCreate(&evx), "event");
-    ok = ok && ck(cudaEventCreate(&e->evFinal), "event");
+    bool ok = ck(e->stream.create(cudaStreamNonBlocking), "stream") && ck(e->copyStream.create(cudaStreamNonBlocking), "copy stream");
+    for (auto &evx : e->ev) ok = ok && ck(evx.create(cudaEventDefault), "event");
+    ok = ok && ck(e->evFinal.create(cudaEventDefault), "event");
     ok = ok && e->allocLevelSlots("level slots") == MV_OK && ck(e->d_objGrid.alloc(E * e->gridCells), "objGrid") &&
          ck(e->d_envs.alloc(E), "envs") && ck(e->d_agents.alloc(N), "agents") && ck(e->d_objects.alloc(E * MV_MAX_OBJECTS), "objects") &&
          ck(e->d_instCounts.alloc(E * 8), "instCounts") && ck(e->d_views.alloc(N * 16), "views") &&
@@ -1732,7 +1737,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
          ck(e->h_rtable.alloc(N * MV_R_COUNT), "h_rtable") && ck(e->h_rewards.alloc(N), "h_rewards") && ck(e->h_dones.alloc(E), "h_dones") && ck(e->h_doneReasons.alloc(E), "h_doneReasons") &&
          ck(e->h_trueObj.alloc(N), "h_trueObj") && ck(e->h_obs.alloc(N * px * 4), "h_obs") && ck(e->h_faults.alloc(E), "h_faults") && ck(e->h_faultWord.alloc(1), "h_faultWord") &&
          ck(e->h_envList.alloc(E), "h_envList") && ck(e->d_envList.alloc(E), "envList") && ck(e->h_active.alloc(E), "h_active") && ck(e->d_active.alloc(E), "active");
-    for (auto &p : e->ring) ok = ok && ck(cudaEventCreateWithFlags(&p.ev, cudaEventDisableTiming), "event") && ck(p.rewards.alloc(N), "ring") && ck(p.trueObj.alloc(N), "ring") && ck(p.dones.alloc(E), "ring") && ck(p.reasons.alloc(E), "ring");
+    for (auto &p : e->ring) ok = ok && ck(p.ev.create(cudaEventDisableTiming), "event") && ck(p.rewards.alloc(N), "ring") && ck(p.trueObj.alloc(N), "ring") && ck(p.dones.alloc(E), "ring") && ck(p.reasons.alloc(E), "ring");
     if (!ok) return fail(MV_ERR_CUDA);
     std::memset(e->h_actions.p, 0, sizeof(int32_t) * N);
     e->h_faultWord.p[0] = 0;
@@ -1747,7 +1752,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
          ck(cudaMemset(e->d_objects.p, 0, sizeof(MvObject) * E * MV_MAX_OBJECTS), "memset");
     if (!ok) return fail(MV_ERR_CUDA);
     e->obsOut = e->d_obs.p;
-    if (uploadPalette(e) != MV_OK) return fail(MV_ERR_CUDA);
+    if (!ck(uploadPalette(), "palette upload")) return fail(MV_ERR_CUDA);
     if (setKernelAttrs(e) != MV_OK) return fail(MV_ERR_CUDA);
     *out = e;
     return MV_OK;
@@ -1759,26 +1764,23 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     const std::string k = key;
     if (k == "depth") {
         if (h->didReset) { h->setError("option depth must be set before the first reset"); return MV_ERR_STATE; }
-        h->wantDepth = value != 0;
-        if (h->wantDepth && !h->d_depth.p) {
+        // on only once both buffers exist: a failed allocation leaves the option off and no buffer held
+        if (value != 0 && !h->d_depth.p) {
             const size_t cnt = size_t(h->N) * h->W * h->H;
-            if (h->d_depth.alloc(cnt) != cudaSuccess || h->h_depth.alloc(cnt) != cudaSuccess) { h->setError("depth allocation failed"); return MV_ERR_CUDA; }
+            if (h->d_depth.alloc(cnt) != cudaSuccess || h->h_depth.alloc(cnt) != cudaSuccess) { h->d_depth.free(); h->setError("depth allocation failed"); return MV_ERR_CUDA; }
             if (!h->depthOut) h->depthOut = h->d_depth.p;
         }
+        h->wantDepth = value != 0;
         return MV_OK;
     }
     if (k == "segmentation") {  // the drawable behind every pixel (see the header); the buffers are allocated here, only when it is on
         if (h->didReset) { h->setError("option segmentation must be set before the first reset"); return MV_ERR_STATE; }
         if (value != 0 && value != 1) { h->setError("segmentation must be 0 or 1"); return MV_ERR_ARG; }
-        h->wantSeg = value != 0;
-        if (h->wantSeg && !h->d_seg.p) {
+        if (value && !h->d_seg.p) {  // as for depth
             const size_t cnt = size_t(h->N) * h->W * h->H;
-            if (h->d_seg.alloc(cnt) != cudaSuccess || h->h_seg.alloc(cnt) != cudaSuccess) {
-                h->d_seg.free(); h->h_seg.free(); h->wantSeg = false;
-                h->setError("segmentation allocation failed");
-                return MV_ERR_CUDA;
-            }
+            if (h->d_seg.alloc(cnt) != cudaSuccess || h->h_seg.alloc(cnt) != cudaSuccess) { h->d_seg.free(); h->setError("segmentation allocation failed"); return MV_ERR_CUDA; }
         }
+        h->wantSeg = value != 0;
         return MV_OK;
     }
     if (k == "final_obs") {  // terminal frames of ended episodes; the buffers are allocated by the first reset (after "depth" / "static_cap")
@@ -1918,7 +1920,6 @@ int mv_reset(mv_handle h) {
                 h->d_finalObs.alloc(N * px * 4) != cudaSuccess || h->h_finalObs.alloc(N * px * 4) != cudaSuccess ||
                 (h->wantDepth && (h->d_finalDepth.alloc(N * px) != cudaSuccess || h->h_finalDepth.alloc(N * px) != cudaSuccess)) ||
                 cudaMemset(h->d_finalObs.p, 0, N * px * 4) != cudaSuccess || (h->wantDepth && cudaMemset(h->d_finalDepth.p, 0, sizeof(float) * N * px) != cudaSuccess)) {
-                h->d_termInst.free(); h->d_termCounts.free(); h->d_termViews.free(); h->d_finalObs.free(); h->h_finalObs.free(); h->d_finalDepth.free(); h->h_finalDepth.free();
                 h->setError("final_obs: allocation failed");
                 return MV_ERR_CUDA;
             }
@@ -1928,8 +1929,7 @@ int mv_reset(mv_handle h) {
         if (h->wantState) {  // the live rows and, with final_obs, the terminal rows: one block, zero until written
             const size_t n = h->stateBlockFloats();
             if (h->d_state.alloc(n) != cudaSuccess || h->h_state.alloc(n) != cudaSuccess || cudaMemset(h->d_state.p, 0, sizeof(float) * n) != cudaSuccess ||
-                cudaEventCreateWithFlags(&h->evState, cudaEventDisableTiming) != cudaSuccess) {
-                h->d_state.free(); h->h_state.free();
+                h->evState.create(cudaEventDisableTiming) != cudaSuccess) {
                 h->setError("state_tensors: allocation failed");
                 return MV_ERR_CUDA;
             }
@@ -1941,8 +1941,7 @@ int mv_reset(mv_handle h) {
                 h->h_rayDist.alloc(n) != cudaSuccess || h->h_rayTag.alloc(n) != cudaSuccess ||
                 cudaMemcpy(h->d_rayDirs.p, h->rayDirs.data(), sizeof(float) * h->rayDirs.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
                 cudaMemset(h->d_rayDist.p, 0, sizeof(float) * n) != cudaSuccess || cudaMemset(h->d_rayTag.p, 0, sizeof(uint16_t) * n) != cudaSuccess ||
-                cudaEventCreate(&h->evRays) != cudaSuccess) {
-                h->d_rayDirs.free(); h->d_rayDist.free(); h->d_rayTag.free(); h->h_rayDist.free(); h->h_rayTag.free();
+                h->evRays.create(cudaEventDefault) != cudaSuccess) {
                 h->setError("rays: allocation failed");
                 return MV_ERR_CUDA;
             }
@@ -2218,7 +2217,6 @@ int mv_states_destroy(mv_handle h, int store) {
     StateStore *st = findStore(h, store, "mv_states_destroy");
     if (!st) return MV_ERR_ARG;
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
-    st->free();
     h->stores[size_t(store)].reset();
     return MV_OK;
 }
@@ -2574,8 +2572,6 @@ int mv_last_rays_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_ARG
 int mv_close(mv_handle h) {
     if (!h) return MV_ERR_ARG;
     DeviceGuard dg__(h->device);  // not MV_ON_DEVICE: the engine is freed even when the switch fails
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    h->freeAll();
     delete h;
     return MV_OK;
 }
@@ -2778,8 +2774,7 @@ int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n
     if (w < 32 || h < 4 || w % 32 || h % 4 || w > kMaxRasterWidth || h > 4096) return MV_ERR_ARG;  // what mv_draw_hires accepts
     const bool fast = opts[0] != 0, wantSeg = opts[1] != 0;
     if ((opts[0] | opts[1]) & ~1 || (wantSeg && !seg)) return MV_ERR_ARG;
-    mv_engine tmp;  // the engine default of tri_cap; the palette upload
-    const int triCap = opts[2] ? opts[2] : tmp.triCap;
+    const int triCap = opts[2] ? opts[2] : kDefaultTriCap;
     if (triCap < 32 || triCap > mvr::kMaxTriCap) return MV_ERR_ARG;
     // row bands: opts[3] of them (the last one may be shorter), or 0 = the rule of mv_draw_hires (bands of about a hundred tiles)
     int bandRows;
@@ -2807,37 +2802,35 @@ int mv_debug_render_instances_ex(const float *view16, const float *inst18, int n
     }
     MvConsts k;
     fillConsts(k, w, h);
-    if (uploadPalette(&tmp) != MV_OK) return MV_ERR_CUDA;
+    if (uploadPalette() != cudaSuccess) return MV_ERR_CUDA;
     const ViewKernel fn = viewKernelOf(mvr::Items::All, wantSeg, fast);
-    MvInstance *dInst = nullptr; int32_t *dCnt = nullptr; float *dView = nullptr, *dDepth = nullptr; uint8_t *dObs = nullptr; uint16_t *dSeg = nullptr;
-    uint32_t *dCtr = nullptr; unsigned long long *dSpill = nullptr, *dStats = nullptr;
+    DevBuf<MvInstance> dInst; DevBuf<int32_t> dCnt; DevBuf<float> dView, dDepth; DevBuf<uint8_t> dObs; DevBuf<uint16_t> dSeg;
+    DevBuf<uint32_t> dCtr; DevBuf<unsigned long long> dSpill, dStats;
     const size_t px = size_t(w) * size_t(h);
     // the attribute is the device maximum, as configureRaster sets it: an engine alive in this process keeps launching with its own tri_cap
-    bool ok = cudaMalloc(&dInst, sizeof(MvInstance) * inst.size()) == cudaSuccess && cudaMalloc(&dCnt, 32) == cudaSuccess &&
-              cudaMalloc(&dView, 64) == cudaSuccess && cudaMalloc(&dObs, px * 4) == cudaSuccess && cudaMalloc(&dDepth, px * 4) == cudaSuccess &&
-              cudaMalloc(&dSeg, px * 2) == cudaSuccess && cudaMalloc(&dStats, 16 * sizeof(unsigned long long)) == cudaSuccess &&
-              cudaMalloc(&dCtr, 16) == cudaSuccess && cudaMalloc(&dSpill, sizeof(unsigned long long) * size_t(bands) * size_t(w) * bandRows) == cudaSuccess &&
+    bool ok = dInst.alloc(inst.size()) == cudaSuccess && dCnt.alloc(8) == cudaSuccess && dView.alloc(16) == cudaSuccess &&
+              dObs.alloc(px * 4) == cudaSuccess && dDepth.alloc(px) == cudaSuccess && dSeg.alloc(px) == cudaSuccess && dStats.alloc(16) == cudaSuccess &&
+              dCtr.alloc(4) == cudaSuccess && dSpill.alloc(size_t(bands) * size_t(w) * bandRows) == cudaSuccess &&
               cudaFuncSetAttribute(reinterpret_cast<const void *>(fn), cudaFuncAttributeMaxDynamicSharedMemorySize, maxOptin) == cudaSuccess;
     if (ok) {
-        cudaMemcpy(dInst, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice);
-        cudaMemcpy(dCnt, cnt, 32, cudaMemcpyHostToDevice);
-        cudaMemcpy(dView, view16, 64, cudaMemcpyHostToDevice);
-        cudaMemset(dCtr, 0, 16);
-        cudaMemset(dStats, 0, 16 * sizeof(unsigned long long));
-        mvr::ViewParams vp = frameParams(w, h, bands, bandRows, dSpill, triCap, k);
-        vp.instances = dInst; vp.instCounts = dCnt; vp.views = dView; vp.instStride = int(inst.size()); vp.obs = dObs; vp.depth = depth ? dDepth : nullptr;
-        vp.seg = wantSeg ? dSeg : nullptr; vp.stats = stats ? dStats : nullptr;
-        vp.workCounter = dCtr; vp.viewBase = 0; vp.N = 1; vp.A = 1;
+        cudaMemcpy(dInst.p, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice);
+        cudaMemcpy(dCnt.p, cnt, 32, cudaMemcpyHostToDevice);
+        cudaMemcpy(dView.p, view16, 64, cudaMemcpyHostToDevice);
+        cudaMemset(dCtr.p, 0, 16);
+        cudaMemset(dStats.p, 0, 16 * sizeof(unsigned long long));
+        mvr::ViewParams vp = frameParams(w, h, bands, bandRows, dSpill.p, triCap, k);
+        vp.instances = dInst.p; vp.instCounts = dCnt.p; vp.views = dView.p; vp.instStride = int(inst.size()); vp.obs = dObs.p; vp.depth = depth ? dDepth.p : nullptr;
+        vp.seg = wantSeg ? dSeg.p : nullptr; vp.stats = stats ? dStats.p : nullptr;
+        vp.workCounter = dCtr.p; vp.viewBase = 0; vp.N = 1; vp.A = 1;
         fn<<<bands, mvr::kThreads, smem>>>(vp);
         ok = cudaDeviceSynchronize() == cudaSuccess;
         if (ok) {
-            cudaMemcpy(rgba, dObs, px * 4, cudaMemcpyDeviceToHost);
-            if (depth) cudaMemcpy(depth, dDepth, px * 4, cudaMemcpyDeviceToHost);
-            if (wantSeg) cudaMemcpy(seg, dSeg, px * 2, cudaMemcpyDeviceToHost);
-            if (stats) cudaMemcpy(stats, dStats, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
+            cudaMemcpy(rgba, dObs.p, px * 4, cudaMemcpyDeviceToHost);
+            if (depth) cudaMemcpy(depth, dDepth.p, px * 4, cudaMemcpyDeviceToHost);
+            if (wantSeg) cudaMemcpy(seg, dSeg.p, px * 2, cudaMemcpyDeviceToHost);
+            if (stats) cudaMemcpy(stats, dStats.p, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
         }
     }
-    cudaFree(dCtr); cudaFree(dSpill); cudaFree(dInst); cudaFree(dCnt); cudaFree(dView); cudaFree(dObs); cudaFree(dDepth); cudaFree(dSeg); cudaFree(dStats);
     return ok ? MV_OK : MV_ERR_CUDA;
 }
 
@@ -2872,27 +2865,24 @@ int mv_debug_cast_rays(const float *views16, const float *inst18, const int32_t 
         }
     }
     const size_t nv = size_t(E) * size_t(A), nr = nv * size_t(R);
-    MvInstance *dInst = nullptr; int32_t *dCnt = nullptr; float *dViews = nullptr, *dDirs = nullptr, *dDist = nullptr; uint8_t *dMask = nullptr;
-    uint16_t *dTag = nullptr;
-    bool ok = cudaMalloc(&dInst, sizeof(MvInstance) * inst.size()) == cudaSuccess && cudaMalloc(&dCnt, sizeof(int32_t) * cnt.size()) == cudaSuccess &&
-              cudaMalloc(&dViews, nv * 64) == cudaSuccess && cudaMalloc(&dDirs, size_t(R) * 12) == cudaSuccess &&
-              cudaMalloc(&dDist, nr * 4) == cudaSuccess && cudaMalloc(&dTag, nr * 2) == cudaSuccess &&
-              (!env_mask || cudaMalloc(&dMask, size_t(E)) == cudaSuccess);
-    ok = ok && cudaMemcpy(dInst, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dCnt, cnt.data(), sizeof(int32_t) * cnt.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dViews, views16, nv * 64, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dDirs, dirs3, size_t(R) * 12, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dDist, dist, nr * 4, cudaMemcpyHostToDevice) == cudaSuccess && cudaMemcpy(dTag, tag, nr * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
-         (!env_mask || cudaMemcpy(dMask, env_mask, size_t(E), cudaMemcpyHostToDevice) == cudaSuccess);
+    DevBuf<MvInstance> dInst; DevBuf<int32_t> dCnt; DevBuf<float> dViews, dDirs, dDist; DevBuf<uint8_t> dMask; DevBuf<uint16_t> dTag;
+    bool ok = dInst.alloc(inst.size()) == cudaSuccess && dCnt.alloc(cnt.size()) == cudaSuccess && dViews.alloc(nv * 16) == cudaSuccess &&
+              dDirs.alloc(size_t(R) * 3) == cudaSuccess && dDist.alloc(nr) == cudaSuccess && dTag.alloc(nr) == cudaSuccess &&
+              (!env_mask || dMask.alloc(size_t(E)) == cudaSuccess);
+    ok = ok && cudaMemcpy(dInst.p, inst.data(), sizeof(MvInstance) * inst.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dCnt.p, cnt.data(), sizeof(int32_t) * cnt.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dViews.p, views16, nv * 64, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dDirs.p, dirs3, size_t(R) * 12, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dDist.p, dist, nr * 4, cudaMemcpyHostToDevice) == cudaSuccess && cudaMemcpy(dTag.p, tag, nr * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
+         (!env_mask || cudaMemcpy(dMask.p, env_mask, size_t(E), cudaMemcpyHostToDevice) == cudaSuccess);
     if (ok) {
         // the engine's launch (Engine::castRays), on the legacy stream
         mvray::RayParams rp;
-        rp.instances = dInst; rp.instCounts = dCnt; rp.views = dViews; rp.dirs = dDirs; rp.envMask = dMask;
-        rp.dist = dDist; rp.tag = dTag; rp.instStride = stride; rp.E = E; rp.A = A; rp.R = R; rp.maxDist = max_dist;
+        rp.instances = dInst.p; rp.instCounts = dCnt.p; rp.views = dViews.p; rp.dirs = dDirs.p; rp.envMask = dMask.p;
+        rp.dist = dDist.p; rp.tag = dTag.p; rp.instStride = stride; rp.E = E; rp.A = A; rp.R = R; rp.maxDist = max_dist;
         ok = mvray::castRays(rp, nullptr) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess &&
-             cudaMemcpy(dist, dDist, nr * 4, cudaMemcpyDeviceToHost) == cudaSuccess && cudaMemcpy(tag, dTag, nr * 2, cudaMemcpyDeviceToHost) == cudaSuccess;
+             cudaMemcpy(dist, dDist.p, nr * 4, cudaMemcpyDeviceToHost) == cudaSuccess && cudaMemcpy(tag, dTag.p, nr * 2, cudaMemcpyDeviceToHost) == cudaSuccess;
     }
-    cudaFree(dInst); cudaFree(dCnt); cudaFree(dViews); cudaFree(dDirs); cudaFree(dDist); cudaFree(dTag); cudaFree(dMask);
     return ok ? MV_OK : MV_ERR_CUDA;
 }
 
@@ -2931,31 +2921,28 @@ int mv_debug_kcc(const int32_t *hdr8, const float *boxes10, const float *agents3
             }
         }
     }
-    int32_t *dHdr = nullptr, *dOutI = nullptr; MvBox *dStatics = nullptr; MvObject *dObjects = nullptr;
-    float *dRot = nullptr, *dAgents = nullptr, *dQuery = nullptr, *dOutF = nullptr;
+    DevBuf<int32_t> dHdr, dOutI; DevBuf<MvBox> dStatics; DevBuf<MvObject> dObjects; DevBuf<float> dRot, dAgents, dQuery, dOutF;
     const size_t nA = size_t(n) * MV_MAX_AGENTS * 3;
-    bool ok = cudaMalloc(&dHdr, size_t(n) * 32) == cudaSuccess && cudaMalloc(&dStatics, statics.size() * sizeof(MvBox)) == cudaSuccess &&
-              cudaMalloc(&dRot, rot.size() * 4) == cudaSuccess && cudaMalloc(&dObjects, objects.size() * sizeof(MvObject)) == cudaSuccess &&
-              cudaMalloc(&dAgents, nA * 4) == cudaSuccess && cudaMalloc(&dQuery, size_t(n) * 80) == cudaSuccess &&
-              cudaMalloc(&dOutI, size_t(n) * 32) == cudaSuccess && cudaMalloc(&dOutF, size_t(n) * 64) == cudaSuccess;
-    ok = ok && cudaMemcpy(dHdr, hdr8, size_t(n) * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dStatics, statics.data(), statics.size() * sizeof(MvBox), cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dRot, rot.data(), rot.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dObjects, objects.data(), objects.size() * sizeof(MvObject), cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dAgents, agents3, nA * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dQuery, query20, size_t(n) * 80, cudaMemcpyHostToDevice) == cudaSuccess;
+    bool ok = dHdr.alloc(size_t(n) * 8) == cudaSuccess && dStatics.alloc(statics.size()) == cudaSuccess && dRot.alloc(rot.size()) == cudaSuccess &&
+              dObjects.alloc(objects.size()) == cudaSuccess && dAgents.alloc(nA) == cudaSuccess && dQuery.alloc(size_t(n) * 20) == cudaSuccess &&
+              dOutI.alloc(size_t(n) * 8) == cudaSuccess && dOutF.alloc(size_t(n) * 16) == cudaSuccess;
+    ok = ok && cudaMemcpy(dHdr.p, hdr8, size_t(n) * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dStatics.p, statics.data(), statics.size() * sizeof(MvBox), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dRot.p, rot.data(), rot.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dObjects.p, objects.data(), objects.size() * sizeof(MvObject), cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dAgents.p, agents3, nA * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(dQuery.p, query20, size_t(n) * 80, cudaMemcpyHostToDevice) == cudaSuccess;
     if (ok) {
         mvk::KccCaseParams kp;
-        kp.hdr = dHdr; kp.statics = dStatics; kp.staticRot = dRot; kp.objects = dObjects; kp.agentPos = dAgents; kp.query = dQuery;
-        kp.outI = dOutI; kp.outF = dOutF;
+        kp.hdr = dHdr.p; kp.statics = dStatics.p; kp.staticRot = dRot.p; kp.objects = dObjects.p; kp.agentPos = dAgents.p; kp.query = dQuery.p;
+        kp.outI = dOutI.p; kp.outF = dOutF.p;
         const int smem = int(sizeof(mvk::WarpShared));
         ok = cudaFuncSetAttribute(mvk::kccCaseKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess;
         if (ok) mvk::kccCaseKernel<<<n, 32, smem>>>(kp);
         ok = ok && cudaGetLastError() == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess &&
-             cudaMemcpy(out_i8, dOutI, size_t(n) * 32, cudaMemcpyDeviceToHost) == cudaSuccess &&
-             cudaMemcpy(out_f16, dOutF, size_t(n) * 64, cudaMemcpyDeviceToHost) == cudaSuccess;
+             cudaMemcpy(out_i8, dOutI.p, size_t(n) * 32, cudaMemcpyDeviceToHost) == cudaSuccess &&
+             cudaMemcpy(out_f16, dOutF.p, size_t(n) * 64, cudaMemcpyDeviceToHost) == cudaSuccess;
     }
-    cudaFree(dHdr); cudaFree(dStatics); cudaFree(dRot); cudaFree(dObjects); cudaFree(dAgents); cudaFree(dQuery); cudaFree(dOutI); cudaFree(dOutF);
     return ok ? MV_OK : MV_ERR_CUDA;
 }
 
