@@ -173,6 +173,96 @@ private:
 using CudaEvent = CudaHandle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
 using CudaStream = CudaHandle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
 
+// an array of `rows` rows re-laid from a pitch of `from` elements to one of `to`: alloc() the new array, then apply() copies every row
+// into it and moves it in.  A change allocates all of its arrays before it applies any, so that a failed allocation changes nothing
+template <typename T, bool Pinned> struct Repitch {
+    CudaBuf<T, Pinned> *buf; size_t rows, from, to; CudaBuf<T, Pinned> next{};
+    bool alloc() { return next.alloc(rows * to) == cudaSuccess; }
+    cudaError_t apply() {
+        const cudaError_t err = cudaMemcpy2D(next.p, sizeof(T) * to, buf->p, sizeof(T) * from, sizeof(T) * from, rows, Pinned ? cudaMemcpyHostToHost : cudaMemcpyDeviceToDevice);
+        if (err == cudaSuccess) *buf = std::move(next);
+        return err;
+    }
+};
+
+// The level arrays: rows in HBM with pinned mirrors, which the level workers write and the uploads, debug dumps and state stores read.  A
+// row holds one MvLevel, staticCap static boxes and their 2 * staticCap rotation floats, decoCap decorations, and the solid, exit and lava
+// bit planes of gridWords words each, of which its level uses levelWords[row].  Which env's level a row holds is the engine's to say.
+struct LevelTable {
+    int staticCap = MV_INITIAL_STATIC_CAP, decoCap = 0, gridWords = 0;  // the pitches; staticCap grows (growStatics)
+    DevBuf<MvLevel> d_levels; DevBuf<MvBox> d_statics; DevBuf<float> d_staticRot; DevBuf<MvDeco> d_deco; DevBuf<uint32_t> d_solid;
+    // `n` rows at the current pitches, on the device and pinned; a failure leaves every array empty
+    bool alloc(size_t n) {
+        const size_t cap = size_t(staticCap), deco = size_t(decoCap), w = size_t(gridWords) * 3;
+        levelWords.assign(n, 0);
+        if (d_levels.alloc(n) == cudaSuccess && d_statics.alloc(n * cap) == cudaSuccess && d_staticRot.alloc(n * cap * 2) == cudaSuccess &&
+            d_deco.alloc(n * deco) == cudaSuccess && d_solid.alloc(n * w) == cudaSuccess && h_levels.alloc(n) == cudaSuccess &&
+            h_statics.alloc(n * cap) == cudaSuccess && h_staticRot.alloc(n * cap * 2) == cudaSuccess && h_deco.alloc(n * deco) == cudaSuccess &&
+            h_solid.alloc(n * w) == cudaSuccess)
+            return true;
+        d_levels.free(); d_statics.free(); d_staticRot.free(); d_deco.free(); d_solid.free();
+        h_levels.free(); h_statics.free(); h_staticRot.free(); h_deco.free(); h_solid.free();
+        return false;
+    }
+    // a level of at most staticCap static boxes into row r's mirrors, not uploaded.  Level workers write rows concurrently, never one row
+    void write(size_t r, const mv::LevelOut &out) {
+        std::memcpy(&h_levels.p[r], &out.level, sizeof(MvLevel));
+        std::copy(out.statics.begin(), out.statics.end(), h_statics.p + r * size_t(staticCap));
+        std::copy(out.staticRot.begin(), out.staticRot.end(), h_staticRot.p + r * size_t(staticCap) * 2);
+        std::copy(out.deco.begin(), out.deco.end(), h_deco.p + r * size_t(decoCap));
+        const size_t nw = std::min(out.solid.size(), size_t(gridWords));
+        const std::vector<uint32_t> *planes[3] = {&out.solid, &out.exitBits, &out.lavaBits};
+        for (int k = 0; k < 3; ++k) std::copy_n(planes[k]->begin(), nw, h_solid.p + (r * 3 + size_t(k)) * size_t(gridWords));
+        levelWords[r] = int(nw);
+    }
+    // row r's mirrors as a level that write() puts back as it was (without the draw sequence, which only the generator reads)
+    mv::LevelOut read(size_t r) const {
+        const MvLevel &L = h_levels.p[r];
+        const size_t ns = size_t(L.n_static), nd = size_t(std::max(0, L.n_deco)), nw = size_t(levelWords[r]);
+        return {L, {statics(r), statics(r) + ns}, {rotations(r), rotations(r) + 2 * ns}, {deco(r), deco(r) + nd}, {},
+                {plane(r, 0), plane(r, 0) + nw}, {plane(r, 1), plane(r, 1) + nw}, {plane(r, 2), plane(r, 2) + nw}};
+    }
+    // row r's mirrors into HBM on stream s: the level, its boxes and decorations, the words its planes use (Tower, Rearrange: one plane)
+    cudaError_t upload(size_t r, cudaStream_t s) const {
+        cudaError_t err = cudaSuccess;
+        auto up = [&](void *dst, const void *src, size_t bytes) { if (err == cudaSuccess) err = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s); };
+        const MvLevel &L = h_levels.p[r];
+        up(&d_levels.p[r], &L, sizeof(MvLevel));
+        if (L.n_static) {
+            up(d_statics.p + r * size_t(staticCap), statics(r), sizeof(MvBox) * size_t(L.n_static));
+            up(d_staticRot.p + r * size_t(staticCap) * 2, rotations(r), sizeof(float) * 2 * size_t(L.n_static));
+        }
+        if (L.n_deco > 0) up(d_deco.p + r * size_t(decoCap), deco(r), sizeof(MvDeco) * size_t(L.n_deco));
+        const int planes = (L.scenario == MV_SCENARIO_TOWER || L.scenario == MV_SCENARIO_REARRANGE) ? 1 : 3;
+        for (int k = 0; k < planes; ++k) up(d_solid.p + (r * 3 + size_t(k)) * size_t(gridWords), plane(r, k), sizeof(uint32_t) * size_t(levelWords[r]));
+        return err;
+    }
+    // the static boxes and rotations at a pitch of `cap` boxes, device and pinned; no change unless every new array is allocated (else
+    // cudaErrorMemoryAllocation) and filled
+    cudaError_t growStatics(int cap) {
+        const size_t rows = d_levels.n, was = size_t(staticCap), to = size_t(cap);
+        Repitch<MvBox, false> d{&d_statics, rows, was, to};
+        Repitch<float, false> dRot{&d_staticRot, rows, was * 2, to * 2};
+        Repitch<MvBox, true> h{&h_statics, rows, was, to};
+        Repitch<float, true> hRot{&h_staticRot, rows, was * 2, to * 2};
+        if (!d.alloc() || !dRot.alloc() || !h.alloc() || !hRot.alloc()) return cudaErrorMemoryAllocation;
+        cudaError_t err;
+        if ((err = d.apply()) || (err = dRot.apply()) || (err = h.apply()) || (err = hRot.apply())) return err;
+        staticCap = cap;
+        return cudaSuccess;
+    }
+    // row views of the mirrors
+    const MvLevel &level(size_t r) const { return h_levels.p[r]; }
+    const MvBox *statics(size_t r) const { return h_statics.p + r * size_t(staticCap); }
+    const float *rotations(size_t r) const { return h_staticRot.p + r * size_t(staticCap) * 2; }
+    const MvDeco *deco(size_t r) const { return h_deco.p + r * size_t(decoCap); }
+    const uint32_t *plane(size_t r, int k) const { return h_solid.p + (r * 3 + size_t(k)) * size_t(gridWords); }  // 0 solid, 1 exit, 2 lava
+
+private:
+    PinBuf<MvLevel> h_levels; PinBuf<MvBox> h_statics; PinBuf<float> h_staticRot; PinBuf<MvDeco> h_deco; PinBuf<uint32_t> h_solid;
+    std::vector<int> levelWords;  // [rows] words of each bit plane the row's level uses
+};
+
 // one per-env device array as the state store sees it: `units` rows per env (the slot count for the arrays that hold the level slots, none
 // of them with a level set) of unitBytes
 struct EnvSlab {
@@ -181,8 +271,7 @@ struct EnvSlab {
     size_t unitBytes;
     size_t rowBytes() const { return size_t(units) * unitBytes; }
 };
-// indices into mv_engine::envSlabs() of the arrays that growStatics re-pitches
-enum { kSlabInst = 4, kSlabStatics = 8, kSlabStaticRot = 9, kSlabCount = 17 };
+constexpr int kSlabCount = 17;  // mv_engine::envSlabs()
 
 // saved env states (mv_states_*): every per-env device row in arrays of `rows` rows with the engine's pitch, plus the host state
 struct StateStore {
@@ -195,13 +284,7 @@ struct StateStore {
         std::string scenario;                   // the saved env's scenario name: only an env of the same name may load the row
         int bankRow = -1, bankSeed = 0;         // level set: the bank row the env was on and the seed of the level it held then
         int slot = 0, episode = 0;
-        // the host mirrors of every level slot that the debug dumps and the uploads read, one entry per slot (option "level_slots")
-        std::vector<int> words;
-        std::vector<MvLevel> level;
-        std::vector<std::vector<MvBox>> statics;
-        std::vector<std::vector<float>> staticRot;
-        std::vector<std::vector<MvDeco>> deco;
-        std::vector<std::vector<uint32_t>> solid;  // the three bit planes, levelWords words each
+        std::vector<mv::LevelOut> levels;       // the level table's rows of the env's slots (option "level_slots"); none with a level set
     };
     std::vector<HostRow> host;
 };
@@ -276,7 +359,7 @@ struct mv_engine {
     std::unique_ptr<WorkerPool> pool;
 
     // pitch of the per-env grid arrays: the largest dense-grid capacity among the engine's scenarios (one pitch for all envs)
-    int gridCells = 0, gridWords = 0;
+    int gridCells = 0;
     int triCap = kDefaultTriCap;
     std::atomic<int> maxObjSeen{0};
     bool wantDepth = false, obsToHost = true, didReset = false, fastShading = true;
@@ -353,11 +436,7 @@ struct mv_engine {
     size_t rowOfSlot(int e, int slot) const { return levelSet ? size_t(slot) : size_t(e) * size_t(levelSlots) + size_t(slot); }
     // ... and the row of env e's live level as of the last retired call
     size_t liveRow(int e) const { return levelSet ? size_t(envBank[size_t(e)]) * size_t(levelSet) + size_t(h_levelIds.p[e]) : rowOfSlot(e, hostSlot[size_t(e)]); }
-    DevBuf<MvLevel> d_levels;      // [E][D]
-    DevBuf<MvBox> d_statics;       // [E][D][staticCap]
-    DevBuf<float> d_staticRot;     // [E][D][staticCap][2]
-    int staticCap = MV_INITIAL_STATIC_CAP;  // grows when a generated level has more static boxes (growStatics)
-    DevBuf<uint32_t> d_solid;
+    LevelTable levels;             // [E][D] level slots, or the bank's rows; its static-box pitch grows with the levels (growStatics)
     DevBuf<uint8_t> d_objGrid;
     DevBuf<MvEnvState> d_envs;
     DevBuf<MvAgent> d_agents;
@@ -405,17 +484,11 @@ struct mv_engine {
         PinBuf<uint32_t> h_range;
     } cams;
     int cameraGrid = 0;  // persistent grid of the camera variants
-    DevBuf<MvDeco> d_deco;         // [E][D][decoCap]
-    PinBuf<MvDeco> h_deco;
-    int decoCap = 1, instCap = MV_DYN_INSTANCES + MV_INITIAL_STATIC_CAP + 1;
+    // pitch of the instance rows: the dynamic instances and every static box and decoration a level row can hold
+    int instCap() const { return MV_DYN_INSTANCES + levels.staticCap + levels.decoCap; }
 
-    PinBuf<MvLevel> h_levels;      // [E][D] staging mirror
-    PinBuf<MvBox> h_statics;       // [E][D][staticCap]
-    PinBuf<float> h_staticRot;
     // levels with more static boxes than the arrays hold: parked here by the workers until flushUploads has grown the arrays
     std::vector<std::pair<int, mv::LevelOut>> oversize;
-    int wantStaticCap = 0;
-    PinBuf<uint32_t> h_solid;      // [E][D][3][gridWords]
     PinBuf<int32_t> h_actions;
     PinBuf<float> h_rtable;
     PinBuf<float> h_rewards;
@@ -440,7 +513,6 @@ struct mv_engine {
     uint64_t asyncSteps = 0;
 
     std::vector<int> hostSlot, hostEpisode;   // mirrors of the device's live slot / episode index
-    std::vector<int> levelWords;              // [E*D] words of the bit planes a staged level uses
     std::vector<int> pendingUpload;           // level ids (env * D + slot) whose freshly generated level waits for H2D
     // an env's levels come from one stateful generator (RNG stream, Sokoban's unplayed levels): its jobs run one after another, in the order
     // they were scheduled, on whichever worker drains the env's queue
@@ -529,7 +601,7 @@ struct mv_engine {
         rp.views = terminal ? d_termViews.p : d_views.p;
         rp.dirs = d_rayDirs.p; rp.envMask = terminal ? d_dones.p : mask;
         rp.dist = d_rayDist.p + (terminal ? rayCount() : 0); rp.tag = d_rayTag.p + (terminal ? rayCount() : 0);
-        rp.instStride = instCap; rp.E = E; rp.A = A; rp.R = nRays; rp.maxDist = rayMaxDist;
+        rp.instStride = instCap(); rp.E = E; rp.A = A; rp.R = nRays; rp.maxDist = rayMaxDist;
         MV_CUDA(mvray::castRays(rp, stream));
         launches += 1;
         return MV_OK;
@@ -604,91 +676,51 @@ struct mv_engine {
     void generateInto(mv::LevelGenerator &gen, int sc, int id, int serial) {
         mv::LevelOut out;
         if (!generateOut(gen, sc, serial, out)) return;
-        if (int(out.statics.size()) > staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
+        if (int(out.statics.size()) > levels.staticCap) {  // the arrays are grown on the caller's thread (flushUploads), then the level goes in
             std::lock_guard<std::mutex> lk(genMutex);
-            wantStaticCap = std::max(wantStaticCap, int(out.statics.size()));
             oversize.emplace_back(id, std::move(out));
             return;
         }
         stageLevel(id, out);
     }
-    // worker thread (or flushUploads for parked levels): copy a generated level into the pinned staging mirrors and queue its upload
+    // worker thread (or flushUploads for parked levels): a generated level into its row's mirrors, and its upload queued
     void stageLevel(int id, const mv::LevelOut &out) {
-        {
-            std::memcpy(&h_levels.p[size_t(id)], &out.level, sizeof(MvLevel));
-            if (!out.statics.empty()) {
-                std::memcpy(h_statics.p + size_t(id) * size_t(staticCap), out.statics.data(), sizeof(MvBox) * out.statics.size());
-                std::memcpy(h_staticRot.p + size_t(id) * size_t(staticCap) * 2, out.staticRot.data(), sizeof(float) * out.staticRot.size());
-            }
-            if (!out.deco.empty()) std::memcpy(&h_deco.p[size_t(id) * size_t(decoCap)], out.deco.data(), sizeof(MvDeco) * out.deco.size());
-            uint32_t *dst = h_solid.p + size_t(id) * 3 * gridWords;  // planes: solid, exit, lava
-            const size_t nw = std::min(out.solid.size(), size_t(gridWords));
-            std::memcpy(dst, out.solid.data(), sizeof(uint32_t) * nw);
-            std::memcpy(dst + gridWords, out.exitBits.data(), sizeof(uint32_t) * nw);
-            std::memcpy(dst + 2 * size_t(gridWords), out.lavaBits.data(), sizeof(uint32_t) * nw);
-            levelWords[size_t(id)] = int(nw);
-            std::lock_guard<std::mutex> lk(genMutex);
-            pendingUpload.push_back(id);
-        }
+        levels.write(size_t(id), out);
+        std::lock_guard<std::mutex> lk(genMutex);
+        pendingUpload.push_back(id);
     }
-    // (re)allocate the level arrays ([E][D] slots, or the rows of a level set), on the device and pinned: levels, static boxes and their rotations (staticCap per level),
-    // decorations and the three bit planes; and the instance rows, whose pitch staticCap sets as well
+    // (re)allocate the level table ([E][D] slots, or the rows of a level set) and the instance rows, whose pitch depends on the table's
     int allocLevelSlots(const char *what) {
-        const size_t rows = levelRows(), cap = size_t(staticCap), deco = size_t(decoCap), words = size_t(gridWords) * 3;
-        levelWords.assign(rows, 0);
-        instCap = MV_DYN_INSTANCES + staticCap + decoCap;
-        if (d_levels.alloc(rows) != cudaSuccess || d_statics.alloc(rows * cap) != cudaSuccess || d_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
-            d_deco.alloc(rows * deco) != cudaSuccess || d_solid.alloc(rows * words) != cudaSuccess || d_inst.alloc(size_t(E) * size_t(instCap)) != cudaSuccess ||
-            h_levels.alloc(rows) != cudaSuccess || h_statics.alloc(rows * cap) != cudaSuccess || h_staticRot.alloc(rows * cap * 2) != cudaSuccess ||
-            h_deco.alloc(rows * deco) != cudaSuccess || h_solid.alloc(rows * words) != cudaSuccess) {
+        if (!levels.alloc(levelRows()) || d_inst.alloc(size_t(E) * size_t(instCap())) != cudaSuccess) {
             setError(std::string(what) + ": allocation failed");
             return MV_ERR_CUDA;
         }
         return MV_OK;
     }
-    // more static boxes per level: re-pitch every array that is laid out by staticCap (level statics, instance lists), device and host
+    // more static boxes per level: re-pitch every array that is laid out by the static-box pitch (level statics, instance lists)
     int growStatics(int need) {
-        const int newCap = std::max(staticCap * 2, ((need + 255) / 256) * 256);
-        const int newInstCap = MV_DYN_INSTANCES + newCap + decoCap;
+        const int newCap = std::max(levels.staticCap * 2, ((need + 255) / 256) * 256);
+        const int newInstCap = MV_DYN_INSTANCES + newCap + levels.decoCap;
         if (newInstCap > mvr::kMaxInstancesPerEnv) { setError("a level needs more drawables than the draw-order key can number"); return MV_ERR_CAPACITY; }
         MV_CUDA(cudaStreamSynchronize(stream));
-        DevBuf<MvBox> nStat; DevBuf<float> nRot; DevBuf<MvInstance> nInst; PinBuf<MvBox> hStat; PinBuf<float> hRot;
-        const size_t rows = levelRows();
-        // the state stores keep the engine's pitch: their copies of the same three arrays are re-pitched alongside (with a level set a
-        // store holds no level, only the instance rows; a replacement can grow the arrays after stores exist)
-        struct Repitch { DevBuf<uint8_t> *buf; DevBuf<uint8_t> next; size_t rows, oldPitch, newPitch; };
-        std::vector<Repitch> storeGrow;
-        for (auto &st : stores) {
-            if (!st) continue;
-            const size_t r = size_t(st->rows);
-            if (!levelSet) {
-                storeGrow.push_back({&st->slabs[kSlabStatics], {}, r * levelSlots, sizeof(MvBox) * staticCap, sizeof(MvBox) * newCap});
-                storeGrow.push_back({&st->slabs[kSlabStaticRot], {}, r * levelSlots, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * newCap});
-            }
-            storeGrow.push_back({&st->slabs[kSlabInst], {}, r, sizeof(MvInstance) * instCap, sizeof(MvInstance) * newInstCap});
-        }
-        bool storesOk = true;
-        for (auto &g : storeGrow) storesOk = storesOk && g.next.alloc(g.rows * g.newPitch) == cudaSuccess;
-        if (!storesOk || nStat.alloc(rows * newCap) != cudaSuccess || nRot.alloc(rows * newCap * 2) != cudaSuccess || nInst.alloc(size_t(E) * newInstCap) != cudaSuccess ||
-            hStat.alloc(rows * newCap) != cudaSuccess || hRot.alloc(rows * newCap * 2) != cudaSuccess) {
-            setError("growing the static-box arrays: allocation failed");
-            return MV_ERR_CUDA;
-        }
-        for (auto &g : storeGrow) {
-            MV_CUDA(cudaMemcpy2D(g.next.p, g.newPitch, g.buf->p, g.oldPitch, g.oldPitch, g.rows, cudaMemcpyDeviceToDevice));
-            *g.buf = std::move(g.next);
-        }
-        MV_CUDA(cudaMemcpy2D(nStat.p, sizeof(MvBox) * newCap, d_statics.p, sizeof(MvBox) * staticCap, sizeof(MvBox) * staticCap, rows, cudaMemcpyDeviceToDevice));
-        MV_CUDA(cudaMemcpy2D(nRot.p, sizeof(float) * 2 * newCap, d_staticRot.p, sizeof(float) * 2 * staticCap, sizeof(float) * 2 * staticCap, rows, cudaMemcpyDeviceToDevice));
-        MV_CUDA(cudaMemcpy2D(nInst.p, sizeof(MvInstance) * newInstCap, d_inst.p, sizeof(MvInstance) * instCap, sizeof(MvInstance) * instCap, size_t(E), cudaMemcpyDeviceToDevice));
-        for (size_t r = 0; r < rows; ++r) {
-            std::memcpy(hStat.p + r * newCap, h_statics.p + r * staticCap, sizeof(MvBox) * staticCap);
-            std::memcpy(hRot.p + r * newCap * 2, h_staticRot.p + r * staticCap * 2, sizeof(float) * 2 * staticCap);
-        }
-        d_statics = std::move(nStat); d_staticRot = std::move(nRot); d_inst = std::move(nInst); h_statics = std::move(hStat); h_staticRot = std::move(hRot);
-        staticCap = newCap; instCap = newInstCap;
+        // the state stores keep the engine's pitch: every store slab whose unit grows is re-pitched alongside, over store rows x units rows
+        Repitch<MvInstance, false> inst{&d_inst, size_t(E), size_t(instCap()), size_t(newInstCap)};
+        std::vector<Repitch<uint8_t, false>> storeGrow;
+        const auto was = envSlabs(), will = envSlabs(newCap, newInstCap);
+        for (auto &st : stores)
+            for (int k = 0; st && k < kSlabCount; ++k)
+                if (will[size_t(k)].rowBytes() != was[size_t(k)].rowBytes())
+                    storeGrow.push_back({&st->slabs[k], size_t(st->rows) * size_t(was[size_t(k)].units), was[size_t(k)].unitBytes, will[size_t(k)].unitBytes});
+        bool ok = inst.alloc();
+        for (auto &g : storeGrow) ok = ok && g.alloc();
+        // the level table last: it changes only once its own arrays are allocated, and then every allocation has succeeded
+        const cudaError_t err = ok ? levels.growStatics(newCap) : cudaErrorMemoryAllocation;
+        if (err == cudaErrorMemoryAllocation) { setError("growing the static-box arrays: allocation failed"); return MV_ERR_CUDA; }
+        MV_CUDA(err);
+        MV_CUDA(inst.apply());
+        for (auto &g : storeGrow) MV_CUDA(g.apply());
         if (d_termInst.p) {  // no copy: a terminal row is written whole before the launch that reads it
-            if (d_termInst.alloc(size_t(E) * size_t(instCap)) != cudaSuccess) { setError("growing the terminal instance rows: allocation failed"); return MV_ERR_CUDA; }
+            if (d_termInst.alloc(size_t(E) * size_t(newInstCap)) != cudaSuccess) { setError("growing the terminal instance rows: allocation failed"); return MV_ERR_CUDA; }
         }
         return MV_OK;
     }
@@ -701,29 +733,18 @@ struct mv_engine {
             if (!genErrors.empty()) { setError("level generation failed: " + genErrors.front()); return MV_ERR_CAPACITY; }
         }
         if (!oversize.empty()) {  // workers are idle (waitAll above): grow, then stage what they parked
-            const int rc = growStatics(wantStaticCap);
+            int need = 0;
+            for (auto &po : oversize) need = std::max(need, int(po.second.statics.size()));
+            const int rc = growStatics(need);
             if (rc) return rc;
             for (auto &po : oversize) stageLevel(po.first, po.second);
             oversize.clear();
-            wantStaticCap = 0;
         }
         {
             std::lock_guard<std::mutex> lk(genMutex);
             todo.swap(pendingUpload);
         }
-        for (int id : todo) {
-            MV_CUDA(cudaMemcpyAsync(&d_levels.p[id], &h_levels.p[id], sizeof(MvLevel), cudaMemcpyHostToDevice, stream));
-            if (const int nst = h_levels.p[id].n_static) {
-                MV_CUDA(cudaMemcpyAsync(d_statics.p + size_t(id) * size_t(staticCap), h_statics.p + size_t(id) * size_t(staticCap), sizeof(MvBox) * size_t(nst), cudaMemcpyHostToDevice, stream));
-                MV_CUDA(cudaMemcpyAsync(d_staticRot.p + size_t(id) * size_t(staticCap) * 2, h_staticRot.p + size_t(id) * size_t(staticCap) * 2, sizeof(float) * 2 * size_t(nst), cudaMemcpyHostToDevice, stream));
-            }
-            if (h_levels.p[id].n_deco > 0)
-                MV_CUDA(cudaMemcpyAsync(&d_deco.p[size_t(id) * size_t(decoCap)], &h_deco.p[size_t(id) * size_t(decoCap)], sizeof(MvDeco) * size_t(h_levels.p[id].n_deco), cudaMemcpyHostToDevice, stream));
-            const size_t nw = size_t(levelWords[size_t(id)]);  // only the words this level's grid uses
-            const int sc = h_levels.p[id].scenario;
-            for (int plane = 0; plane < ((sc == MV_SCENARIO_TOWER || sc == MV_SCENARIO_REARRANGE) ? 1 : 3); ++plane)
-                MV_CUDA(cudaMemcpyAsync(d_solid.p + (size_t(id) * 3 + plane) * gridWords, h_solid.p + (size_t(id) * 3 + plane) * gridWords, sizeof(uint32_t) * nw, cudaMemcpyHostToDevice, stream));
-        }
+        for (int id : todo) MV_CUDA(levels.upload(size_t(id), stream));
         return MV_OK;
     }
 
@@ -743,11 +764,12 @@ struct mv_engine {
         sp.hostRewards = mirror ? mirror->rewards.p : nullptr; sp.hostTrueObjectives = mirror ? mirror->trueObj.p : nullptr;
         sp.hostDones = mirror ? mirror->dones.p : nullptr;
         sp.hostFaults = h_faultWord.p;
-        sp.levels = d_levels.p; sp.statics = d_statics.p; sp.staticRot = d_staticRot.p; sp.staticCap = staticCap; sp.solid = d_solid.p; sp.objGrid = d_objGrid.p; sp.envs = d_envs.p; sp.agents = d_agents.p;
+        sp.levels = levels.d_levels.p; sp.statics = levels.d_statics.p; sp.staticRot = levels.d_staticRot.p; sp.staticCap = levels.staticCap; sp.solid = levels.d_solid.p;
+        sp.objGrid = d_objGrid.p; sp.envs = d_envs.p; sp.agents = d_agents.p;
         sp.objects = d_objects.p; sp.instances = d_inst.p; sp.instCounts = d_instCounts.p; sp.views = d_views.p;
         sp.actions = dActions; sp.rtable = d_rtable.p; sp.rewards = d_rewards.p; sp.dones = d_dones.p; sp.trueObjectives = d_trueObj.p;
         sp.prof = d_prof.p;
-        sp.deco = d_deco.p; sp.decoCap = decoCap; sp.instStride = instCap;
+        sp.deco = levels.d_deco.p; sp.decoCap = levels.decoCap; sp.instStride = instCap();
         sp.ready = d_ready.p; sp.readyStamp = ++readyStamp;
         sp.envOrder = rasterSched ? d_viewCost.p + costItems() : nullptr;  // a permutation at all times (identity until a cost-ordered raster launch has sorted it)
         sp.ends = dEnds;
@@ -763,7 +785,7 @@ struct mv_engine {
         sp.termStAgents = stateTensor(termSt, 0, true); sp.termStEnvs = stateTensor(termSt, 1, true); sp.termStObjects = stateTensor(termSt, 2, true);
         sp.termStRewards = stateTensor(termSt, 3, true);
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
-        sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = gridWords; sp.forceReset = forceReset ? 1 : 0;
+        sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = levels.gridWords; sp.forceReset = forceReset ? 1 : 0;
         sp.k = consts;
         return sp;
     }
@@ -836,7 +858,7 @@ struct mv_engine {
     // between the step kernel and its programmatic dependent).  Every engine launch reads instance lists at the engine's pitch.
     int launchView(mvr::ViewParams &vp, bool dependent, mvr::Items items = mvr::Items::All) {
         const int grid = rasterGridFor(vp);
-        vp.A = A; vp.instStride = instCap;
+        vp.A = A; vp.instStride = instCap();
         vp.workCounter = d_workCounter.p; vp.counterBase = counterBase;
         counterBase += uint32_t(vp.N) * uint32_t(vp.bands) + uint32_t(grid);
         cudaLaunchConfig_t cfg = {};
@@ -1005,13 +1027,13 @@ struct mv_engine {
     // about y), decorations (a unit mesh's reach along each column, the capsule's y doubled) and terrain slabs
     void levelBounds(int e, float *out6) const {
         const size_t row = liveRow(e);
-        const MvLevel &L = h_levels.p[row];
+        const MvLevel &L = levels.level(row);
         float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
         auto add = [&](const float c[3], const float r[3]) {
             for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], c[a] - r[a]); hi[a] = std::max(hi[a], c[a] + r[a]); }
         };
-        const MvBox *st = h_statics.p + row * size_t(staticCap);
-        const float *rot = h_staticRot.p + row * size_t(staticCap) * 2;
+        const MvBox *st = levels.statics(row);
+        const float *rot = levels.rotations(row);
         for (int i = 0; i < L.n_static; ++i) {
             float r[3] = {st[i].h[0], st[i].h[1], st[i].h[2]};
             if (st[i].flags & MV_ROTATED) {
@@ -1021,7 +1043,7 @@ struct mv_engine {
             }
             add(st[i].c, r);
         }
-        const MvDeco *dc = h_deco.p + row * size_t(decoCap);
+        const MvDeco *dc = levels.deco(row);
         for (int i = 0; i < L.n_deco; ++i) {
             const float *m = dc[i].model;
             const float ys = dc[i].mesh == 1 ? 2.0f : 1.0f;
@@ -1255,19 +1277,20 @@ struct mv_engine {
     }
 
     // ------------------------------------------------------------------ state stores (mv_states_*)
-    // every per-env device row, in the order of StateStore::slabs
-    std::array<EnvSlab, kSlabCount> envSlabs() {
+    // every per-env device row, in the order of StateStore::slabs, at the engine's pitches or, for growStatics, at the grown ones
+    std::array<EnvSlab, kSlabCount> envSlabs() { return envSlabs(levels.staticCap, instCap()); }
+    std::array<EnvSlab, kSlabCount> envSlabs(int staticPitch, int instPitch) {
         auto s = [](void *p, int units, size_t bytes) { return EnvSlab{static_cast<uint8_t *>(p), units, bytes}; };
         // with a level set a row holds no level: the bank is shared and immutable, MvEnvState names the row.  The levels' place in the
         // list is taken by the env's level id, so that a loaded env reports its level before it is stepped again
         const int D = levelSet ? 0 : levelSlots;
-        const EnvSlab levelsOrId = levelSet ? s(d_levelIds.p, 1, sizeof(int32_t)) : s(d_levels.p, D, sizeof(MvLevel));
+        const EnvSlab levelsOrId = levelSet ? s(d_levelIds.p, 1, sizeof(int32_t)) : s(levels.d_levels.p, D, sizeof(MvLevel));
         return {{s(d_envs.p, 1, sizeof(MvEnvState)), s(d_agents.p, 1, sizeof(MvAgent) * A), s(d_objects.p, 1, sizeof(MvObject) * MV_MAX_OBJECTS),
-                 s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instCap), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
-                 s(d_views.p, 1, sizeof(float) * 16 * A), levelsOrId, s(d_statics.p, D, sizeof(MvBox) * staticCap),
-                 s(d_staticRot.p, D, sizeof(float) * 2 * staticCap), s(d_deco.p, D, sizeof(MvDeco) * decoCap), s(d_solid.p, D, sizeof(uint32_t) * 3 * gridWords),
-                 s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1), s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t)),
-                 s(d_doneReasons.p, 1, 1)}};
+                 s(d_objGrid.p, 1, size_t(gridCells)), s(d_inst.p, 1, sizeof(MvInstance) * instPitch), s(d_instCounts.p, 1, sizeof(int32_t) * 8),
+                 s(d_views.p, 1, sizeof(float) * 16 * A), levelsOrId, s(levels.d_statics.p, D, sizeof(MvBox) * staticPitch),
+                 s(levels.d_staticRot.p, D, sizeof(float) * 2 * staticPitch), s(levels.d_deco.p, D, sizeof(MvDeco) * levels.decoCap),
+                 s(levels.d_solid.p, D, sizeof(uint32_t) * 3 * levels.gridWords), s(d_rewards.p, 1, sizeof(float) * A), s(d_dones.p, 1, 1),
+                 s(d_trueObj.p, 1, sizeof(float) * A), s(d_faults.p, 1, sizeof(int32_t)), s(d_doneReasons.p, 1, 1)}};
     }
     size_t stateRowBytes() {
         size_t b = 0;
@@ -1360,22 +1383,8 @@ struct mv_engine {
                 continue;
             }
             r.gen = gens[size_t(e)];
-            const size_t D = size_t(levelSlots);
-            r.words.resize(D); r.level.resize(D); r.statics.resize(D); r.staticRot.resize(D); r.deco.resize(D); r.solid.resize(D);
-            for (size_t s = 0; s < D; ++s) {
-                const size_t id = size_t(e) * D + s;
-                const MvLevel &L = h_levels.p[id];
-                r.level[s] = L;
-                r.words[s] = levelWords[id];
-                r.statics[s].assign(h_statics.p + id * staticCap, h_statics.p + id * staticCap + L.n_static);
-                r.staticRot[s].assign(h_staticRot.p + id * staticCap * 2, h_staticRot.p + (id * staticCap + L.n_static) * 2);
-                r.deco[s].assign(h_deco.p + id * decoCap, h_deco.p + id * decoCap + std::max(0, L.n_deco));
-                r.solid[s].clear();
-                for (int plane = 0; plane < 3; ++plane) {
-                    const uint32_t *src = h_solid.p + (id * 3 + plane) * gridWords;
-                    r.solid[s].insert(r.solid[s].end(), src, src + r.words[s]);
-                }
-            }
+            r.levels.clear();
+            for (int s = 0; s < levelSlots; ++s) r.levels.push_back(levels.read(rowOfSlot(e, s)));
         }
         MV_CUDA(cudaStreamSynchronize(stream));
         readKernelTimes();
@@ -1394,16 +1403,7 @@ struct mv_engine {
             const StateStore::HostRow &r = st.host[size_t(rows[i])];
             if (r.gen) gens[size_t(e)] = *r.gen;
             hostSlot[size_t(e)] = r.slot; hostEpisode[size_t(e)] = r.episode;
-            for (size_t s = 0; s < r.level.size(); ++s) {  // the store's slot count is the engine's
-                const size_t id = size_t(e) * size_t(levelSlots) + s;
-                h_levels.p[id] = r.level[s];
-                levelWords[id] = r.words[s];
-                std::copy(r.statics[s].begin(), r.statics[s].end(), h_statics.p + id * staticCap);
-                std::copy(r.staticRot[s].begin(), r.staticRot[s].end(), h_staticRot.p + id * staticCap * 2);
-                std::copy(r.deco[s].begin(), r.deco[s].end(), h_deco.p + id * decoCap);
-                for (int plane = 0; plane < 3; ++plane)
-                    std::copy_n(r.solid[s].begin() + ptrdiff_t(plane) * r.words[s], r.words[s], h_solid.p + (id * 3 + plane) * gridWords);
-            }
+            for (size_t s = 0; s < r.levels.size(); ++s) levels.write(rowOfSlot(e, int(s)), r.levels[s]);  // the store's slot count is the engine's
             if (!lastAsyncDone.empty()) lastAsyncDone[size_t(e)] = -1000;  // the loaded env's last episode end is not this engine's
         }
     }
@@ -1529,7 +1529,7 @@ struct mv_engine {
                 setError("level generation failed: " + r.error);
                 return MV_ERR_CAPACITY;
             }
-            if (int(r.out.statics.size()) > staticCap) {
+            if (int(r.out.statics.size()) > levels.staticCap) {
                 if (const int rc = growStatics(int(r.out.statics.size()))) return rc;
             }
             stageLevel(r.row, r.out);
@@ -1706,9 +1706,8 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
     e->genBusy.assign(size_t(e->E), 0);
     e->pool.reset(new WorkerPool(e->threads));
     // one pitch for all envs: the largest capacity among the engine's scenarios
-    e->gridCells = 0; e->decoCap = 0;
-    for (int sc : scs) { e->gridCells = std::max(e->gridCells, mv::gridCapacity(sc)); e->decoCap = std::max(e->decoCap, mv::decoCapacity(sc)); }
-    e->gridWords = e->gridCells / 32;
+    for (int sc : scs) { e->gridCells = std::max(e->gridCells, mv::gridCapacity(sc)); e->levels.decoCap = std::max(e->levels.decoCap, mv::decoCapacity(sc)); }
+    e->levels.gridWords = e->gridCells / 32;
     fillConsts(e->consts, w, h);
 
     auto ck = [&](cudaError_t err, const char *what) { if (err != cudaSuccess) { e->setError(std::string(what) + ": " + cudaGetErrorString(err)); return false; } return true; };
@@ -1726,7 +1725,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
          ck(e->d_viewCost.alloc(e->costItems() + size_t(E) + 1), "viewCost") && ck(e->resetViewOrder(), "viewOrder") && ck(e->d_ready.alloc(E), "ready") &&
          ck(cudaMemset(e->d_ready.p, 0, sizeof(uint32_t) * size_t(E)), "ready");
     { cudaDeviceProp prop; if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) e->numSMs = prop.multiProcessorCount; }
-    if (e->instCap > mvr::kMaxInstancesPerEnv) { e->setError("instance capacity exceeds the draw-order key range"); return fail(MV_ERR_CAPACITY); }
+    if (e->instCap() > mvr::kMaxInstancesPerEnv) { e->setError("instance capacity exceeds the draw-order key range"); return fail(MV_ERR_CAPACITY); }
     // few views: split every view into row bands so that the persistent grid (2 CTAs per SM) has something to balance; every band repeats
     // the view's geometry.  Measured on an H100 (ms per step, 1 / 2 / 3 bands): TowerBuilding 64 views 0.106 / 0.091 / 0.085, 256 views
     // 0.135 / 0.148 / 0.139, 512 views 0.185 / 0.185; Collect 256 views 0.546 / 0.425 / 0.387, 512 views 0.564 / 0.421
@@ -1824,7 +1823,7 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     if (k == "static_cap") {  // initial size of the per-level static-box arrays (they grow on demand; tests start small to exercise that)
         if (h->didReset) { h->setError("option static_cap must be set before the first reset"); return MV_ERR_STATE; }
         if (value < 1 || value > (1 << 20)) return MV_ERR_ARG;
-        h->staticCap = value;
+        h->levels.staticCap = value;
         return h->allocLevelSlots("static_cap");
     }
     if (k == "raster_bands") {  // row bands per view (each band is one work item of the persistent raster grid)
@@ -1916,7 +1915,7 @@ int mv_reset(mv_handle h) {
         if (cudaMemcpy(h->d_envs.p, init.data(), sizeof(MvEnvState) * init.size(), cudaMemcpyHostToDevice) != cudaSuccess) { h->setError("env init upload failed"); return MV_ERR_CUDA; }
         if (h->wantFinal) {
             const size_t E = size_t(h->E), N = size_t(h->N), px = size_t(h->W) * h->H;
-            if (h->d_termInst.alloc(E * size_t(h->instCap)) != cudaSuccess || h->d_termCounts.alloc(E * 8) != cudaSuccess || h->d_termViews.alloc(N * 16) != cudaSuccess ||
+            if (h->d_termInst.alloc(E * size_t(h->instCap())) != cudaSuccess || h->d_termCounts.alloc(E * 8) != cudaSuccess || h->d_termViews.alloc(N * 16) != cudaSuccess ||
                 h->d_finalObs.alloc(N * px * 4) != cudaSuccess || h->h_finalObs.alloc(N * px * 4) != cudaSuccess ||
                 (h->wantDepth && (h->d_finalDepth.alloc(N * px) != cudaSuccess || h->h_finalDepth.alloc(N * px) != cudaSuccess)) ||
                 cudaMemset(h->d_finalObs.p, 0, N * px * 4) != cudaSuccess || (h->wantDepth && cudaMemset(h->d_finalDepth.p, 0, sizeof(float) * N * px) != cudaSuccess)) {
@@ -2553,7 +2552,7 @@ int mv_debug_raster_stats(mv_handle h, unsigned long long *out16, int enable) {
     else h->d_rasterStats.free();
     return MV_OK;
 }
-int mv_debug_static_cap(mv_handle h) { return h ? h->staticCap : MV_ERR_ARG; }  // current size of the per-level static-box arrays
+int mv_debug_static_cap(mv_handle h) { return h ? h->levels.staticCap : MV_ERR_ARG; }  // current size of the per-level static-box arrays
 int mv_debug_raster_config(mv_handle h, int32_t *out4) {  // {persistent grid, CTAs per SM, dynamic shared memory bytes, row bands per view}
     if (!h || !out4) return MV_ERR_ARG;
     out4[0] = h->rasterGrid; out4[1] = h->rasterCtasPerSM; out4[2] = int32_t(h->rasterSmem); out4[3] = h->rasterBands;
@@ -2624,7 +2623,7 @@ static int dumpLevel(const MvLevel &L, const MvBox *statics, const float *static
 int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
     const size_t lid = h->liveRow(env);
-    return dumpLevel(h->h_levels.p[lid], h->h_statics.p + lid * size_t(h->staticCap), h->h_staticRot.p + lid * size_t(h->staticCap) * 2, h->A, false, out, cap);
+    return dumpLevel(h->levels.level(lid), h->levels.statics(lid), h->levels.rotations(lid), h->A, false, out, cap);
 }
 
 int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
@@ -2638,10 +2637,10 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
     if (cudaMemcpy(ag.data(), &h->d_agents.p[size_t(env) * h->A], sizeof(MvAgent) * h->A, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cudaMemcpy(ob.data(), &h->d_objects.p[size_t(env) * MV_MAX_OBJECTS], sizeof(MvObject) * MV_MAX_OBJECTS, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     const size_t lid = h->rowOfSlot(env, es.slot);
-    const MvLevel &L = h->h_levels.p[lid];
+    const MvLevel &L = h->levels.level(lid);
     std::vector<float> o;
     int ncol = h->A + L.n_obj;
-    const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
+    const MvBox *statics = h->levels.statics(lid);
     for (int i = 0; i < L.n_static; ++i) ncol += (statics[i].flags & MV_SOLID) ? 1 : 0;
     const float len = L.episode_len;
     o.push_back(es.episode_sec); o.push_back(len); o.push_back(float(es.num_frames)); o.push_back(float(es.highest_tower));
@@ -2685,9 +2684,9 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     const size_t lid = h->rowOfSlot(env, es.slot);
-    const MvLevel &L = h->h_levels.p[lid];
-    const uint32_t *sol = h->h_solid.p + lid * 3 * h->gridWords;
-    const MvBox *statics = h->h_statics.p + lid * size_t(h->staticCap);
+    const MvLevel &L = h->levels.level(lid);
+    const uint32_t *sol = h->levels.plane(lid, 0), *exitBits = h->levels.plane(lid, 1), *lavaBits = h->levels.plane(lid, 2);
+    const MvBox *statics = h->levels.statics(lid);
     std::vector<uint8_t> og(size_t(h->gridCells));
     if (cudaMemcpy(og.data(), h->d_objGrid.p + size_t(env) * h->gridCells, og.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     // opacity is a property of the box a solid voxel belongs to
@@ -2707,8 +2706,8 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
                     }
                 }
                 if (og[size_t(idx)] != MV_NO_OBJECT) flags |= 4;
-                if ((sol[size_t(h->gridWords) + (idx >> 5)] >> (idx & 31)) & 1u) flags |= 1 << 8;
-                if ((sol[2 * size_t(h->gridWords) + (idx >> 5)] >> (idx & 31)) & 1u) flags |= 2 << 8;
+                if ((exitBits[idx >> 5] >> (idx & 31)) & 1u) flags |= 1 << 8;
+                if ((lavaBits[idx >> 5] >> (idx & 31)) & 1u) flags |= 2 << 8;
                 if (flags) v.push_back({x + L.grid_org[0], y + L.grid_org[1], z + L.grid_org[2], flags});
             }
     std::sort(v.begin(), v.end());
@@ -2724,7 +2723,7 @@ int mv_debug_get_instances(mv_handle h, int env, float *out, int cap) {
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(cnt, h->d_instCounts.p + size_t(env) * 8, 32, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     std::vector<MvInstance> inst(static_cast<size_t>(cnt[1] > 0 ? cnt[1] : 1));
-    if (cudaMemcpy(inst.data(), h->d_inst.p + size_t(env) * size_t(h->instCap), sizeof(MvInstance) * inst.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
+    if (cudaMemcpy(inst.data(), h->d_inst.p + size_t(env) * size_t(h->instCap()), sizeof(MvInstance) * inst.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (cnt[1] * 18 > cap) return -cnt[1] * 18;
     for (int i = 0; i < cnt[1]; ++i) {
         out[i * 18] = float(inst[size_t(i)].mesh); out[i * 18 + 1] = float(inst[size_t(i)].color);

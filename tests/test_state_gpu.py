@@ -145,9 +145,19 @@ def test_clone_runs_the_saved_env_and_matches_the_oracle(built):
 def test_load_after_the_static_arrays_grew(built):
     """save with 16-box static arrays' first growth behind, run until a later level grows them again (the store is re-pitched with the
     engine), load and replay: identical"""
-    E, A, t0, M = 2, 2, 2, 120  # (master seed 48: the third maze of both envs has ~280 walls)
+    _load_after_growth(2, 48)  # (master seed 48: env 0's third maze has 281 walls)
+
+
+def test_load_after_the_static_arrays_grew_four_slots(built):
+    """the same with four level slots: the store's level slabs, four per env, are re-pitched too"""
+    _load_after_growth(4, 1)  # (master seed 1: no env's first four mazes have more than 211 walls, env 0's fifth has 267)
+
+
+def _load_after_growth(slots, seed):
+    """the reset stages the first `slots` levels of each env and grows the 16-box arrays to 256 boxes; a later maze has more walls"""
+    E, A, t0, M = 2, 2, 2, 120
     params = {"episodeLengthSec": 0.6}
-    g = _engine("HexExplore", E, A, 48, params, static_cap=16)
+    g = _engine("HexExplore", E, A, seed, params, static_cap=16, level_slots=slots)
     acts = _actions(E * A, t0 + M, seed=8)
     for t in range(t0):
         g.step(acts[t])
