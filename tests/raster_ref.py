@@ -45,12 +45,22 @@ def projection(W, H):
 _MESHES = {}
 
 
-def mesh(kind):
-    """(vertex positions float32 [n][3], triangle indices int64 [t][3]) of mesh type kind (0 box .. 4 cylinder)"""
+def _mesh_tables(kind):
     if kind not in _MESHES:
         vtx, idx = orc.mesh(kind)
-        _MESHES[kind] = (vtx.view(np.float32).reshape(-1, 6)[:, :3].copy(), idx.reshape(-1, 3).astype(np.int64))
+        v6 = vtx.view(np.float32).reshape(-1, 6)
+        _MESHES[kind] = (v6[:, :3].copy(), idx.reshape(-1, 3).astype(np.int64), v6[:, 3:].astype(np.float64))
     return _MESHES[kind]
+
+
+def mesh(kind):
+    """(vertex positions float32 [n][3], triangle indices int64 [t][3]) of mesh type kind (0 box .. 4 cylinder)"""
+    return _mesh_tables(kind)[:2]
+
+
+def normals(kind):
+    """vertex normals float64 [n][3] of mesh type kind (the mesh tables' float32 values)"""
+    return _mesh_tables(kind)[2]
 
 
 def model_view(view16, model16):
@@ -139,14 +149,29 @@ def _min_tile_part(lo, hi, size):
 class Render:
     """w: float64 [H][W] (view-space w of the visible fragment, 0 = empty); inst: int32 [H][W] (index + 1 of the winning instance, 0 =
     empty); z: float64 [H][W] window depth; tris: one dict per source triangle; pieces: one dict per drawn (front-facing, on-screen)
-    screen triangle; ties: samples that lay exactly on an edge of a front-facing triangle"""
+    screen triangle; ties: samples that lay exactly on an edge of a front-facing triangle.
+    The varyings of the visible fragment, interpolated with perspective correction: P, N float64 [H][W][3] (camera-space position and
+    unnormalised normal); color: int32 [H][W] palette index (-1 = empty).  frag runs the fragment stage on them."""
 
     def __init__(self, W, H):
         self.W, self.H = W, H
         self.z = np.full((H, W), np.inf)
         self.w = np.zeros((H, W))
         self.inst = np.zeros((H, W), dtype=np.int32)
+        self.P = np.zeros((H, W, 3))
+        self.N = np.zeros((H, W, 3))
+        self.color = np.full((H, W), -1, dtype=np.int32)
+        self.tri = np.full((H, W), -1, dtype=np.int32)  # index into tris of the visible fragment's source triangle
         self.tris, self.pieces, self.ties = [], [], 0
+        self.scene = None
+        self._frag = None
+
+    @property
+    def frag(self):
+        """the float64 fragment stage of every pixel (Fragments), computed once"""
+        if self._frag is None:
+            self._frag = shade64(self.P, self.N, self.color)
+        return self._frag
 
     @property
     def clipped(self):
@@ -156,14 +181,22 @@ class Render:
         return sum(1 for t in self.tris if t.get(key) == value)
 
 
-def render(view16, instances, W, H):
-    """draw the instances (rows of 18 floats: mesh, colour, 16 model floats column-major, in draw order) by the specification's rules"""
+def render(view16, instances, W, H, naive_normals=False):
+    """draw the instances (rows of 18 floats: mesh, colour, 16 model floats column-major, in draw order) by the specification's rules.
+    naive_normals: transform the normals by the model-view 3 x 3 itself instead of its inverse transpose (a deliberately wrong vertex
+    stage, for proving that a scene tells the two apart)"""
     R = Render(W, H)
+    R.scene = (view16, instances)
     for ii, row in enumerate(np.asarray(instances, dtype=F32).reshape(-1, 18)):
         verts, tris = mesh(int(row[0]))
         mv = model_view(view16, row[2:18])
         mirrored = bool(np.linalg.det(mv[:3, :3].astype(np.float64)) <= 0)
         clip = vertex_stage(view16, row[2:18], verts, W, H)
+        # varyings in float64 from the float32 model-view matrix: camera-space position and normal (inverse transpose, by numpy)
+        M = mv.T.astype(np.float64)  # [row][col]
+        nm = M[:3, :3] if naive_normals else np.linalg.inv(M[:3, :3]).T
+        cam64 = verts.astype(np.float64) @ M[:3, :3].T + M[:3, 3]
+        vary = np.concatenate([clip.astype(np.float64), cam64, normals(int(row[0])) @ nm.T], axis=1)  # [n][10]: clip, P, N
         p00, p11, _, _ = projection(W, H)
         cam = np.stack([clip[:, 0] / np.float64(p00), clip[:, 1] / np.float64(p11), -clip[:, 3].astype(np.float64)], axis=1)
         for ti, tri in enumerate(tris):
@@ -176,17 +209,19 @@ def render(view16, instances, W, H):
             rec = {"inst": ii, "tri": ti, "mirrored": mirrored, "behind_near": bool(near_out.all()), "beyond_far": bool(far_out.all()),
                    "clip": {(False, False): "none", (True, False): "near", (False, True): "far", (True, True): "both"}[(bool(near_out.any()), bool(far_out.any()))],
                    "culled": False, "front": False, "small": False, "bound": 0, "max_coord": 0, "max_delta": 0, "pieces": 0, "covered": 0,
-                   "sin": float(abs(np.dot(n, a)) / den) if den > 0 else None, "min_extent": 1 << 62}
+                   "sin": float(abs(np.dot(n, a)) / den) if den > 0 else None, "min_extent": 1 << 62,
+                   "flat": bool((normals(int(row[0]))[tri] == normals(int(row[0]))[tri[0]]).all())}
             R.tris.append(rec)
+            v = vary[tri]
             if rec["clip"] != "none":
-                poly = clip_polygon([c[k].astype(np.float64) for k in range(3)])
+                poly = clip_polygon([v[k] for k in range(3)])  # the varyings ride along as extra components
                 pieces = [(poly[0], poly[k], poly[k + 1]) for k in range(1, len(poly) - 1)]
                 rec["poly"] = len(poly)
             else:
-                pieces = [(c[0], c[1], c[2])]
+                pieces = [(v[0], v[1], v[2])]
             rec["pieces"] = len(pieces)
             for piece in pieces:
-                sv = [snap(np.asarray(v, dtype=F32), W, H) for v in piece]
+                sv = [snap(np.asarray(v[:4], dtype=F32), W, H) for v in piece]
                 xs, ys = [s[0] for s in sv], [s[1] for s in sv]
                 rec["max_coord"] = max(rec["max_coord"], max(abs(v) for v in xs + ys))
                 rec["max_delta"] = max(rec["max_delta"], max(abs(xs[i] - xs[j]) for i in range(3) for j in range(3)),
@@ -236,4 +271,87 @@ def render(view16, instances, W, H):
                 R.z[py0:py1 + 1, px0:px1 + 1] = np.where(win, z, bz)
                 R.w[py0:py1 + 1, px0:px1 + 1] = np.where(win, w, R.w[py0:py1 + 1, px0:px1 + 1])
                 R.inst[py0:py1 + 1, px0:px1 + 1] = np.where(win, ii + 1, R.inst[py0:py1 + 1, px0:px1 + 1])
+                # perspective-correct varyings: weights lambda_i / w_i, w_i in float64 from the (clipped) vertex itself
+                k = [lam[i] / piece[i][3] for i in range(3)]
+                s = k[0] + k[1] + k[2]
+                for dst, c0 in ((R.P, 4), (R.N, 7)):
+                    val = sum((k[i] / s)[..., None] * piece[i][c0:c0 + 3] for i in range(3))
+                    dst[py0:py1 + 1, px0:px1 + 1] = np.where(win[..., None], val, dst[py0:py1 + 1, px0:px1 + 1])
+                R.color[py0:py1 + 1, px0:px1 + 1] = np.where(win, int(row[1]), R.color[py0:py1 + 1, px0:px1 + 1])
+                R.tri[py0:py1 + 1, px0:px1 + 1] = np.where(win, len(R.tris) - 1, R.tri[py0:py1 + 1, px0:px1 + 1])
     return R
+
+
+# ---------------------------------------------------------------------------------------------------- the fragment stage in float64
+def _palette():
+    from test_ref_golden import PALETTE
+
+    return np.array([[(c >> 16) & 255, (c >> 8) & 255, c & 255] for c in PALETTE], dtype=np.float64) / 255.0
+
+
+LIGHT = np.array([0.0, 4.0, 2.0])  # camera space (v4r_env_renderer.cpp:220)
+SPEC_GATE = 0.001                  # the highlight is computed only where intensity > SPEC_GATE (uber.frag)
+SHININESS = 300
+
+
+class Fragments:
+    """per pixel of a Render: lo float64 [H][W][3] (the colour in LSB, 255 * clamp(Lo, 0, 1)), byte uint8 [H][W][3] (UNORM8: floor(lo +
+    0.5)), margin float64 [H][W][3] (distance of 255 * Lo from the nearest rounding boundary k + 1/2, k = 0 .. 254, in LSB; inf where
+    nothing was drawn), intensity = max(N.L, 0), vdr = V.reflect(-L, N) (nan where the highlight is gated off or nothing was drawn), spec
+    (the highlight term, 0 where gated off)"""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+def shade64(P, N, color):
+    """uber.frag:112-141 (the non-Blinn-Phong branch) restated in float64 for every pixel: P, N [H][W][3] camera-space position and
+    unnormalised normal, color [H][W] palette index (-1: nothing drawn, black).  Light at LIGHT, colour 0.66, specular 1, shininess 300:
+        Lo = 0.33 d + 0.73 * 0.66 d * max(N.L, 0) + (N.L > 0.001 ? clamp(max(V.R, 0)^300, 0, 1) : 0),   R = reflect(-L, N)"""
+    drawn = color >= 0
+    d = _palette()[np.where(drawn, color, 0)]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        cd = -P
+        nl = (LIGHT + cd) / np.linalg.norm(LIGHT + cd, axis=-1, keepdims=True)
+        nn = N / np.linalg.norm(N, axis=-1, keepdims=True)
+        ndl = (nn * nl).sum(-1)
+        intensity = np.maximum(ndl, 0.0)
+        refl = -nl + 2.0 * ndl[..., None] * nn
+        vdr = (cd / np.linalg.norm(cd, axis=-1, keepdims=True) * refl).sum(-1)
+    lit = drawn & (intensity > SPEC_GATE)
+    vdr = np.where(lit, vdr, np.nan)
+    spec = np.where(lit, np.clip(np.maximum(np.nan_to_num(vdr), 0.0) ** SHININESS, 0.0, 1.0), 0.0)
+    Lo = 0.33 * d + (0.73 * 0.66) * d * np.where(drawn, intensity, 0.0)[..., None] + spec[..., None]
+    x = np.where(drawn[..., None], 255.0 * Lo, 0.0)
+    margin = np.where(drawn[..., None], np.abs(x - np.clip(np.floor(x) + 0.5, 0.5, 254.5)), np.inf)
+    lo = np.clip(x, 0.0, 255.0)
+    return Fragments(lo=lo, byte=np.floor(lo + 0.5).astype(np.uint8), margin=margin, intensity=np.where(drawn, intensity, np.nan), vdr=vdr,
+                     spec=spec)
+
+
+# The colour rule.  A rasteriser that computes the fragment stage in float32 (the oracle; the kernel's exact variant reproduces it byte
+# for byte) writes, wherever it draws the same surface as the reference, bytes within 1 LSB of the float64 ones, and a byte may differ at
+# all only where 255 Lo lies within M LSB of a rounding boundary (k + 1/2):
+#   M = M0 + 255 * 300 * max(vdr, 0)^299 * EPS_VDR   [+ 255 * spec where vdr <= FAST_CUT, fast fragment stage only]
+#   * M0 = 0.02 LSB: the ambient and diffuse terms move by 255 * 0.81 * (error of N.L); N.L carries float32 rounding of the vertex stage,
+#     the normal matrix, the interpolation and two normalisations, a few ulp, below 1e-6 -- 2e-4 LSB; M0 leaves a hundredfold margin
+#     (measured on every family against the oracle: at most 0.006 LSB, all of it in highlights);
+#   * the highlight vdr^300 multiplies an error of vdr by 300 vdr^299: EPS_VDR = 2^-20 (16 ulp of 1.0 in float32; the fast stage's
+#     rsqrt.approx is within 2 ulp) covers the dot products and normalisations vdr goes through -- up to 0.073 LSB at vdr = 1;
+#   * the fast stage drops the highlight where vdr <= 0.97 (0.97^300 = 1.1e-4, at most 0.028 LSB): there the float64 value it is held to
+#     is shifted by exactly the term dropped.
+M0, EPS_VDR, FAST_CUT = 0.02, 2.0 ** -20, 0.97
+
+
+def colour_rule(frag, rgb, same, fast=False):
+    """rgb uint8 [H][W][3] against the float64 fragments where `same` (both sides drew the same surface) holds: (bytes that break the rule,
+    bytes that differ, the largest margin among the differing bytes in LSB, the largest difference)"""
+    vdr = np.maximum(np.nan_to_num(frag.vdr, nan=0.0), 0.0)
+    M = M0 + 255.0 * SHININESS * vdr ** (SHININESS - 1) * EPS_VDR
+    if fast:
+        M = M + np.where(vdr <= FAST_CUT, 255.0 * frag.spec, 0.0)
+    d = np.abs(rgb[..., :3].astype(np.int16) - frag.byte.astype(np.int16))
+    d = np.where(same[..., None], d, 0)
+    differ = d > 0
+    broken = (d > 1) | (differ & (frag.margin >= M[..., None]))
+    return int(broken.sum()), int(differ.sum()), float(frag.margin[differ].max(initial=0.0)), int(d.max(initial=0))

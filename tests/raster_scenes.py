@@ -260,9 +260,139 @@ def offscreen_vertex(W, H, log2_px, opposite=False):
     return _scene(rows)
 
 
+def _unit(v):
+    return np.asarray(v, dtype=np.float64) / np.linalg.norm(v)
+
+
+def _basis(axis_dir, axis, hint=(0.3, 0.9, 0.2)):
+    """a rotation whose column `axis` is the unit vector axis_dir"""
+    n = _unit(axis_dir)
+    u = _unit(np.cross(n, hint))
+    R = np.zeros((3, 3))
+    R[:, axis], R[:, (axis + 1) % 3], R[:, (axis + 2) % 3] = n, u, np.cross(n, u)
+    return R
+
+
+def _cells(n, W, H, max_aspect=None):
+    """centres (px, py) and size in pixels of n cells of a grid laid over the frame with about square cells; max_aspect: over the central
+    part of the frame at most that many times wider than high or higher than wide"""
+    w, h = (W, H) if max_aspect is None else (min(W, max_aspect * H), min(H, max_aspect * W))
+    cols = max(1, min(n, int(round(np.sqrt(n * w / h)))))
+    rows = -(-n // cols)
+    cw, ch = w / cols, h / rows
+    return [((W - w) / 2 + (k % cols + 0.5) * cw, (H - h) / 2 + (k // cols + 0.5) * ch) for k in range(n)], min(cw, ch)
+
+
+def _px_size(z, W, H):
+    """view-space length of one pixel at distance z (pixels are square)"""
+    p00, _, _, _ = ref.projection(W, H)
+    return z / (float(p00) * W / 2)
+
+
+def _bisector(c):
+    """unit normal that reflects the light at point c (view space) into the eye: the bisector of the directions to the light and the eye"""
+    return _unit(_unit(ref.LIGHT - c) + _unit(-c))
+
+
+def highlights(W, H, seed=0):
+    """spheres, capsules, cylinders and boxes turned so that the light's reflection reaches the eye: box faces and curved sides whose
+    normal is the bisector of the light and eye directions -- highlights that saturate, and the fall-off around them through the fast
+    fragment stage's vdr cut-off (0.97)"""
+    rng = np.random.default_rng(seed)
+    kinds = [0, 2, 0, 1, 4, 0, 2, 4, 0, 1, 3, 2]
+    centres, cell = _cells(len(kinds), W, H)
+    rows = []
+    for k, (mesh, (px, py)) in enumerate(zip(kinds, centres)):
+        z = rng.uniform(3.0, 8.0)
+        c = np.array(list(_view_xy(px, py, z, W, H)) + [-z])
+        r = 0.42 * cell * _px_size(z, W, H)
+        b = _bisector(c)
+        if mesh == 0:  # face +z across the bisector, its centre at c
+            R = _basis(b, 2)
+            half = np.array([r, r * rng.uniform(0.6, 1.0), 0.3 * r])
+            rows.append(_row(0, k % 22, _model(c - b * half[2], half, R)))
+        elif mesh == 2:
+            rows.append(_row(2, k % 22, _model(c - b * r, [r, r, r], _rot(*rng.uniform(0, 2 * np.pi, 3)))))
+        else:  # capsule, cone, cylinder: axis (y) across the bisector, so that a line of the side faces it
+            R = _basis(b, 0)
+            ry = r * (0.5 if mesh == 1 else 1.0)
+            rows.append(_row(mesh, k % 22, _model(c - b * 0.6 * r, [0.6 * r, ry, 0.6 * r], R)))
+    return _scene(rows)
+
+
+def light_gates(W, H, seed=0):
+    """box faces in planes that pass the light at a chosen signed distance: N.L = delta / |light - P| over the whole face, so a face lies
+    wholly at intensity 0, inside (0, 0.001] (the highlight is gated off), or just above 0.001 (it is computed)"""
+    rng = np.random.default_rng(seed)
+    targets = [-0.05, 0.0, 0.0005, 0.0008, 0.0013, 0.002, -0.0005, 0.0006, 0.0016]
+    centres, cell = _cells(len(targets), W, H, max_aspect=2)  # (at the far ends of a 16:1 frame the eye and light directions nearly meet)
+    rows = []
+    for k, (t, (px, py)) in enumerate(zip(targets, centres)):
+        z = rng.uniform(3.0, 8.0)
+        c = np.array(list(_view_xy(px, py, z, W, H)) + [-z])
+        L, V = _unit(ref.LIGHT - c), _unit(-c)
+        perp = _unit(V - V.dot(L) * L)   # in the plane through the light, as near the eye direction as it gets
+        n = np.sqrt(1.0 - t * t) * perp + t * L   # N.(light - c) = t |light - c|: the plane passes the light at distance t |light - c|
+        r = 0.45 * cell * _px_size(z, W, H) / max(0.3, n.dot(V))  # the face is seen obliquely: stretch it to fill the cell
+        half = np.array([r, r, 0.2 * r])
+        rows.append(_row(0, k % 22, _model(c - n * half[2], half, _basis(n, 2, hint=np.cross(n, V) + 0.01))))
+    return _scene(rows)
+
+
+def scaled_normals(W, H, seed=0):
+    """spheres, capsules, cones, cylinders and boxes under rotations with per-axis scales from 1e-2 to 1e2 of a common size (ratios up to
+    1e4), some mirrored: the normal matrix (inverse transpose) and the model matrix turn the normals far apart"""
+    rng = np.random.default_rng(seed)
+    kinds = [2, 1, 3, 4, 2, 0, 2, 4, 3, 1, 2, 0]
+    centres, cell = _cells(len(kinds), W, H)
+    rows = []
+    for k, (mesh, (px, py)) in enumerate(zip(kinds, centres)):
+        z = rng.uniform(4.0, 10.0)
+        c = np.array(list(_view_xy(px, py, z, W, H)) + [-z])
+        u = np.zeros(3)
+        u[k % 3], u[(k + 1) % 3], u[(k + 2) % 3] = 2.0, rng.uniform(1.0, 2.0), -2.0  # one axis long, one thin: plates
+        s = 10.0 ** u
+        s *= 0.45 * cell * _px_size(z, W, H) / s.max()
+        if k % 3 == 2:
+            s[k % 3] *= -1  # mirrored
+        if k % 6 == 5:
+            s[:] *= -1      # mirrored along all three axes
+        rows.append(_row(mesh, k % 22, _model(c, s, _rot(*rng.uniform(0, 2 * np.pi, 3)))))
+    return _scene(rows)
+
+
+def near_plane(W, H, seed=0):
+    """boxes, rods and spheres from behind the camera to in front of it: the near plane cuts flat faces and curved sides (the clipper
+    makes vertices whose position and normal are interpolated), to the left, right, above and below the eye and straight ahead"""
+    rng = np.random.default_rng(seed)
+    rows = [_row(0, 8, _model([0.0, -1.2, -4.0], [3.0, 0.4, 6.0], _rot(0.05, 0.1, 0.0))),   # a floor slab under the camera
+            _row(0, 9, _model([1.0, 0.0, -2.0], [0.2, 0.6, 4.0], _rot(0.0, -0.1, 0.05)))]     # and a wall beside it
+    for k, (x, y) in enumerate(((0.5, 0.0), (-0.55, 0.05), (0.0, 0.4), (0.05, -0.45))):
+        rot = _basis([0.1 * x, 0.1 * y, 1.0], 1)   # cylinder / capsule axis (y) along the view direction
+        r = rng.uniform(0.15, 0.25)
+        rows.append(_row(4 if k % 2 == 0 else 1, 1 + k, _model([x, y, -1.0], [r, 2.0 if k % 2 == 0 else 1.0, r], rot)))
+    for k, (x, y) in enumerate(((0.6, -0.3), (-0.5, 0.3))):
+        rows.append(_row(2, 6 + k, _model([x, y, 0.0], [0.45, 0.45, 0.45], _rot(*rng.uniform(0, 2 * np.pi, 3)))))
+    rows.append(_row(3, 11, _model([0.0, 0.0, -0.3], [0.08, 0.5, 0.08], _basis([0.05, 0.02, 1.0], 1))))  # a cone pointing at the eye
+    return _scene(rows)
+
+
+def palette(W, H, seed=0):
+    """the 22 colours of the palette on boxes facing the camera, lit by the light above and behind it"""
+    rng = np.random.default_rng(seed)
+    centres, cell = _cells(22, W, H, max_aspect=4)
+    rows = []
+    for k, (px, py) in enumerate(centres):
+        z = rng.uniform(3.0, 8.0)
+        h = 0.42 * cell
+        rows.append(_window_box(px - h, py - h, px + h, py + h, -z, 0.3, W, H, k))
+    return _scene(rows)
+
+
 FAMILIES = {"far_plane": far_plane, "edge_bounds": edge_bounds, "tiny_and_large": tiny_and_large, "duplicates": duplicates, "mirrored": mirrored,
-            "grazing": grazing, "frustum_tangent": frustum_tangent, "slivers": slivers, "borders": borders, "ties": ties}
-CLIPPED = {"far_plane"}  # families whose triangles the clipper cuts (new vertices: a few pixels may differ)
+            "grazing": grazing, "frustum_tangent": frustum_tangent, "slivers": slivers, "borders": borders, "ties": ties,
+            "highlights": highlights, "light_gates": light_gates, "scaled_normals": scaled_normals, "near_plane": near_plane, "palette": palette}
+CLIPPED = {"far_plane", "near_plane"}  # families whose triangles the clipper cuts (new vertices: a few pixels may differ)
 
 
 def build(family, W, H, seed=0, **kw):
@@ -303,3 +433,34 @@ def check_reach(family, R, W, H):
         assert R.ties > 50, "samples on edges"
         if family == "borders":
             assert (R.inst[:, W - 1] > 0).any() and (R.inst[H - 1] > 0).any(), "the last column and row drawn"
+    elif family == "highlights":
+        F, drawn = R.frag, R.inst > 0
+        vdr = np.nan_to_num(F.vdr, nan=-1.0)
+        flat = np.array([t["flat"] for t in R.tris] + [False])[R.tri] & drawn
+        assert ((vdr > 0.97) & flat).sum() >= 100 and ((vdr > 0.97) & ~flat & drawn).sum() >= 20, "highlights on flat and curved triangles"
+        assert ((vdr > 0.9) & (vdr <= 0.97)).sum() >= 100, "the highlights' fall-off below the fast stage's cut-off"
+        assert (F.lo[drawn] >= 254.5).sum() >= 100, "saturated channels"
+    elif family == "light_gates":
+        I = R.frag.intensity[R.inst > 0]
+        assert (I == 0).sum() >= 100, "lit-away faces (intensity 0)"
+        assert ((I > 0) & (I <= ref.SPEC_GATE)).sum() >= 100, "intensity in (0, 0.001]: the highlight gated off"
+        assert ((I > ref.SPEC_GATE) & (I <= 3 * ref.SPEC_GATE)).sum() >= 100, "intensity just above 0.001: the highlight computed"
+    elif family == "scaled_normals":
+        drawn = R.inst > 0
+        naive = render_naive(R)
+        off = (np.abs(naive.frag.byte.astype(np.int16) - R.frag.byte.astype(np.int16)).max(-1) > 2) & drawn
+        assert off.sum() >= 200 and off.sum() >= 0.25 * drawn.sum(), "normals by the model matrix instead of the normal matrix shade " \
+            "%d of %d pixels within 2 LSB" % (int(drawn.sum() - off.sum()), int(drawn.sum()))
+        assert sum(1 for t in front if t["mirrored"]) >= 4, "front faces of mirrored instances drawn"
+    elif family == "near_plane":
+        cut = [t for t in front if t["clip"] in ("near", "both")]
+        assert sum(1 for t in cut if t["flat"]) >= 2 and sum(1 for t in cut if not t["flat"]) >= 4, \
+            "flat and curved triangles cut by the near plane cover samples"
+    elif family == "palette":
+        lit = (R.inst > 0) & (np.nan_to_num(R.frag.intensity) > 0.3)
+        assert all((lit & (R.color == k)).sum() >= 20 for k in range(22)), "every palette colour on lit faces"
+
+
+def render_naive(R):
+    """the scene of R drawn once more with normals transformed by the model-view 3 x 3 instead of its inverse transpose"""
+    return ref.render(*R.scene, R.W, R.H, naive_normals=True)

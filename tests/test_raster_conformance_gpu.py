@@ -8,7 +8,10 @@ was built for (test_raster_independent.py checks the same families against the o
     triangles at extreme aspect, near-equal depths of two instances);
   * clipped scenes: at most 8 pixels per 128 x 72 frame's worth differ (new clipper vertices in float32 and float64 can snap one
     sub-pixel apart; w near the far plane carries float32 rounding of 1 / w);
-  * fast against exact: depth and segmentation byte-identical, colour within 1 LSB with more than 99.9 % of the bytes identical.
+  * fast against exact: depth and segmentation byte-identical, colour within 1 LSB with more than 99.9 % of the bytes identical;
+  * colour: the exact variant byte-identical to the oracle's rasteriser in colour and depth (every family, list capacity, band count
+    and size); both variants against the float64 fragment stage (raster_ref.shade64) by raster_ref.colour_rule wherever the same
+    instance won, with at least 99.9 % of the bytes equal to the float64 byte.
 
 Variants run as a sparse matrix: every family at 128 x 72 in all four shading x segmentation variants; triangle-list capacity x band
 count on a subset; other sizes up to the widest the API accepts (768) on a subset.  The off-screen envelope: triangles with a corner
@@ -31,23 +34,39 @@ def _draw(view16, inst, W, H, fast=0, tri_cap=0, bands=0):
     return rgba, depth, seg, stats
 
 
-def _check(family, R, depth, seg, W, H, clipped=None):
+def _check(family, R, out, W, H, fast, clipped=None):
+    """out = (rgba, depth, seg, ...) of _draw for the scene R was drawn from"""
+    rgba, depth, seg = out[:3]
     clipped = family in scenes.CLIPPED if clipped is None else clipped
     cov_dev, cov_ref = depth > 0, R.w > 0
     mism = int((cov_dev != cov_ref).sum())
     both = cov_dev & cov_ref
     rel = np.abs(depth[both].astype(np.float64) - R.w[both]) / R.w[both]
     assert np.array_equal(seg > 0, cov_dev), "segmentation 0 exactly where nothing was drawn"
+    if not fast:  # the exact fragment stage reproduces the oracle's float32 arithmetic: colour and depth byte for byte
+        o_rgba, o_depth = orc.render_instances(*R.scene, W, H, want_depth=True)
+        assert np.array_equal(depth.view(np.uint32), o_depth.view(np.uint32)), "depth differs from the oracle's in %d pixels" % int((depth != o_depth).sum())
+        assert np.array_equal(rgba, o_rgba), "colour differs from the oracle's in %d pixels" % int((rgba != o_rgba).any(-1).sum())
+    # colour against the float64 fragment stage wherever the same instance won (raster_ref.colour_rule)
+    same = both & (seg.astype(np.int32) == R.inst)
+    broken, differ, worst, dmax = ref.colour_rule(R.frag, rgba, same, fast=bool(fast))
+    print("%s %dx%d %s: %d colour bytes differ from the float64 ones (by up to %d), worst boundary margin among them %.4f LSB, %d break the "
+          "rule" % (family, W, H, "fast" if fast else "exact", differ, dmax, worst, broken))
     if clipped:  # 8 pixels per 128 x 72 frame's worth of pixels
         allowed = max(8, 8 * W * H // (128 * 72))
         assert mism <= allowed, "coverage differs in %d pixels" % mism
         assert (rel > 1e-4).sum() <= allowed, "w differs in %d pixels" % int((rel > 1e-4).sum())
+        assert broken <= 3 * allowed, "%d colour bytes break the rule (%d differ, by up to %d)" % (broken, differ, dmax)
+        assert differ <= 0.001 * W * H * 3, "%d of the %d colour bytes differ from the float64 ones" % (differ, W * H * 3)
         return
     assert mism == 0, "coverage differs in %d pixels" % mism
     loose = 0 if (W, H) == (128, 72) else 8
     assert rel.max(initial=0) < 1e-4 and (rel > 2e-5).sum() <= loose, "depth differs by %.3g" % rel.max(initial=0)
     wrong = int((seg[cov_dev].astype(np.int32) != R.inst[cov_dev]).sum())  # (elsewhere near-equal depths of two instances may swap)
     assert wrong <= loose, "the winning instance differs in %d pixels" % wrong
+    assert broken == 0, "%d colour bytes break the rule (%d differ, by up to %d; worst margin %.4f LSB)" % (broken, differ, dmax, worst)
+    # of the frame's colour bytes (as fast against exact above), those where the same instance won equal the float64 byte
+    assert differ <= 0.001 * W * H * 3, "%d of the %d colour bytes differ from the float64 ones" % (differ, W * H * 3)
 
 
 @pytest.mark.parametrize("family", sorted(scenes.FAMILIES))
@@ -60,7 +79,8 @@ def test_every_family_every_variant_at_128x72(family):
 
     exact, d_exact, s_exact, st = _draw(view16, inst, W, H, fast=0)
     fast, d_fast, s_fast, _ = _draw(view16, inst, W, H, fast=1)
-    _check(family, R, d_exact, s_exact, W, H)
+    _check(family, R, (exact, d_exact, s_exact), W, H, fast=0)
+    _check(family, R, (fast, d_fast, s_fast), W, H, fast=1)
     assert np.array_equal(d_exact.view(np.uint32), d_fast.view(np.uint32)) and np.array_equal(s_exact, s_fast), "fast and exact differ in depth or segmentation"
     diff = np.abs(exact.astype(np.int16) - fast.astype(np.int16))
     assert diff.max() <= 1 and (diff == 0).mean() > 0.999
@@ -73,16 +93,17 @@ def test_every_family_every_variant_at_128x72(family):
 
 @pytest.mark.parametrize("tri_cap", [0, 96, 32])
 @pytest.mark.parametrize("bands", [1, 2, 3])
-@pytest.mark.parametrize("family", ["duplicates", "tiny_and_large", "edge_bounds", "borders"])
+@pytest.mark.parametrize("family", ["duplicates", "tiny_and_large", "edge_bounds", "borders", "highlights", "near_plane"])
 def test_list_capacity_and_bands(family, tri_cap, bands):
     W, H = 128, 72
     kw = {"band_rows": [((H // 4 + bands - 1) // bands) * 4 * k for k in range(1, bands)]} if family == "borders" else {}
     view16, inst = scenes.build(family, W, H, **kw)
     R = ref.render(view16, inst, W, H)
     scenes.check_reach(family, R, W, H)
-    _, depth, seg, st = _draw(view16, inst, W, H, tri_cap=tri_cap, bands=bands)
-    _check(family, R, depth, seg, W, H)
-    if tri_cap == 32 and family in ("duplicates", "tiny_and_large"):
+    out = _draw(view16, inst, W, H, tri_cap=tri_cap, bands=bands)
+    _check(family, R, out, W, H, fast=0)
+    st = out[3]
+    if tri_cap == 32 and family in ("duplicates", "tiny_and_large", "highlights", "near_plane"):
         assert st[6] > bands, "views drawn in several list batches"
 
 
@@ -106,10 +127,10 @@ def test_duplicates_across_instance_chunks_and_list_batches(gap):
         assert not (R.inst == j + 1).any() or won, "the later copy wins every tie"
     assert split >= 3, "pairs in different chunks, with at least 32 drawn triangles between the copies"
     for tri_cap, bands in ((0, 0), (32, 1)):
-        _, depth, seg, st = _draw(view16, inst, W, H, tri_cap=tri_cap, bands=bands)
-        _check("duplicates", R, depth, seg, W, H)
+        out = _draw(view16, inst, W, H, tri_cap=tri_cap, bands=bands)
+        _check("duplicates", R, out, W, H, fast=0)
         if tri_cap == 32:
-            assert st[6] > 2
+            assert out[3][6] > 2
 
 
 def test_far_clipping_matches_the_oracle_bit_for_bit():
@@ -130,14 +151,15 @@ SIZES = [(64, 64), (160, 96), (32, 512), (512, 32), (768, 432), (768, 32)]
 
 
 @pytest.mark.parametrize("size", SIZES)
-@pytest.mark.parametrize("family", ["ties", "borders", "tiny_and_large", "far_plane", "mirrored", "grazing", "edge_bounds", "slivers"])
+@pytest.mark.parametrize("family", ["ties", "borders", "tiny_and_large", "far_plane", "mirrored", "grazing", "edge_bounds", "slivers", "highlights",
+                                    "scaled_normals", "near_plane", "palette"])
 def test_other_sizes(family, size):
     W, H = size
     view16, inst = scenes.build(family, W, H)
     R = ref.render(view16, inst, W, H)
     scenes.check_reach(family, R, W, H)
-    _, depth, seg, _ = _draw(view16, inst, W, H, fast=1)
-    _check(family, R, depth, seg, W, H)
+    for fast in (1, 0):
+        _check(family, R, _draw(view16, inst, W, H, fast=fast), W, H, fast=fast)
 
 
 @pytest.mark.parametrize("W,H", [(128, 72), (768, 32)])

@@ -15,6 +15,9 @@ bounds the window coordinates the product's own scenes produce (the envelope ins
 Compared: the oracle's depth image (view-space w of the visible fragment, 0 = nothing drawn) -- its zero pattern IS the coverage
 mask.  Scenes without clipping must agree in every pixel (coverage exactly, depth to float32 rounding); scenes cut by the near
 plane (the clipper creates new vertices, whose float32 vs float64 positions can snap one sub-pixel apart) in all but a handful.
+Colour: raster_ref.shade64 restates the fragment stage (uber.frag:112-141) in float64 on float64 varyings (camera-space position and
+normal, the normal by numpy's inverse transpose, carried through the clipper, interpolated with perspective correction); the oracle's
+float32 bytes must follow raster_ref.colour_rule, whose tolerance is derived there.
 """
 import warnings
 
@@ -72,6 +75,16 @@ def _compare(view16, inst):
     return cov_ref, cov_mine, rel, clipped
 
 
+def _colour(view16, inst, W, H, R=None):
+    """the oracle's colour against the float64 fragment stage (raster_ref.colour_rule) where both draw the same surface (depth within
+    2e-5): (broken bytes, differing bytes, worst margin among them, largest difference)"""
+    R = ref.render(view16, inst, W, H) if R is None else R
+    rgba, od = orc.render_instances(view16, inst, W, H, want_depth=True)
+    same = (od > 0) & (R.w > 0)
+    same[same] = np.abs(od[same].astype(np.float64) - R.w[same]) / R.w[same] < 2e-5
+    return ref.colour_rule(R.frag, rgba, same)
+
+
 @pytest.mark.parametrize("seed", range(8))
 def test_unclipped_scenes_agree_in_every_pixel(seed):
     rng = np.random.default_rng(1000 + seed)
@@ -82,6 +95,8 @@ def test_unclipped_scenes_agree_in_every_pixel(seed):
     assert np.array_equal(cov_ref, cov_mine), "coverage differs in %d pixels" % int((cov_ref != cov_mine).sum())
     # same visible surface: w agrees to float32 rounding of the oracle's arithmetic (a different winner would be a different surface)
     assert rel.max() < 2e-5, "depth differs by %.3g" % rel.max()
+    broken, differ, worst, dmax = _colour(view16, inst, W, H)
+    assert broken == 0, "%d colour bytes break the rule (%d differ, by up to %d)" % (broken, differ, dmax)
 
 
 @pytest.mark.parametrize("seed", range(6))
@@ -93,6 +108,8 @@ def test_scenes_cut_by_the_near_plane_agree(seed):
     mism = int((cov_ref != cov_mine).sum())
     assert mism <= 8, "coverage differs in %d pixels" % mism  # new vertices made by the clipper may snap one sub-pixel apart
     assert (rel > 1e-4).sum() <= 8, "visible surface differs in %d pixels" % int((rel > 1e-4).sum())
+    broken, differ, worst, dmax = _colour(view16, inst, W, H)
+    assert broken <= 3 * 8, "%d colour bytes break the rule (%d differ, by up to %d)" % (broken, differ, dmax)
 
 
 @pytest.mark.parametrize("seed", range(4))
@@ -199,7 +216,10 @@ import raster_scenes as scenes  # noqa: E402
 @pytest.mark.parametrize("family", sorted(scenes.FAMILIES))
 def test_scene_families_reach_their_branch_and_agree_with_the_oracle(family, size):
     """every constructed family of test_raster_conformance_gpu.py, drawn by the restatement: it reaches what it was built for, and the
-    oracle agrees with it as on the random scenes (the window coordinates stay far inside the int32 range the oracle snaps to)"""
+    oracle agrees with it as on the random scenes (the window coordinates stay far inside the int32 range the oracle snaps to) -- in
+    coverage, depth and colour (raster_ref.colour_rule: within 1 LSB of the float64 fragment stage, and different only within M LSB of
+    a rounding boundary; clipped families and sizes other than 128 x 72 in at most 8 pixels' worth of bytes, where near-equal depths of
+    two surfaces or clipper vertices one sub-pixel apart make the two sides draw different surfaces)"""
     W, H = size
     view16, inst = scenes.build(family, W, H)
     R = ref.render(view16, inst, W, H)
@@ -215,6 +235,11 @@ def test_scene_families_reach_their_branch_and_agree_with_the_oracle(family, siz
     else:
         assert mism == 0, "coverage differs in %d pixels" % mism
         assert rel.max() < 1e-4 and (rel > 2e-5).sum() <= (0 if size == (128, 72) else 8), "depth differs by %.3g" % rel.max()
+    broken, differ, worst, dmax = _colour(view16, inst, W, H, R)
+    print("%s %dx%d: %d colour bytes differ from the float64 ones (by up to %d), worst boundary margin among them %.4f LSB" % (
+        family, W, H, differ, dmax, worst))
+    loose = 0 if size == (128, 72) and family not in scenes.CLIPPED else 3 * 8
+    assert broken <= loose, "%d colour bytes break the rule (%d differ, by up to %d)" % (broken, differ, dmax)
 
 
 def test_reference_takes_window_coordinates_unbounded():
