@@ -214,6 +214,37 @@ int mv_rays_host(mv_handle h, const float **dist, const uint16_t **tag);
 int mv_rays_device(mv_handle h, float **dist, uint16_t **tag);
 int mv_final_rays_host(mv_handle h, const float **dist, const uint16_t **tag);
 int mv_final_rays_device(mv_handle h, float **dist, uint16_t **tag);
+/* Reward components, option "reward_components" (0/1, before the first reset: MV_ERR_STATE after it, MV_ERR_ARG for any other value;
+ * default 0).  The reward is a weighted sum of named shaping rules; these two float32 tensors say which rule paid what.  Both are
+ * [N][MV_REWARD_COMPONENTS]: row env*A + agent, column k = shaping slot k of that env's scenario (mv_reward_component_keys names the slots).
+ *   step rows    the call's reward split by the slot whose weight paid it.  Every term the step kernel adds to an agent's tick reward is
+ *                rt[slot] * ... (rewardAgent, both halves of rewardTeam, the team share other agents receive included); each is also
+ *                added to column `slot` of the agent it is paid to.  Within a tick the terms are summed in the kernel's event order from
+ *                0.0f, across the call the tick sums in tick order from 0.0f; the ticks that count are those the reward counts (the tick
+ *                that ends an episode pays 0).  Column 0 (teamSpirit scales terms, it never pays) is always 0, and so is a slot the
+ *                scenario has a key for but never pays (Collect's collectAbyss).  A Collect agent that falls is paid under
+ *                collectSingleBad, as in the reference.  The columns sum to rewards[view] up to float rounding, not bit for bit.
+ *   episode rows for every view of an env that ended in the call (dones[env] == 1, requested ends included): the column-wise float32
+ *                sum, in call order from 0.0f, of the step rows of every call of the finished episode, the ending call included -- what
+ *                a caller that summed the step rows holds.  Other rows keep the previous finished episode's values (0 before the first).
+ *                The running totals behind them live on the device, one per view and column.
+ * mv_reset and mv_reset_envs write step rows 0 for the envs they restart, zero their running totals and write no episode row.  Inactive
+ * envs (mv_step_envs, mv_step_device_active) get step rows 0 and keep their running totals and episode rows.  With action_repeat, mixed
+ * engines and level sets the rules above hold as stated (each env uses its own scenario's slots).  mv_states_load restores the saved
+ * step's step rows, episode rows and running totals, so a loaded or cloned env's later rows replay bit for bit (the state store carries
+ * them: mv_state_row_bytes grows by 96 * A bytes with the option on).
+ * Delivery follows the state tensors: host-facing calls (mv_step, mv_step_envs, mv_step_begin/end, mv_reset, mv_reset_envs,
+ * mv_states_load) return with both tensors in pinned host memory (mv_reward_components_host); mv_step_device* leaves them in HBM
+ * (mv_reward_components_device) in stream order, and mv_fetch_obs copies them down.  Nothing else changes with the option: every other
+ * output is byte-identical with it on and off.  Memory: 96 B per view in HBM (the running totals included) and 64 B per view pinned;
+ * nothing is allocated while the option is off.  The getters take NULL out pointers; MV_ERR_ARG for a null handle and while the option
+ * is off, MV_ERR_STATE before mv_reset.
+ * mv_reward_component_keys (host-only, no engine): keys8[k] = the shaping key (mv_set_reward_shaping) of slot k in `scenario`, NULL for
+ * slot 0 and for slots the scenario has no key for; strings are static.  MV_ERR_ARG for a null pointer or an unknown scenario. */
+#define MV_REWARD_COMPONENTS 8 /* columns: MV_R_COUNT, the reward-table slots */
+int mv_reward_components_host(mv_handle h, const float **step, const float **episode);
+int mv_reward_components_device(mv_handle h, float **step, float **episode);
+int mv_reward_component_keys(const char *scenario, const char **keys8);
 
 /* MegaverseGym::getRewardShaping / setRewardShaping (megaverse.cpp:214-222).  get: fills up to cap entries, returns the
  * number of keys in *n.  Key strings are owned by the engine. */
@@ -245,6 +276,8 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * "segmentation" (0/1, before the first reset, default 0: the class and index of the drawable behind every pixel, see
  * mv_segmentation_host),
  * "state_tensors" (0/1, before the first reset, default 0: agent, env, object and reward rows beside the frames, see mv_state_tensors_host),
+ * "reward_components" (0/1, before the first reset, default 0: the reward split by shaping slot, per call and per finished episode, see
+ * mv_reward_components_host),
  * "action_repeat" (1..4, before the first reset (MV_ERR_STATE after it, MV_ERR_ARG outside the range), default 1: action repeat, or
  * frame skip, inside the engine.  Every step call (mv_step, mv_step_begin/end, mv_step_device[_ends]) runs up to k physics ticks of
  * 1/15 s per env with the same action masks, then draws once.  Interact acts on the first tick only (it toggles carrying, so one call

@@ -85,6 +85,9 @@ def lib():
         L.mv_level_set_pick.restype = C.c_uint32
         for name in ("mv_state_tensors_host", "mv_state_tensors_device", "mv_final_state_tensors_host", "mv_final_state_tensors_device"):
             getattr(L, name).argtypes = [vp] + [C.POINTER(vp)] * 4
+        for name in ("mv_reward_components_host", "mv_reward_components_device"):
+            getattr(L, name).argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
+        L.mv_reward_component_keys.argtypes = [C.c_char_p, C.POINTER(C.c_char_p)]
         L.mv_draw_cameras.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint32)]
         L.mv_draw_cameras_device.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, vp, C.POINTER(vp)]
         L.mv_level_bounds.argtypes = [vp, vp]
@@ -107,9 +110,21 @@ EXPORTS = [
     "mv_draw_cameras", "mv_draw_cameras_device", "mv_views_device", "mv_level_bounds", "mv_debug_view_order",
     "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms", "mv_debug_cast_rays",
     "mv_debug_kcc", "mv_replace_levels", "mv_level_rows",
+    "mv_reward_components_host", "mv_reward_components_device", "mv_reward_component_keys",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
+R_COUNT = 8  # MV_R_COUNT: reward-table slots, the columns of the reward components
+
+
+def reward_component_keys(scenario):
+    """the shaping key of each reward-component column (slot) of `scenario`: a list of MV_R_COUNT names, None for slot 0 (teamSpirit, which
+    scales terms and never pays) and for slots the scenario has no key for (mv_reward_component_keys)"""
+    out = (C.c_char_p * R_COUNT)()
+    rc = lib().mv_reward_component_keys(scenario.encode(), out)
+    if rc != MV_OK:
+        raise MegaverseError(rc, "unknown scenario %r" % scenario)
+    return [k.decode() if k is not None else None for k in out]
 
 
 class CameraFrames(tuple):
@@ -291,7 +306,8 @@ class Engine:
         ... (state_tensors()), and with option level_set "level_ids" int32[E] (the level each env is on) and
         "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream), and "views"
         float32[N,16] (the last step's view matrices, column-major: chase cameras on the device), and with rays (set_rays) "rays_dist"
-        float32[N,R] / "rays_tag" uint16[N,R] and, with option final_obs too, "final_rays_dist" / "final_rays_tag".  Valid in the engine
+        float32[N,R] / "rays_tag" uint16[N,R] and, with option final_obs too, "final_rays_dist" / "final_rays_tag", and with option
+        reward_components "reward_components" / "episode_reward_components" float32[N,8] (reward_components()).  Valid in the engine
         stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
@@ -303,8 +319,12 @@ class Engine:
         for prefix in ("", "final_"):
             shapes[prefix + "rays_dist"] = ((self.N, self.num_rays), "<f4")
             shapes[prefix + "rays_tag"] = ((self.N, self.num_rays), "<u2")
+        for k in ("reward_components", "episode_reward_components"):
+            shapes[k] = ((self.N, R_COUNT), "<f4")
         shape, typestr = shapes[what]
-        if what.endswith(("rays_dist", "rays_tag")):
+        if what.endswith("reward_components"):
+            ptr = self._rc_ptrs("mv_reward_components_device")[1 if what.startswith("episode_") else 0]
+        elif what.endswith(("rays_dist", "rays_tag")):
             ptr = self._ray_ptrs("mv_%srays_device" % ("final_" if what.startswith("final_") else ""))[0 if what.endswith("dist") else 1]
         elif what.startswith(("state_", "final_state_")):
             ptr = self._state_ptrs("mv_%s_tensors_device" % what.rsplit("_", 1)[0])[what.rsplit("_", 1)[1]]
@@ -401,6 +421,19 @@ class Engine:
     def final_state_tensors(self):
         """options state_tensors and final_obs: the same dict of terminal rows, the state each env's last episode ended on"""
         return self._state_views("mv_final_state_tensors_host")
+
+    def _rc_ptrs(self, fn):
+        step, episode = C.c_void_p(), C.c_void_p()
+        self._ck(getattr(lib(), fn)(self._h, C.byref(step), C.byref(episode)))
+        return step.value, episode.value
+
+    def reward_components(self):
+        """option reward_components: (step float32[N,8], episode float32[N,8]), views of the engine's pinned rows after the last host-facing
+        call (or fetch_obs).  Column k of row env*A + agent is what shaping slot k (reward_component_keys) paid: step, in the last call;
+        episode, over the whole episode of each env that ended in the call (others keep their previous finished episode's)"""
+        n = self.N * R_COUNT * 4
+        return tuple(np.frombuffer((C.c_char * n).from_address(p), dtype=np.float32).reshape(self.N, R_COUNT)
+                     for p in self._rc_ptrs("mv_reward_components_host"))
 
     def set_rays(self, directions, max_distance):
         """ray sensors (mv_set_rays, before the first reset): directions float32[R,3] in camera space (x right, y up, -z forward; rays.fan /

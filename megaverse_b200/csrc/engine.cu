@@ -278,6 +278,7 @@ struct StateStore {
     int rows = 0;
     DevBuf<uint8_t> slabs[kSlabCount];  // same order as mv_engine::envSlabs()
     DevBuf<uint8_t> stateSlabs[4];      // option state_tensors: the live rows of the four state tensors (mv_engine::stateTensor order)
+    DevBuf<uint8_t> rcSlabs[3];         // option reward_components: step rows, episode rows, running totals (mv_engine::rcTensor order)
     struct HostRow {
         bool saved = false;
         std::optional<mv::LevelGenerator> gen;  // the env's level stream; empty with a level set (the bank is the engine's, the pick is in MvEnvState)
@@ -293,6 +294,7 @@ struct StateStore {
 
 static void fillConsts(MvConsts &k, int W, int H);
 static_assert(MV_STATE_OBJECT_ROWS == MV_MAX_OBJECTS && MV_STATE_REWARD_ROWS == MV_MAX_REWARD, "state tensor rows");
+static_assert(MV_REWARD_COMPONENTS == MV_R_COUNT, "reward component columns");
 
 // the frame part of a raster launch: frame size, row bands of bandRows rows, the per-CTA spill slab (one band of the frame per CTA), the
 // triangle-list capacity and the projection of k; the rest is zero (no stats, no ready stamps, no mask, natural order)
@@ -343,6 +345,18 @@ static ViewKernel viewKernelOf(mvr::Items items, bool seg, bool fast) {
         if (seg) return fast ? viewKernel<true, Items::All, true> : viewKernel<false, Items::All, true>;
         return fast ? viewKernel<true> : viewKernel<false>;
     }
+}
+
+// the step kernel variant of a launch: level set, state tensors, reward components
+using StepKernel = void (*)(mvk::StepParams);
+static StepKernel stepKernelOf(bool levelSet, bool state, bool rc) {
+    using mvk::stepKernel;
+    if (rc) {
+        if (levelSet) return state ? stepKernel<true, true, true> : stepKernel<true, false, true>;
+        return state ? stepKernel<false, true, true> : stepKernel<false, false, true>;
+    }
+    if (levelSet) return state ? stepKernel<true, true> : stepKernel<true>;
+    return state ? stepKernel<false, true> : stepKernel<false>;
 }
 
 struct mv_engine {
@@ -578,6 +592,22 @@ struct mv_engine {
         return MV_OK;
     }
 
+    // reward components (option "reward_components", allocated at the first reset): one HBM block of three [N][MV_R_COUNT] tensors -- the
+    // step rows, the episode rows and the running totals of the episodes under way -- written by the step kernel (StepParams::rcStep).  A
+    // host-facing call copies the first two into their pinned twin behind its step; mv_step_device leaves them in HBM (mv_fetch_obs
+    // copies them down).  The running totals never leave the device
+    bool wantRC = false;
+    DevBuf<float> d_rc;
+    PinBuf<float> h_rc;
+    size_t rcFloats() const { return size_t(N) * MV_R_COUNT; }
+    // tensor k (0 step rows, 1 episode rows, 2 running totals) of the block
+    float *rcTensor(float *block, int k) const { return block ? block + size_t(k) * rcFloats() : nullptr; }
+    size_t rcRowBytes() const { return sizeof(float) * MV_R_COUNT * size_t(A); }  // per env and tensor (the state store's slabs)
+    int downloadRC(cudaStream_t s) {
+        if (wantRC) MV_CUDA(cudaMemcpyAsync(h_rc.p, d_rc.p, sizeof(float) * 2 * rcFloats(), cudaMemcpyDeviceToHost, s));
+        return MV_OK;
+    }
+
     // ray sensors (mv_set_rays, allocated at the first reset): dist float[N][R] and tag uint16[N][R] in HBM, each followed with option
     // final_obs by the terminal rays of the same shape.  Every call that draws the step's frames casts them behind its raster launches
     // (castRays); a host-facing call then copies both blocks into their pinned twins on the stream
@@ -784,6 +814,8 @@ struct mv_engine {
         sp.stAgents = stateTensor(st, 0, false); sp.stEnvs = stateTensor(st, 1, false); sp.stObjects = stateTensor(st, 2, false); sp.stRewards = stateTensor(st, 3, false);
         sp.termStAgents = stateTensor(termSt, 0, true); sp.termStEnvs = stateTensor(termSt, 1, true); sp.termStObjects = stateTensor(termSt, 2, true);
         sp.termStRewards = stateTensor(termSt, 3, true);
+        float *rc = wantRC ? d_rc.p : nullptr;
+        sp.rcStep = rcTensor(rc, 0); sp.rcEpisode = rcTensor(rc, 1); sp.rcRun = rcTensor(rc, 2);
         sp.maxObj = std::min(int(MV_MAX_OBJECTS), maxObjSeen.load());
         sp.E = E; sp.A = A; sp.gridCells = gridCells; sp.gridWords = levels.gridWords; sp.forceReset = forceReset ? 1 : 0;
         sp.k = consts;
@@ -793,11 +825,9 @@ struct mv_engine {
     int launchStepKernel(const mvk::StepParams &sp) {
         const int warpsPerBlock = 2;
         const int blocks = (sp.E + warpsPerBlock - 1) / warpsPerBlock;
-        const size_t smem = sizeof(mvk::WarpShared) * warpsPerBlock;
-        if (sp.levelSet && sp.stAgents) mvk::stepKernel<true, true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
-        else if (sp.levelSet) mvk::stepKernel<true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
-        else if (sp.stAgents) mvk::stepKernel<false, true><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
-        else mvk::stepKernel<false><<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        const bool rc = sp.rcStep != nullptr;
+        const size_t smem = (sizeof(mvk::WarpShared) + (rc ? mvk::kRcTickBytes : 0)) * warpsPerBlock;
+        stepKernelOf(sp.levelSet > 0, sp.stAgents != nullptr, rc)<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
         launches += 1;
         return MV_OK;
@@ -1142,6 +1172,7 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
+        if (const int rc = downloadRC(stream)) return rc;
         if (levelSet) {
             MV_CUDA(cudaMemcpyAsync(h_levelIds.p, d_levelIds.p, sizeof(int32_t) * E, cudaMemcpyDeviceToHost, stream));
             publishedCall = stepCalls - 1;  // every call so far is behind this copy
@@ -1296,6 +1327,7 @@ struct mv_engine {
         size_t b = 0;
         for (const EnvSlab &s : envSlabs()) b += s.rowBytes();
         for (int k = 0; k < 4 && wantState; ++k) b += stateRowBytes(k);
+        if (wantRC) b += 3 * rcRowBytes();
         return b;
     }
     int statesCreate(int rows, int *id) {
@@ -1306,6 +1338,8 @@ struct mv_engine {
             if (st->slabs[k].alloc(size_t(rows) * sl[size_t(k)].rowBytes()) != cudaSuccess) { setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
         for (int k = 0; k < 4 && wantState; ++k)
             if (st->stateSlabs[k].alloc(size_t(rows) * stateRowBytes(k)) != cudaSuccess) { setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
+        for (int k = 0; k < 3 && wantRC; ++k)
+            if (st->rcSlabs[k].alloc(size_t(rows) * rcRowBytes()) != cudaSuccess) { setError("mv_states_create: allocation failed"); return MV_ERR_CUDA; }
         st->host.resize(size_t(rows));
         stores.push_back(std::move(st));
         *id = int(stores.size()) - 1;
@@ -1336,14 +1370,18 @@ struct mv_engine {
         MV_CUDA(cudaEventRecord(ev[0], stream));
         MV_CUDA(mvs::copyRows(table, kSlabCount, d_pairs.p, n, stream));
         launches += 1;
-        if (wantState) {  // the state-tensor rows: a second launch of the same kernel, so that its table keeps its size
-            mvs::Slab stTable[4];
-            for (int k = 0; k < 4; ++k) {
-                uint8_t *eng = reinterpret_cast<uint8_t *>(stateTensor(d_state.p, k, false)), *sto = st.stateSlabs[k].p;
-                const size_t rb = stateRowBytes(k);
-                stTable[k] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
-            }
-            MV_CUDA(mvs::copyRows(stTable, 4, d_pairs.p, n, stream));
+        // the rows of the options' tensors (state tensors, reward components): a second launch of the same kernel, so that the first table
+        // keeps its size
+        mvs::Slab optTable[7];
+        int nOpt = 0;
+        auto optSlab = [&](float *engRows, uint8_t *sto, size_t rb) {
+            uint8_t *eng = reinterpret_cast<uint8_t *>(engRows);
+            optTable[nOpt++] = mvs::Slab{toStore ? eng : sto, toStore ? sto : eng, rb, rb, rb};
+        };
+        for (int k = 0; k < 4 && wantState; ++k) optSlab(stateTensor(d_state.p, k, false), st.stateSlabs[k].p, stateRowBytes(k));
+        for (int k = 0; k < 3 && wantRC; ++k) optSlab(rcTensor(d_rc.p, k), st.rcSlabs[k].p, rcRowBytes());
+        if (nOpt) {
+            MV_CUDA(mvs::copyRows(optTable, nOpt, d_pairs.p, n, stream));
             launches += 1;
         }
         if (toStore) return endTimes(Timed::FirstOnly);
@@ -1597,10 +1635,12 @@ cudaError_t uploadPalette() {
 }
 
 int setKernelAttrs(mv_engine *h) {
-    cudaError_t err = cudaFuncSetAttribute(mvk::stepKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(mvk::stepKernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(mvk::WarpShared) * 4));
+    cudaError_t err = cudaSuccess;
+    for (int v = 0; v < 8 && err == cudaSuccess; ++v) {
+        const bool rc = v >= 4;
+        const int smem = int((sizeof(mvk::WarpShared) + (rc ? mvk::kRcTickBytes : 0)) * 4);
+        err = cudaFuncSetAttribute(reinterpret_cast<const void *>(stepKernelOf(v & 1, v & 2, rc)), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    }
     if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
     return MV_OK;
 }
@@ -1793,6 +1833,12 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         h->wantState = value != 0;
         return MV_OK;
     }
+    if (k == "reward_components") {  // the reward split by shaping slot, per call and per finished episode (see the header); allocated by the first reset
+        if (h->didReset) { h->setError("option reward_components must be set before the first reset"); return MV_ERR_STATE; }
+        if (value != 0 && value != 1) { h->setError("reward_components must be 0 or 1"); return MV_ERR_ARG; }
+        h->wantRC = value != 0;
+        return MV_OK;
+    }
     if (k == "action_repeat") {  // physics ticks per step call (see the header); the state store keeps no copy: it belongs to the engine
         if (h->didReset) { h->setError("option action_repeat must be set before the first reset"); return MV_ERR_STATE; }
         if (value < 1 || value > 4) { h->setError("action_repeat out of range [1,4]"); return MV_ERR_ARG; }
@@ -1933,6 +1979,14 @@ int mv_reset(mv_handle h) {
                 return MV_ERR_CUDA;
             }
             std::memset(h->h_state.p, 0, sizeof(float) * n);
+        }
+        if (h->wantRC) {  // step rows, episode rows, running totals: zero until written
+            const size_t n = h->rcFloats();
+            if (h->d_rc.alloc(3 * n) != cudaSuccess || h->h_rc.alloc(2 * n) != cudaSuccess || cudaMemset(h->d_rc.p, 0, sizeof(float) * 3 * n) != cudaSuccess) {
+                h->setError("reward_components: allocation failed");
+                return MV_ERR_CUDA;
+            }
+            std::memset(h->h_rc.p, 0, sizeof(float) * 2 * n);
         }
         if (h->nRays) {  // the fan, and the live and terminal rays: zero until cast
             const size_t n = h->rayBlock();
@@ -2314,6 +2368,8 @@ int mv_fetch_obs(mv_handle h) {
     }
     // the rays (live and terminal): always current in HBM
     if (h->nRays && h->didReset && h->downloadRays(h->stream) != MV_OK) { h->setError("ray download failed"); return MV_ERR_CUDA; }
+    // the reward components (step and episode rows): always current in HBM
+    if (h->wantRC && h->didReset && h->downloadRC(h->stream) != MV_OK) { h->setError("reward component download failed"); return MV_ERR_CUDA; }
     // after a zero-copy host-facing step the host buffer holds the newer frames: no copy.  Rows copied from a caller's tensor are not the
     // engine's to vouch for: the next step with an active set draws every view again
     if (h->deviceObsFresh) {
@@ -2422,6 +2478,30 @@ int mv_final_state_tensors_device(mv_handle h, float **agents, float **envs, flo
     const int rc = stateTensorCall(h, true, "mv_final_state_tensors_device");
     if (rc == MV_OK) stateTensorOuts(h, h->d_state.p, true, agents, envs, objects, rewards);
     return rc;
+}
+// option reward_components is on and the engine reset
+static int rewardComponentCall(mv_handle h, const char *fn) {
+    if (!h) return MV_ERR_ARG;
+    if (!h->wantRC) { h->setError(std::string(fn) + ": option reward_components is off"); return MV_ERR_ARG; }
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+int mv_reward_components_host(mv_handle h, const float **step, const float **episode) {
+    const int rc = rewardComponentCall(h, "mv_reward_components_host");
+    if (rc == MV_OK) { if (step) *step = h->rcTensor(h->h_rc.p, 0); if (episode) *episode = h->rcTensor(h->h_rc.p, 1); }
+    return rc;
+}
+int mv_reward_components_device(mv_handle h, float **step, float **episode) {
+    const int rc = rewardComponentCall(h, "mv_reward_components_device");
+    if (rc == MV_OK) { if (step) *step = h->rcTensor(h->d_rc.p, 0); if (episode) *episode = h->rcTensor(h->d_rc.p, 1); }
+    return rc;
+}
+int mv_reward_component_keys(const char *scenario, const char **keys8) {
+    if (!scenario || !keys8) return MV_ERR_ARG;
+    const int sc = mv::scenarioFromName(scenario);
+    if (sc < 0) return MV_ERR_ARG;
+    for (int k = 0; k < MV_R_COUNT; ++k) keys8[k] = mv::rewardKey(sc, k);
+    return MV_OK;
 }
 int mv_set_rays(mv_handle h, const float *dirs3, int n, float max_dist) {
     if (!h) return MV_ERR_ARG;

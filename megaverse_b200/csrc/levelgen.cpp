@@ -221,40 +221,43 @@ std::vector<std::pair<std::string, float>> defaultRewardShaping(const std::strin
     return {};
 }
 
+// the shaping keys of every scenario and the reward-table slot (MV_R_*) each one fills; teamSpirit (slot 0) is every scenario's
+namespace {
+struct RewardSlotKey { int scenario; int slot; const char *key; };
+const RewardSlotKey kRewardSlots[] = {
+    {MV_SCENARIO_TOWER, MV_R_TOWER_PICKED_UP, "towerPickedUpObject"},
+    {MV_SCENARIO_TOWER, MV_R_TOWER_VISITED_BZ, "towerVisitedBuildingZoneWithObject"},
+    {MV_SCENARIO_TOWER, MV_R_TOWER_BUILDING, "towerBuildingReward"},
+    {MV_SCENARIO_COLLECT, MV_R_COLLECT_GOOD, "collectSingleGood"},
+    {MV_SCENARIO_COLLECT, MV_R_COLLECT_BAD, "collectSingleBad"},
+    {MV_SCENARIO_COLLECT, MV_R_COLLECT_ALL, "collectAll"},
+    {MV_SCENARIO_COLLECT, MV_R_COLLECT_ABYSS, "collectAbyss"},
+    {MV_SCENARIO_OBSTACLES, MV_R_OBST_AGENT_AT_EXIT, "obstaclesAgentAtExit"},
+    {MV_SCENARIO_OBSTACLES, MV_R_OBST_ALL_AT_EXIT, "obstaclesAllAgentsAtExit"},
+    {MV_SCENARIO_OBSTACLES, MV_R_OBST_EXTRA, "obstaclesExtraReward"},
+    {MV_SCENARIO_OBSTACLES, MV_R_OBST_CARRIED_TO_EXIT, "obstaclesAgentCarriedObjectToExit"},
+    {MV_SCENARIO_HEX_EXPLORE, MV_R_EXPLORE_SOLVED, "exploreSolved"},
+    {MV_SCENARIO_HEX_MEMORY, MV_R_MEMORY_GOOD, "memoryCollectGood"},
+    {MV_SCENARIO_HEX_MEMORY, MV_R_MEMORY_BAD, "memoryCollectBad"},
+    {MV_SCENARIO_SOKOBAN, MV_R_SOKOBAN_ON_TARGET, "sokobanBoxOnTarget"},
+    {MV_SCENARIO_SOKOBAN, MV_R_SOKOBAN_LEAVES_TARGET, "sokobanBoxLeavesTarget"},
+    {MV_SCENARIO_SOKOBAN, MV_R_SOKOBAN_ALL, "sokobanAllBoxesOnTarget"},
+    {MV_SCENARIO_REARRANGE, MV_R_REARRANGE_ONE_MORE, "rearrangeOneMoreObjectCorrectPosition"},
+    {MV_SCENARIO_REARRANGE, MV_R_REARRANGE_ALL, "rearrangeAllObjectsCorrectPosition"},
+};
+}  // namespace
+
 int rewardSlot(int scenario, const std::string &key) {
     if (key == "teamSpirit") return MV_R_TEAM_SPIRIT;
-    if (scenario == MV_SCENARIO_TOWER) {
-        if (key == "towerPickedUpObject") return MV_R_TOWER_PICKED_UP;
-        if (key == "towerVisitedBuildingZoneWithObject") return MV_R_TOWER_VISITED_BZ;
-        if (key == "towerBuildingReward") return MV_R_TOWER_BUILDING;
-    }
-    if (scenario == MV_SCENARIO_COLLECT) {
-        if (key == "collectSingleGood") return MV_R_COLLECT_GOOD;
-        if (key == "collectSingleBad") return MV_R_COLLECT_BAD;
-        if (key == "collectAll") return MV_R_COLLECT_ALL;
-        if (key == "collectAbyss") return MV_R_COLLECT_ABYSS;
-    }
-    if (scenario == MV_SCENARIO_OBSTACLES) {
-        if (key == "obstaclesAgentAtExit") return MV_R_OBST_AGENT_AT_EXIT;
-        if (key == "obstaclesAllAgentsAtExit") return MV_R_OBST_ALL_AT_EXIT;
-        if (key == "obstaclesExtraReward") return MV_R_OBST_EXTRA;
-        if (key == "obstaclesAgentCarriedObjectToExit") return MV_R_OBST_CARRIED_TO_EXIT;
-    }
-    if (scenario == MV_SCENARIO_HEX_EXPLORE && key == "exploreSolved") return MV_R_EXPLORE_SOLVED;
-    if (scenario == MV_SCENARIO_HEX_MEMORY) {
-        if (key == "memoryCollectGood") return MV_R_MEMORY_GOOD;
-        if (key == "memoryCollectBad") return MV_R_MEMORY_BAD;
-    }
-    if (scenario == MV_SCENARIO_SOKOBAN) {
-        if (key == "sokobanBoxOnTarget") return MV_R_SOKOBAN_ON_TARGET;
-        if (key == "sokobanBoxLeavesTarget") return MV_R_SOKOBAN_LEAVES_TARGET;
-        if (key == "sokobanAllBoxesOnTarget") return MV_R_SOKOBAN_ALL;
-    }
-    if (scenario == MV_SCENARIO_REARRANGE) {
-        if (key == "rearrangeOneMoreObjectCorrectPosition") return MV_R_REARRANGE_ONE_MORE;
-        if (key == "rearrangeAllObjectsCorrectPosition") return MV_R_REARRANGE_ALL;
-    }
+    for (const RewardSlotKey &r : kRewardSlots)
+        if (r.scenario == scenario && key == r.key) return r.slot;
     return -1;
+}
+
+const char *rewardKey(int scenario, int slot) {
+    for (const RewardSlotKey &r : kRewardSlots)
+        if (r.scenario == scenario && r.slot == slot) return r.key;
+    return nullptr;
 }
 
 std::vector<uint32_t> colorTables() {

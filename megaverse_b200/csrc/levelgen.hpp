@@ -76,5 +76,6 @@ std::vector<uint32_t> colorTables();
 int gridCapacity(int scenario);
 int decoCapacity(int scenario);  // most decorations a level of the scenario can hold  // dense voxel grid capacity in cells
 int rewardSlot(int scenario, const std::string &key);  // -1 if unknown
+const char *rewardKey(int scenario, int slot);         // the inverse for slots 1.. (nullptr: teamSpirit's slot 0, or no key of the scenario)
 
 }  // namespace mv

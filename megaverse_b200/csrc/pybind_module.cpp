@@ -286,6 +286,13 @@ public:
         d["rewards"] = py::array_t<float>({numEnvs_, MV_STATE_REWARD_ROWS, 4}, p[3], py::none{});
         return d;
     }
+    // (extension, option "reward_components") float32 [N,8] views of the engine's pinned step rows, or episode rows (layout in the header)
+    py::array_t<float> getRewardComponents(bool episode) {
+        alive();
+        const float *step, *ep;
+        check(mv_reward_components_host(h__, &step, &ep));
+        return py::array_t<float>({int(masks_.size()), int(MV_REWARD_COMPONENTS)}, episode ? ep : step, py::none{});
+    }
     // (extension) ray sensors (mv_set_rays): directions float32 [R,3] in camera space, before the first reset
     void setRays(py::array_t<float, py::array::c_style | py::array::forcecast> dirs, float maxDist) {
         alive();
@@ -382,6 +389,16 @@ private:
 PYBIND11_MODULE(megaverse, m) {
     m.doc() = "megaverse_b200 Python bindings (MegaverseGym surface of the reference)";
     m.def("set_megaverse_log_level", &setMegaverseLogLevel, "Megaverse Log Level (0 to disable all logs, 2 for warnings");
+    m.def(
+        "reward_component_keys",
+        [](const std::string &scenario) {
+            const char *keys[MV_REWARD_COMPONENTS];
+            if (mv_reward_component_keys(scenario.c_str(), keys) != MV_OK) throw std::invalid_argument("unknown scenario " + scenario);
+            py::list out;
+            for (const char *k : keys) out.append(k ? py::object(py::str(k)) : py::object(py::none()));
+            return out;
+        },
+        py::arg("scenario"), "(extension) the shaping key of each reward-component column of a scenario, None for slot 0 and unused slots");
     py::class_<MegaverseGym>(m, "MegaverseGym")
         .def(py::init<const std::string &, int, int, int, int, int, bool, const std::map<std::string, float> &>())
         .def(py::init<const std::vector<std::string> &, int, int, int, int, int, bool, const std::map<std::string, float> &>())
@@ -435,6 +452,10 @@ PYBIND11_MODULE(megaverse, m) {
              "(dist float32 [N,R], tag uint16 [N,R]): distance to the first front face along each ray (0: none) and its MV_SEG_* << 8 | index")
         .def("get_final_rays", [](MegaverseGym &g) { return g.getRays(true); },
              "the terminal rays (rays and option final_obs): cast from the scene each env's last episode ended on, same pair")
+        .def("get_reward_components", [](MegaverseGym &g) { return g.getRewardComponents(false); },
+             "float32 [N,8] view (option reward_components): the last call's reward split by the shaping slot that paid it")
+        .def("get_episode_reward_components", [](MegaverseGym &g) { return g.getRewardComponents(true); },
+             "float32 [N,8] view (option reward_components): the per-slot totals of each env's last finished episode")
         .def("get_final_state_tensors", [](MegaverseGym &g) { return g.getStateTensors(true); },
              "the terminal rows (options state_tensors and final_obs): the state each env's last episode ended on, same dict")
         .def("step_envs", &MegaverseGym::stepEnvs, py::arg("envs"),

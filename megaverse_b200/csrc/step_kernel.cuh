@@ -103,7 +103,15 @@ struct StepParams {
     // level set: [levelSet * banks] 0 for a row being replaced (mv_replace_levels), which no flip may land on; the host keeps at least one
     // row of every bank pickable.  Last, so that no other field moves
     const uint8_t *rowPickable;
+    // option "reward_components" (nullptr: off; the stepKernel<.., .., true> variants only), each [E*A][MV_R_COUNT]: the call's reward split
+    // by the shaping slot whose weight paid it, the totals of the episodes that ended in the call, and the running totals of the episodes
+    // under way (include/megaverse_b200.h has the rules)
+    float *rcStep, *rcEpisode, *rcRun;
 };
+
+// option "reward_components": per warp, after the block's WarpShared records, one agent's tick columns per row -- what each shaping slot
+// paid the agent this tick, [tick] like WarpShared::lastReward.  Only the stepKernel<.., .., true> variants are launched with this space
+constexpr size_t kRcTickBytes = sizeof(float) * MV_MAX_AGENTS * MV_R_COUNT;
 
 // row of the level arrays that holds slot `slot` of env `env`: the env's own ring of slots, or, with a level set, the bank row itself
 template <bool kLevelSet> __device__ __forceinline__ size_t levelRow(const StepParams &P, int env, int slot) {
@@ -1048,9 +1056,10 @@ __device__ void writeStateRows(const WarpShared &S, const MvLevel &L, const MvIn
 
 // ---------------------------------------------------------------- the kernel
 // kLevelSet: the level-set variant (StepParams::levelSet > 0).  A template parameter, not a run-time branch, so that the default
-// variant is the code it was before level sets existed.  kState: the state-tensor variant (StepParams::stAgents set), a template
-// parameter for the same reason
-template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
+// variant is the code it was before level sets existed.  kState: the state-tensor variant (StepParams::stAgents set), kRC: the
+// reward-component variant (StepParams::rcStep set, launched with kRcTickBytes more shared memory per warp), template parameters for the
+// same reason
+template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     extern __shared__ __align__(128) unsigned char smemRaw[];
     const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slotInGrid = blockIdx.x * (blockDim.x >> 5) + warpInBlock;
@@ -1066,6 +1075,8 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
             P.rewards[idx] = 0.0f;
             if (P.hostRewards) { P.hostRewards[idx] = 0.0f; P.hostTrueObjectives[idx] = P.trueObjectives[idx]; }
         }
+        if (kRC)  // step rows 0; the running and episode totals are left alone
+            for (int i = lane; i < P.A * MV_R_COUNT; i += 32) P.rcStep[size_t(env) * P.A * MV_R_COUNT + i] = 0.0f;
         __syncwarp();
         if (lane == 0) {
             P.dones[env] = 0;
@@ -1117,6 +1128,9 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
     bool doneFlag = false;
     // lane i < A: agent i's reward summed over the call's ticks, in tick order from 0 (the tick that ends the episode pays 0, as one step does)
     float rewardSum = 0.0f;
+    // kRC: this warp's tick columns, [agent][slot]; lane l folds entries l and l + 32 into rcCall by the rewardSum rule
+    float *rcTick = kRC ? reinterpret_cast<float *>(smemRaw + sizeof(WarpShared) * (blockDim.x >> 5) + kRcTickBytes * warpInBlock) : nullptr;
+    float rcCall[2] = {0.0f, 0.0f};
     MV_PROBE(0);  // state staged
 
     if (!P.forceReset) {
@@ -1128,6 +1142,8 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
         // row, flip, write-back, instance list) sees the state of the tick that ended it, or of the last tick.
         for (int tick = 0; tick < P.repeat; ++tick) {
             for (int i = lane; i < MV_MAX_AGENTS; i += 32) S.lastReward[i] = 0.0f;
+            if (kRC)
+                for (int i = lane; i < MV_MAX_AGENTS * MV_R_COUNT; i += 32) rcTick[i] = 0.0f;
             if (lane == 0) S.memoryNear = 0u;
             __syncwarp();
 
@@ -1245,10 +1261,15 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
             if (lane == 0) {
                 MvEnvState &e = S.env;
                 const float *rt = P.rtable + size_t(env) * A * MV_R_COUNT;
-                auto rewardAgent = [&](int slotR, int ai, float mult) { S.lastReward[ai] += rt[ai * MV_R_COUNT + slotR] * mult; };
+                // every term paid is also added, with kRC, to the paying slot's tick column of the agent it is paid to
+                auto pay = [&](int slotR, int ai, float v) {
+                    S.lastReward[ai] += v;
+                    if (kRC) rcTick[ai * MV_R_COUNT + slotR] += v;
+                };
+                auto rewardAgent = [&](int slotR, int ai, float mult) { pay(slotR, ai, rt[ai * MV_R_COUNT + slotR] * mult); };
                 auto rewardTeam = [&](int slotR, int ai, float mult) {
                     rewardAgent(slotR, ai, mult * (1 - rt[ai * MV_R_COUNT + MV_R_TEAM_SPIRIT]));
-                    for (int j = 0; j < A; ++j) S.lastReward[j] += rt[j * MV_R_COUNT + slotR] * rt[j * MV_R_COUNT + MV_R_TEAM_SPIRIT] * mult / A;
+                    for (int j = 0; j < A; ++j) pay(slotR, j, rt[j * MV_R_COUNT + slotR] * rt[j * MV_R_COUNT + MV_R_TEAM_SPIRIT] * mult / A);
                 };
                 const float carryingScale = 0.78f, carryingScaleInverse = 1.0f / carryingScale;
                 // RearrangeScenario::checkDone / countMatchingObjects (scenario_rearrange.cpp:134-177)
@@ -1570,6 +1591,7 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
             doneFlag = S.doneFlag != 0;
             if (doneFlag) break;
             if (lane < A) rewardSum += S.lastReward[lane];
+            if (kRC) { rcCall[0] += rcTick[lane]; rcCall[1] += rcTick[lane + 32]; }
         }
         resetNow = doneFlag;
         MV_PROBE(5);  // scenario logic
@@ -1585,6 +1607,25 @@ template <bool kLevelSet, bool kState = false> __global__ void __launch_bounds__
         const float r = P.forceReset ? 0.0f : rewardSum;  // i == lane: A <= MV_MAX_AGENTS < 32
         P.rewards[idx] = r;
         if (P.hostRewards) { P.hostRewards[idx] = r; P.hostTrueObjectives[idx] = to; }
+    }
+    if (kRC) {  // the step rows; the running totals take them in call order, and an end moves its total to the episode rows
+        const size_t base = size_t(env) * A * MV_R_COUNT;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const int i = lane + 32 * k;
+            if (i < A * MV_R_COUNT) {
+                const float s = P.forceReset ? 0.0f : rcCall[k];
+                P.rcStep[base + i] = s;
+                if (P.forceReset) {
+                    P.rcRun[base + i] = 0.0f;
+                } else if (doneFlag) {
+                    P.rcEpisode[base + i] = P.rcRun[base + i] + s;
+                    P.rcRun[base + i] = 0.0f;
+                } else {
+                    P.rcRun[base + i] += s;
+                }
+            }
+        }
     }
     if (lane == 0) {
         const uint8_t dn = (!P.forceReset && doneFlag) ? 1 : 0;

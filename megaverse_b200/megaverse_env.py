@@ -9,7 +9,7 @@ from .cameras import chase_views, overview_views
 from .gym_shim import Box, Discrete, Env, Tuple
 
 # the product fails loudly when its native extension is missing
-from .extension.megaverse import MegaverseGym, set_megaverse_log_level  # noqa: E402
+from .extension.megaverse import MegaverseGym, reward_component_keys, set_megaverse_log_level  # noqa: E402
 
 MEGAVERSE8 = ['TowerBuilding', 'ObstaclesEasy', 'ObstaclesHard', 'Collect', 'Sokoban', 'HexMemory', 'HexExplore', 'Rearrange']
 OBSTACLES_MULTITASK = ['ObstaclesWalls', 'ObstaclesSteps', 'ObstaclesLava', 'ObstaclesEasy', 'ObstaclesHard']
@@ -72,7 +72,7 @@ class MegaverseEnv(Env):
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
                  action_repeat=1, segmentation=False, num_levels=None, start_level=0, state_tensors=False,
-                 ray_directions=None, ray_max_distance=120.0):
+                 ray_directions=None, ray_max_distance=120.0, reward_components=False):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
@@ -90,6 +90,9 @@ class MegaverseEnv(Env):
         # every agent casts these rays against its env's drawn scene, up to ray_max_distance; ray_observations() gives each ray's hit
         # distance and segmentation tag, and with final_observation=True the infos of done agents carry 'final_rays', the agent's rays
         # cast from the scene the episode ended on.  step()'s return values do not change
+        # (extension) reward_components=True: reward_components() gives, per agent, what each shaping rule paid in the last step (columns
+        # named by reward_component_keys()), and the infos of done agents carry 'reward_components', {key: the agent's total under that key
+        # over the finished episode} (option "reward_components").  step()'s return values do not change
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -134,6 +137,9 @@ class MegaverseEnv(Env):
             dirs = np.ascontiguousarray(ray_directions, dtype=np.float32).reshape(-1, 3)
             self.env.set_rays(dirs, float(ray_max_distance))
             self.num_rays = len(dirs)
+        self.reward_components_enabled = bool(reward_components)
+        if self.reward_components_enabled:
+            self.env.set_option("reward_components", 1)
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
         self.num_levels = None if num_levels is None else int(num_levels)
@@ -185,6 +191,17 @@ class MegaverseEnv(Env):
         distance along each ray to the first front face it meets (0: none within ray_max_distance) and that drawable's MV_SEG_* class << 8 |
         index (0: none).  Views of engine memory, valid until the next step."""
         return self.env.get_rays()
+
+    def reward_components(self):
+        """(extension, reward_components=True) float32 [num_agents, 8]: column k of row i is what shaping slot k paid agent i in the last step
+        (reward_component_keys(i) names the columns); the row sums to the agent's reward up to float rounding.  A view of engine memory,
+        valid until the next step."""
+        return self.env.get_reward_components()
+
+    def reward_component_keys(self, actor_idx):
+        """the shaping key of each column of reward_components() for agent actor_idx's scenario: 8 entries, None for column 0 (teamSpirit
+        scales the other terms and pays nothing itself) and for columns the scenario does not use"""
+        return reward_component_keys(self.scenarios[actor_idx // self.num_agents_per_env])
 
     def check_faults(self):
         """raise if the engine latched a fault bit (one pinned-memory read, no device round trip)"""
@@ -269,6 +286,7 @@ class MegaverseEnv(Env):
             final = self.env.get_final_observations()
             final_state = self.env.get_final_state_tensors()['agents'] if self.state_tensors_enabled else None
             final_rays = self.env.get_final_rays() if self.num_rays else None
+        episode_components = self.env.get_episode_reward_components() if self.reward_components_enabled else None
         dones, infos = [], []
         for env_i in range(self.num_envs):
             done = bool(env_dones[env_i])
@@ -278,6 +296,11 @@ class MegaverseEnv(Env):
                 if self.num_levels is not None:
                     for j in range(self.num_agents_per_env):
                         infos[env_i * self.num_agents_per_env + j]['level'] = self._levels_played[env_i]
+                if episode_components is not None:
+                    keys = reward_component_keys(self.scenarios[env_i])
+                    for j in range(self.num_agents_per_env):
+                        view = env_i * self.num_agents_per_env + j
+                        infos[view]['reward_components'] = {k: float(episode_components[view, c]) for c, k in enumerate(keys) if k is not None}
                 if self.final_observation:
                     for j in range(self.num_agents_per_env):
                         view = env_i * self.num_agents_per_env + j
