@@ -323,6 +323,26 @@ int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_en
 /* mv_step_device_ends with an active set (see mv_step_envs for what an inactive env does and reports): d_active = uint8[num_envs] in DEVICE
  * memory, read in the engine stream's order; non-zero means active.  d_active == NULL is mv_step_device_ends: the same kernels and launches. */
 int mv_step_device_active(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends, const uint8_t *d_active);
+/* Stream steps: mv_step_device_active enqueued on the caller's CUDA stream (cudaStream_t; NULL = the engine stream, mv_stream) as device
+ * work only, so that the call may be captured into a CUDA graph (cudaStreamBeginCapture, torch.cuda.graph) beside the caller's own
+ * work, and every replay of the graph takes the steps again.  The same kernels as mv_step_device_active: the step kernel, the raster
+ * launch (a programmatic dependent with option "overlap"), and the terminal frames and rays when their options are on; the engine
+ * stream is forked from `stream` and joined back to it (event, wait, work, event, wait).  No host copy, no timing event, no host wait,
+ * no level work.  With d_active every view is drawn (the frames of inactive envs are drawn again, the same bytes).  Results go to the
+ * device arrays only (mv_*_device); mv_fault_word still sees the fault bits.
+ * NULL cannot name the legacy default stream (handle 0, e.g. PyTorch's default stream): pass cudaStreamLegacy (or cudaStreamPerThread)
+ * for it.  Given NULL, the step is ordered only on the engine stream, and nothing orders it against work the caller put on another stream.
+ * MV_ERR_STATE without option "level_set" (an episode end must need no host work), before mv_reset, with an mv_step_begin outstanding,
+ * with mv_replace_levels requests pending, and inside a capture when mv_set_reward_shaping changed the table since the last step.
+ * Stream mode: from the first stream step until mv_close.  The host cannot see graph replays, so every other entry point but the pointer
+ * getters (mv_*_device, mv_stream, mv_*_host) becomes a synchronisation point: it waits for the whole device (cudaDeviceSynchronize),
+ * refreshes the host mirrors from HBM (level ids, episode counters, rewards, dones, reasons, true objectives) and waits for its own
+ * device work before it returns -- mv_step_device* then return after their step, and mv_set_next_levels and mv_set_reward_shaping
+ * upload at once.  Call none of them while a capture is under way.  Refused in stream mode (MV_ERR_STATE): mv_replace_levels, options
+ * "tri_cap" and "raster_bands", mv_debug_step_profile and mv_debug_raster_stats, which reallocate what a captured launch refers to.  A
+ * graph keeps the pointers of its capture: mv_set_obs_buffer and option "raster_grid" apply to steps captured after them.  Engines that
+ * never take a stream step behave and cost exactly as before. */
+int mv_step_stream(mv_handle h, void *stream, const int32_t *d_masks, const uint8_t *d_ends, const uint8_t *d_active);
 /* Restart chosen envs now: envs[i] start a new episode.  seeds == NULL: each continues its own level stream (it takes its pre-staged
  * next level, as at a natural episode end); else env envs[i] is first reseeded with seeds[i] and plays the first level of that stream --
  * it then behaves exactly as env envs[i] of a fresh engine after mv_seed_env and mv_reset (unlike mv_seed_env, a Sokoban env also drops

@@ -16,6 +16,7 @@ MV_END_NONE, MV_END_TIME, MV_END_SOLVED, MV_END_REQUESTED = 0, 1, 2, 3  # done_r
 MV_SEG_NONE, MV_SEG_STATIC, MV_SEG_TERRAIN, MV_SEG_OBJECT, MV_SEG_AGENT, MV_SEG_REWARD = 0, 1, 2, 3, 4, 5
 MAX_OBJECTS, MAX_AGENTS, MAX_CAND = 128, 8, 96  # MV_MAX_OBJECTS, MV_MAX_AGENTS, MV_MAX_CAND (csrc/mv_types.h)
 MV_FAULT_ENVELOPE, MV_FAULT_CAND_OVERFLOW = 16, 32
+CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: the legacy default stream, which a null cudaStream_t cannot name where NULL means something else
 
 
 class MegaverseError(RuntimeError):
@@ -44,6 +45,7 @@ def lib():
         L.mv_step_device.argtypes = [vp, vp]
         L.mv_step_device_ends.argtypes = [vp, vp, vp]
         L.mv_step_device_active.argtypes = [vp, vp, vp, vp]
+        L.mv_step_stream.argtypes = [vp, vp, vp, vp, vp]
         L.mv_step_envs.argtypes = [vp, vp, ci]
         L.mv_reset_envs.argtypes = [vp, vp, vp, ci]
         for name in ("mv_obs_host", "mv_depth_host", "mv_rewards", "mv_dones", "mv_true_objectives", "mv_actions_device", "mv_obs_device",
@@ -111,6 +113,7 @@ EXPORTS = [
     "mv_set_rays", "mv_rays_host", "mv_rays_device", "mv_final_rays_host", "mv_final_rays_device", "mv_last_rays_ms", "mv_debug_cast_rays",
     "mv_debug_kcc", "mv_replace_levels", "mv_level_rows",
     "mv_reward_components_host", "mv_reward_components_device", "mv_reward_component_keys",
+    "mv_step_stream",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -232,6 +235,34 @@ class Engine:
         pointer is the engine's own actions, no end requests, every env active"""
         p = [C.c_void_p(x) if x else None for x in (d_masks_ptr, d_ends_ptr, d_active_ptr)]
         self._ck(lib().mv_step_device_active(self._h, *p))
+
+    def step_stream(self, stream_ptr=None, d_masks_ptr=None, d_ends_ptr=None, d_active_ptr=None):
+        """step_device_active() enqueued on the caller's CUDA stream (stream_ptr, a cudaStream_t such as torch.cuda.current_stream().cuda_stream)
+        as device work only, so that a CUDA graph may capture it (mv_step_stream).  stream_ptr 0 is the legacy default stream (PyTorch's
+        default stream), passed on as cudaStreamLegacy; None is the engine stream alone, ordered against no stream of the caller's.  Needs
+        option level_set and a reset; from the first call on every other method but the device pointers is a synchronisation point.
+        Results are in the device arrays (device_array).  A policy and T steps as one graph launch, with actions encoded on the device (helpers.encode's bit layout):
+
+            obs = torch.as_tensor(eng.device_array("obs"), device="cuda")
+            rewards = torch.as_tensor(eng.device_array("rewards"), device="cuda")
+            offsets = torch.tensor([0, 2, 4, 6, 7, 8], dtype=torch.int32, device="cuda")  # head i's choice c > 0 sets bit offsets[i] + c
+            masks = torch.zeros((T, eng.N), dtype=torch.int32, device="cuda")
+            ret = torch.zeros((T, eng.N), device="cuda")
+            eng.step_stream(torch.cuda.current_stream().cuda_stream)  # one eager step first: warms up, uploads a changed reward table
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                s = torch.cuda.current_stream().cuda_stream
+                for t in range(T):
+                    heads = policy(obs)                    # int64 [N, 6]: one choice per action head, 0 = none
+                    masks[t] = ((heads > 0).to(torch.int32) << (heads.to(torch.int32) + offsets)).sum(1, dtype=torch.int32)
+                    eng.step_stream(s, masks[t].data_ptr())
+                    ret[t].copy_(rewards)
+            g.replay()                                     # T policy evaluations and T steps, one launch
+
+        Capture after every option is set, and call no other engine method inside the capture."""
+        stream = None if stream_ptr is None else C.c_void_p(stream_ptr or CUDA_STREAM_LEGACY)
+        p = [C.c_void_p(x) if x else None for x in (d_masks_ptr, d_ends_ptr, d_active_ptr)]
+        self._ck(lib().mv_step_stream(self._h, stream, *p))
 
     def reset_envs(self, envs, seeds=None):
         """envs[i] start a new episode now; with seeds, env envs[i] is reseeded with seeds[i] first (mv_reset_envs).  With option level_set,

@@ -400,6 +400,10 @@ struct mv_engine {
     MvConsts consts{};
 
     CudaStream stream;
+    // stream steps (mv_step_stream): the fork from the caller's stream onto the engine stream and the join back; stream mode from the
+    // first one until mv_close (every other entry point is then a synchronisation point, see streamSync)
+    CudaEvent evFork, evJoin;
+    bool streamMode = false;
     // kernel times of the last timed call, read by readKernelTimes only.  The call records ev[0] before its first kernel, ev[1] after it
     // when its raster launch is serialised behind it, evFinal before a terminal-frame launch and ev[2] at the end
     CudaEvent ev[3];
@@ -470,8 +474,9 @@ struct mv_engine {
     uint8_t *obsOut = nullptr;     // where the rasteriser writes in HBM: d_obs, or the caller's tensor slice (mv_set_obs_buffer)
     float *depthOut = nullptr;
     DevBuf<int32_t> d_faults;
-    // rasteriser (raster_view.cuh): a persistent grid of CTAs pulling (view, band) items from a never-reset counter
-    DevBuf<uint32_t> d_workCounter;
+    // rasteriser (raster_view.cuh): a persistent grid of CTAs pulling (view, band) items from a counter that host-path calls never reset
+    // (word E of d_ready, so that a stream step zeroes the stamps and the counter in one memset)
+    uint32_t *workCounter() const { return d_ready.p + E; }
     uint32_t counterBase = 0;          // what the counter read before the next launch's first claim
     DevBuf<unsigned long long> d_spill;  // [rasterGrid][spillStride]
     DevBuf<unsigned long long> d_rasterStats;  // mv_debug_raster_stats only
@@ -521,8 +526,8 @@ struct mv_engine {
     bool asyncContractBroken = false;
     Pending ring[3];
     DevBuf<uint32_t> d_prof;  // mv_debug_step_profile only
-    DevBuf<uint32_t> d_ready; // per-env step completion stamps (step kernel -> geometry kernel)
-    uint32_t readyStamp = 0;
+    DevBuf<uint32_t> d_ready; // [E + 1]: per-env step completion stamps (step kernel -> geometry kernel), then the raster work counter
+    uint32_t readyStamp = 0;  // the last host-path call's stamp: mv_reset's is 1, which every stream step uses (stepStream)
     bool overlap = true;      // geometry kernel launched as a programmatic dependent of the step kernel
     uint64_t asyncSteps = 0;
 
@@ -835,17 +840,18 @@ struct mv_engine {
     // One step (or forced flip) of sp.E envs: the step kernel, the raster launch of every view (of the active envs' views, see launchRaster,
     // when sp.active is set) -- a programmatic dependent of the step kernel when `dependent` and option overlap are on, else in stream order
     // behind it -- and, unless the step is a forced reset, the terminal frames of the envs that ended.  Every call but the asynchronous one
-    // with option overlap records kernel times.
-    int launchStep(const mvk::StepParams &sp, bool dependent) {
-        const bool async = sp.hostRewards != nullptr;  // mv_step_device: results land in its ring slot, terminal frames in HBM
-        const bool dep = dependent && overlap, timed = !(async && overlap), final = wantFinal && !sp.forceReset;
+    // with option overlap records kernel times.  `capturable` (mv_step_stream): device work only -- results and terminal frames in HBM, no
+    // event, no copy, and every view drawn (the host cannot vouch for the destination's rows at a graph replay)
+    int launchStep(const mvk::StepParams &sp, bool dependent, bool capturable = false) {
+        const bool async = sp.hostRewards != nullptr || capturable;  // mv_step_device: results land in its ring slot, terminal frames in HBM
+        const bool dep = dependent && overlap, timed = !capturable && !(async && overlap), final = wantFinal && !sp.forceReset;
         if (timed) MV_CUDA(cudaEventRecord(ev[0], stream));
         if (const int rc = launchStepKernel(sp)) return rc;
         if (timed && !dep) MV_CUDA(cudaEventRecord(ev[1], stream));  // an event between the two kernels would serialise them
         // host-facing: the state block goes down while the frames are drawn -- or, behind a programmatic dependent raster launch, while its
         // terminal frames are (the event the download waits for would serialise the two kernels)
         if (!async && !dep) { if (const int rc = downloadState()) return rc; }
-        if (const int rc = launchRaster(dep, sp.active)) return rc;
+        if (const int rc = launchRaster(capturable ? nullptr : sp.active, dep ? sp.readyStamp : 0)) return rc;
         if (!async && dep) { if (const int rc = downloadState()) return rc; }
         if (final) {  // after the step's own frames: the terminal frames of the envs that ended (stream order, no stamps)
             if (timed) MV_CUDA(cudaEventRecord(evFinal, stream));
@@ -889,7 +895,7 @@ struct mv_engine {
     int launchView(mvr::ViewParams &vp, bool dependent, mvr::Items items = mvr::Items::All) {
         const int grid = rasterGridFor(vp);
         vp.A = A; vp.instStride = instCap();
-        vp.workCounter = d_workCounter.p; vp.counterBase = counterBase;
+        vp.workCounter = workCounter(); vp.counterBase = counterBase;
         counterBase += uint32_t(vp.N) * uint32_t(vp.bands) + uint32_t(grid);
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(unsigned(grid)); cfg.blockDim = dim3(mvr::kThreads); cfg.dynamicSmemBytes = rasterSmem; cfg.stream = stream;
@@ -907,9 +913,11 @@ struct mv_engine {
         for (int e = 0; e < E; ++e) init[costItems() + size_t(e)] = uint32_t(e);
         return cudaMemcpy(d_viewCost.p, init.data(), sizeof(uint32_t) * init.size(), cudaMemcpyHostToDevice);
     }
-    // dep: a programmatic dependent launch of the step kernel just enqueued.  active: the step's active mask (or nullptr): when the
-    // destination already holds every view's current frame, only the views of the active envs are drawn -- the rows of the others stay
-    int launchRaster(bool dep, const uint8_t *active) {
+    // depStamp: the ready stamp of the step kernel just enqueued when this is its programmatic dependent launch, else 0.  active: the step's
+    // active mask (or nullptr): when the destination already holds every view's current frame, only the views of the active envs are drawn
+    // -- the rows of the others stay
+    int launchRaster(const uint8_t *active, uint32_t depStamp) {
+        const bool dep = depStamp != 0;
         mvr::ViewParams vp = frameParams(W, H, rasterBands, bandRows, d_spill.p, triCap, consts);
         vp.instances = d_inst.p; vp.instCounts = d_instCounts.p; vp.views = d_views.p;
         // pinned allocations are mapped into the device address space (UVA), so the kernel can store through the host pointer
@@ -917,7 +925,7 @@ struct mv_engine {
         vp.seg = wantSeg ? (rasterToHost ? h_seg.p : d_seg.p) : nullptr;
         vp.stats = d_rasterStats.p;
         // programmatic dependent launch: the grid may start before the step kernel has drained; a CTA waits for its env's stamp
-        vp.ready = dep ? d_ready.p : nullptr; vp.readyStamp = dep ? readyStamp : 0;
+        vp.ready = dep ? d_ready.p : nullptr; vp.readyStamp = depStamp;
         const bool fresh = rasterToHost ? hostObsFresh : (ownDeviceObsFresh && ownDeviceBuffers());
         const uint8_t *mask = fresh ? active : nullptr;
         const mvr::Items items = mask ? mvr::Items::Active : mvr::Items::All;
@@ -1265,6 +1273,60 @@ struct mv_engine {
         ++asyncSteps;
         return MV_OK;
     }
+    // mv_step_stream: the device work of stepAsync, forked from stream s onto the engine stream and joined back, with nothing a stream capture
+    // refuses and nothing a graph replay would repeat stale.  The per-call scalars of a host-path step become constants of the step: a
+    // memset zeroes the ready stamps and the work counter, the step kernel stamps 1 (mv_reset used it, so host-path calls stamp 2 and up),
+    // and the raster launches count their work from base 0.  The memset precedes the step kernel in stream order, so it has finished
+    // before the raster grid, the step kernel's programmatic dependent, can start
+    int stepStream(cudaStream_t s, const int32_t *dActions, const uint8_t *dEnds, const uint8_t *dActive) {
+        if (!levelSet) { setError("mv_step_stream: option level_set is off (without it every episode end needs host level generation)"); return MV_ERR_STATE; }
+        if (!didReset) { setError("mv_step_stream before mv_reset"); return MV_ERR_STATE; }
+        if (hostStepPending) { setError("mv_step_stream: mv_step_begin is outstanding, call mv_step_end first"); return MV_ERR_STATE; }
+        if (!replacements.empty()) { setError("mv_step_stream: mv_replace_levels requests are pending (host-path steps carry them out)"); return MV_ERR_STATE; }
+        if (!s) s = stream;
+        if (rtableDirty) {  // only before the first stream step: in stream mode mv_set_reward_shaping uploads at once
+            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+            MV_CUDA(cudaStreamIsCapturing(s, &cs));
+            if (cs != cudaStreamCaptureStatusNone) { setError("mv_step_stream: the reward shaping changed since the last step; take one step outside the capture first"); return MV_ERR_STATE; }
+            if (const int rc = uploadRtable()) return rc;
+        }
+        if (s != stream.h) {
+            MV_CUDA(cudaEventRecord(evFork, s));
+            MV_CUDA(cudaStreamWaitEvent(stream, evFork, 0));
+        }
+        streamMode = true;
+        MV_CUDA(cudaMemsetAsync(d_ready.p, 0, sizeof(uint32_t) * (size_t(E) + 1), stream));
+        counterBase = 0;
+        chooseDelivery(false);
+        mvk::StepParams sp = stepParams(dActions, false, nullptr, dEnds, dActive);
+        sp.readyStamp = 1;
+        if (const int rc = launchStep(sp, true, true)) return rc;
+        if (s != stream.h) {
+            MV_CUDA(cudaEventRecord(evJoin, stream));
+            MV_CUDA(cudaStreamWaitEvent(s, evJoin, 0));
+        }
+        return MV_OK;
+    }
+    // Stream mode: the head of every other entry point but the pointer getters.  Graph replays run on the caller's streams, unseen by the
+    // host: wait for the whole device, retire the asynchronous ring, refresh the host mirrors of what the last step left in HBM (level ids,
+    // episode counters, rewards, dones, reasons, true objectives) and restart the work counter.  An outstanding mv_step_begin keeps its
+    // own mirrors: mv_step_end publishes them
+    int streamSync() {
+        MV_CUDA(cudaDeviceSynchronize());
+        MV_CUDA(cudaMemset(workCounter(), 0, sizeof(uint32_t)));
+        counterBase = 0;
+        if (hostStepPending) return MV_OK;
+        if (const int rc = drain()) return rc;
+        MV_CUDA(cudaMemcpy(h_levelIds.p, d_levelIds.p, sizeof(int32_t) * size_t(E), cudaMemcpyDeviceToHost));
+        publishedCall = stepCalls - 1;
+        static_assert(sizeof(MvEnvState::episode_idx) == sizeof(int), "hostEpisode mirrors MvEnvState::episode_idx");
+        MV_CUDA(cudaMemcpy2D(hostEpisode.data(), sizeof(int), &d_envs.p[0].episode_idx, sizeof(MvEnvState), sizeof(int), size_t(E), cudaMemcpyDeviceToHost));
+        MV_CUDA(cudaMemcpy(h_rewards.p, d_rewards.p, sizeof(float) * size_t(N), cudaMemcpyDeviceToHost));
+        MV_CUDA(cudaMemcpy(h_dones.p, d_dones.p, size_t(E), cudaMemcpyDeviceToHost));
+        MV_CUDA(cudaMemcpy(h_doneReasons.p, d_doneReasons.p, size_t(E), cudaMemcpyDeviceToHost));
+        MV_CUDA(cudaMemcpy(h_trueObj.p, d_trueObj.p, sizeof(float) * size_t(N), cudaMemcpyDeviceToHost));
+        return MV_OK;
+    }
 
     int stepCommon(const int32_t *dActions, bool copyObs, bool split = false, const uint8_t *dActive = nullptr) {
         if (!didReset) { setError("mv_step before mv_reset"); return MV_ERR_STATE; }
@@ -1387,7 +1449,7 @@ struct mv_engine {
         if (toStore) return endTimes(Timed::FirstOnly);
         if (const int rc = downloadState()) return rc;  // the loaded rows, while the views are drawn again
         MV_CUDA(cudaEventRecord(ev[1], stream));
-        int rc = launchRaster(false, nullptr);
+        int rc = launchRaster(nullptr, 0);
         if (!rc && nRays) {  // the loaded envs' rays, behind the redraw (no terminal rays: the store keeps no terminal rows)
             MV_CUDA(cudaEventRecord(evRays, stream));
             rc = castRays(false, nullptr);
@@ -1661,6 +1723,27 @@ static void fillConsts(MvConsts &k, int W, int H) {
     k.p32 = farZ * nearZ / (nearZ - farZ);
 }
 
+// In stream mode an entry point is a synchronisation point: its head is mv_engine::streamSync, and its tail waits for the work it put on
+// the engine stream, which later graph replays on the caller's streams are not ordered behind.  Without stream steps both are one test
+namespace {
+struct StreamTail {
+    mv_engine *h;
+    ~StreamTail() { if (h->streamMode) cudaStreamSynchronize(h->stream); }
+};
+int streamHead(mv_engine *h) {
+    if (!h->streamMode) return MV_OK;
+    DeviceGuard dg(h->device);
+    if (!dg.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    return h->streamSync();
+}
+}  // namespace
+#define MV_SYNC_POINT(h)                                                                                          \
+    StreamTail tail__{(h)};                                                                                       \
+    if (const int rcs__ = streamHead(h)) return rcs__;
+// the calls that would reallocate or re-pitch a buffer a captured launch refers to
+#define MV_NOT_IN_STREAM_MODE(h, what)                                                                            \
+    if ((h)->streamMode) { (h)->setError(std::string(what) + ": refused after mv_step_stream (a captured launch may refer to the buffers it reallocates)"); return MV_ERR_STATE; }
+
 extern "C" {
 
 const char *mv_last_error(mv_handle h) { return h ? h->error.c_str() : g_createError.c_str(); }
@@ -1761,9 +1844,9 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
          ck(e->d_actions.alloc(N), "actions") && ck(e->d_rtable.alloc(N * MV_R_COUNT), "rtable") && ck(e->d_rewards.alloc(N), "rewards") &&
          ck(e->d_dones.alloc(E), "dones") && ck(e->d_doneReasons.alloc(E), "doneReasons") && ck(cudaMemset(e->d_doneReasons.p, 0, E), "doneReasons") &&
          ck(e->d_trueObj.alloc(N), "trueObj") && ck(e->d_obs.alloc(N * px * 4), "obs") && ck(e->d_faults.alloc(E), "faults") &&
-         ck(e->d_workCounter.alloc(4), "workCounter") && ck(cudaMemset(e->d_workCounter.p, 0, 16), "workCounter") &&
-         ck(e->d_viewCost.alloc(e->costItems() + size_t(E) + 1), "viewCost") && ck(e->resetViewOrder(), "viewOrder") && ck(e->d_ready.alloc(E), "ready") &&
-         ck(cudaMemset(e->d_ready.p, 0, sizeof(uint32_t) * size_t(E)), "ready");
+         ck(e->d_viewCost.alloc(e->costItems() + size_t(E) + 1), "viewCost") && ck(e->resetViewOrder(), "viewOrder") && ck(e->d_ready.alloc(E + 1), "ready") &&
+         ck(cudaMemset(e->d_ready.p, 0, sizeof(uint32_t) * (E + 1)), "ready");
+    ok = ok && ck(e->evFork.create(cudaEventDisableTiming), "event") && ck(e->evJoin.create(cudaEventDisableTiming), "event");
     { cudaDeviceProp prop; if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) e->numSMs = prop.multiProcessorCount; }
     if (e->instCap() > mvr::kMaxInstancesPerEnv) { e->setError("instance capacity exceeds the draw-order key range"); return fail(MV_ERR_CAPACITY); }
     // few views: split every view into row bands so that the persistent grid (2 CTAs per SM) has something to balance; every band repeats
@@ -1800,6 +1883,7 @@ int mv_create_mixed(const char *const *scenarios, int w, int h, int num_envs, in
 int mv_set_option(mv_handle h, const char *key, int value) {
     if (!key) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const std::string k = key;
     if (k == "depth") {
         if (h->didReset) { h->setError("option depth must be set before the first reset"); return MV_ERR_STATE; }
@@ -1859,6 +1943,7 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         return h->allocLevelSet();
     }
     if (k == "tri_cap") {  // triangles a raster CTA keeps in shared memory; views with more are drawn in several batches
+        MV_NOT_IN_STREAM_MODE(h, "option tri_cap")
         if (value < 32 || value > mvr::kMaxTriCap) { h->setError("tri_cap out of range [32,1022]"); return MV_ERR_ARG; }
         const int old = h->triCap;
         h->triCap = value;
@@ -1873,6 +1958,7 @@ int mv_set_option(mv_handle h, const char *key, int value) {
         return h->allocLevelSlots("static_cap");
     }
     if (k == "raster_bands") {  // row bands per view (each band is one work item of the persistent raster grid)
+        MV_NOT_IN_STREAM_MODE(h, "option raster_bands")
         if (value < 1 || value > h->H / 4 || (h->H / 4) % value) { h->setError("raster_bands must divide the number of 4-pixel tile rows"); return MV_ERR_ARG; }
         h->rasterBands = value;
         return h->configureRaster();
@@ -1913,6 +1999,7 @@ static void ensureMirrors(mv_handle h) {
 
 int mv_seed(mv_handle h, int seed) {
     if (!h) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     h->pool->waitAll();
     h->master.seed((unsigned long)seed);
     for (int e = 0; e < h->E; ++e) {  // one draw per env: its generator's seed, and its pick seed in a level set
@@ -1933,6 +2020,7 @@ int mv_seed(mv_handle h, int seed) {
 
 int mv_seed_env(mv_handle h, int env, int seed) {
     if (!h || env < 0 || env >= h->E) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     h->pool->waitAll();
     h->gens[size_t(env)].seed((unsigned long)seed);
     h->pickSeed[size_t(env)] = uint32_t(seed);
@@ -1946,6 +2034,7 @@ int mv_seed_env(mv_handle h, int env, int seed) {
 
 int mv_reset(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     ensureMirrors(h);
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     if (const int rcb = h->bankCall()) return rcb;
@@ -2036,17 +2125,20 @@ int mv_set_actions(mv_handle h, const int32_t *masks) {
 
 int mv_step(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     return h->stepHost(nullptr);
 }
 
 int mv_step_begin(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     if (cudaMemcpyAsync(h->d_actions.p, h->h_actions.p, sizeof(int32_t) * h->N, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { h->setError("actions upload failed"); return MV_ERR_CUDA; }
     return h->stepCommon(h->d_actions.p, h->obsToHost, true);
 }
 
 int mv_step_end(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     return h->stepEnd();
 }
 
@@ -2056,7 +2148,13 @@ int mv_step_device_ends(mv_handle h, const int32_t *d_masks, const uint8_t *d_en
 
 int mv_step_device_active(mv_handle h, const int32_t *d_masks, const uint8_t *d_ends, const uint8_t *d_active) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     return h->stepAsync(d_masks ? d_masks : h->d_actions.p, d_ends, d_active);
+}
+
+int mv_step_stream(mv_handle h, void *stream, const int32_t *d_masks, const uint8_t *d_ends, const uint8_t *d_active) {
+    MV_ON_DEVICE(h)
+    return h->stepStream(static_cast<cudaStream_t>(stream), d_masks ? d_masks : h->d_actions.p, d_ends, d_active);
 }
 
 // host-only: the colour tables of the level generators followed by the rasteriser's palette (float bit patterns), in the layout of
@@ -2111,6 +2209,7 @@ int mv_levels_skipped(mv_handle h) { return h ? h->levelsSkipped.load() : MV_ERR
 
 int mv_draw_hires(mv_handle h, int w, int hgt, const uint8_t **out) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const int rc = h->drawHires(w, hgt);
     if (rc) return rc;
     if (out) *out = h->hires.h_obs.p;
@@ -2130,6 +2229,7 @@ static int cameraCall(mv_handle h, const void *envs, const void *views, int n, i
 int mv_draw_cameras(mv_handle h, const int32_t *envs, const float *views16, int n, int w, int hgt, int want_depth, int want_seg, const uint8_t **obs,
                     const float **depth, const uint16_t **seg, uint32_t *out_of_range) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = cameraCall(h, envs, views16, n, w, hgt, "mv_draw_cameras");
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
@@ -2146,6 +2246,7 @@ int mv_draw_cameras(mv_handle h, const int32_t *envs, const float *views16, int 
 int mv_draw_cameras_device(mv_handle h, const int32_t *d_envs, const float *d_views16, int n, int w, int hgt, uint8_t *d_obs, float *d_depth,
                            uint16_t *d_seg, uint32_t **d_out_of_range) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const int rc = cameraCall(h, d_envs, d_views16, n, w, hgt, "mv_draw_cameras_device");
     if (rc) return rc;
     if (n > 0 && !d_obs) { h->setError("mv_draw_cameras_device: null obs buffer"); return MV_ERR_ARG; }
@@ -2159,6 +2260,7 @@ int mv_views_device(mv_handle h, float **d_views) { if (!h || !d_views) return M
 
 int mv_level_bounds(mv_handle h, float *out6) {
     if (!h || !out6) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     if (!h->didReset) { h->setError("mv_level_bounds before mv_reset"); return MV_ERR_STATE; }
     for (int e = 0; e < h->E; ++e) h->levelBounds(e, out6 + size_t(e) * 6);
     return MV_OK;
@@ -2190,6 +2292,7 @@ static int checkStatePairs(mv_handle h, const StateStore &st, const int32_t *env
 int mv_states_create(mv_handle h, int rows, int *store) {
     if (!store) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_states_create");
     if (rc) return rc;
     if (rows < 1) { h->setError("mv_states_create: rows must be positive"); return MV_ERR_ARG; }
@@ -2198,6 +2301,7 @@ int mv_states_create(mv_handle h, int rows, int *store) {
 
 int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *rows, int n) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_states_save");
     if (rc) return rc;
     StateStore *st = findStore(h, store, "mv_states_save");
@@ -2209,6 +2313,7 @@ int mv_states_save(mv_handle h, int store, const int32_t *envs, const int32_t *r
 
 int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *envs, int n) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_states_load");
     if (rc) return rc;
     StateStore *st = findStore(h, store, "mv_states_load");
@@ -2237,6 +2342,7 @@ int mv_states_load(mv_handle h, int store, const int32_t *rows, const int32_t *e
 
 int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_reset_envs");
     if (rc) return rc;
     if (n < 0 || (n > 0 && !envs)) { h->setError("mv_reset_envs: bad env array"); return MV_ERR_ARG; }
@@ -2251,6 +2357,7 @@ int mv_reset_envs(mv_handle h, const int32_t *envs, const int32_t *seeds, int n)
 
 int mv_step_envs(mv_handle h, const int32_t *envs, int n) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_step_envs");
     if (rc) return rc;
     if (n < 0 || (n > 0 && !envs)) { h->setError("mv_step_envs: bad env array"); return MV_ERR_ARG; }
@@ -2267,6 +2374,7 @@ int mv_step_envs(mv_handle h, const int32_t *envs, int n) {
 
 int mv_states_destroy(mv_handle h, int store) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     StateStore *st = findStore(h, store, "mv_states_destroy");
     if (!st) return MV_ERR_ARG;
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
@@ -2287,6 +2395,7 @@ static int levelSetCall(mv_handle h, const char *fn) {
 }
 int mv_level_ids(mv_handle h, const int32_t **out) {
     if (!h || !out) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     const int rc = levelSetCall(h, "mv_level_ids");
     if (rc == MV_OK) *out = h->h_levelIds.p;
     return rc;
@@ -2305,6 +2414,7 @@ int mv_next_levels_device(mv_handle h, int32_t **p) {
 }
 int mv_set_next_levels(mv_handle h, const int32_t *envs, const int32_t *levels, int n) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const int rc = levelSetCall(h, "mv_set_next_levels");
     if (rc) return rc;
     if (n < 0 || (n > 0 && (!envs || !levels))) { h->setError("mv_set_next_levels: bad env / level arrays"); return MV_ERR_ARG; }
@@ -2320,6 +2430,7 @@ int mv_replace_levels(mv_handle h, const int32_t *rows, const int32_t *seeds, in
     if (!h) return MV_ERR_ARG;
     int rc = levelSetCall(h, "mv_replace_levels");
     if (rc) return rc;
+    MV_NOT_IN_STREAM_MODE(h, "mv_replace_levels")
     if ((rc = statesCallState(h, "mv_replace_levels"))) return rc;
     if (n < 0 || (n > 0 && (!rows || !seeds))) { h->setError("mv_replace_levels: bad row / seed arrays"); return MV_ERR_ARG; }
     const size_t B = h->levelRows();
@@ -2352,6 +2463,7 @@ int mv_level_rows(mv_handle h, const int32_t **seeds, const uint8_t **retiring) 
 
 int mv_fetch_obs(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     if (h->hostStepPending) { const int rcp = h->stepEnd(); if (rcp) return rcp; }
     const int rc = h->drain();
     if (rc) return rc;
@@ -2383,6 +2495,7 @@ int mv_fetch_obs(mv_handle h) {
 
 int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable) {
     MV_ON_DEVICE(h)
+    MV_NOT_IN_STREAM_MODE(h, "mv_debug_step_profile")
     cudaStreamSynchronize(h->stream);
     if (enable && !h->d_prof.p) {
         if (h->d_prof.alloc(size_t(h->E) * 16) != cudaSuccess) { h->setError("profile buffer allocation failed"); return MV_ERR_CUDA; }
@@ -2395,6 +2508,7 @@ int mv_debug_step_profile(mv_handle h, uint32_t *out, int enable) {
 
 int mv_sync(mv_handle h) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const int rc = h->drain();
     if (rc) return rc;
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->setError("stream sync failed"); return MV_ERR_CUDA; }
@@ -2410,10 +2524,10 @@ int mv_segmentation_host(mv_handle h, const uint16_t **out) {
     *out = h->h_seg.p;
     return MV_OK;
 }
-int mv_rewards(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_rewards.p; return MV_OK; }
-int mv_dones(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_dones.p; return MV_OK; }
-int mv_true_objectives(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_trueObj.p; return MV_OK; }
-int mv_done_reasons(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; *out = h->h_doneReasons.p; return MV_OK; }
+int mv_rewards(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_rewards.p; return MV_OK; }
+int mv_dones(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_dones.p; return MV_OK; }
+int mv_true_objectives(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_trueObj.p; return MV_OK; }
+int mv_done_reasons(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_doneReasons.p; return MV_OK; }
 static int finalBuffer(mv_handle h, bool depth, const char *fn) {
     if (!h->wantFinal || (depth && !h->wantDepth)) { h->setError(std::string(fn) + ": option final_obs" + (depth ? " and option depth are" : " is") + " off"); return MV_ERR_ARG; }
     if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
@@ -2595,6 +2709,7 @@ int mv_get_reward_shaping(mv_handle h, int env, int agent, const char **keys, fl
 
 int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *keys, const float *vals, int n) {
     if (!h || env < 0 || env >= h->E || agent < 0 || agent >= h->A) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     // Scenario::setRewardShaping replaces the whole map (scenario.hpp:215); a scheme lacking a key the scenario reads
     // makes the reference throw std::out_of_range at the next reward event (scenario.hpp:253) -> reject it up front
     std::map<std::string, float> m;
@@ -2605,12 +2720,17 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
     h->shaping[view].assign(m.begin(), m.end());
     h->fillRtableRow(int(view));
     h->rtableDirty = true;
-    return MV_OK;
+    if (!h->streamMode) return MV_OK;
+    // in stream mode at once, on the engine's device: a host-path step may never come
+    DeviceGuard dg(h->device);
+    if (!dg.ok) { h->setError("cudaSetDevice failed"); return MV_ERR_CUDA; }
+    return h->uploadRtable();
 }
 
 int mv_faults(mv_handle h, int32_t *out) {
     if (!out) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     if (h->stream) cudaStreamSynchronize(h->stream);
     std::vector<MvEnvState> st(size_t(h->E));
     if (cudaMemcpy(st.data(), h->d_envs.p, sizeof(MvEnvState) * st.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -2623,6 +2743,7 @@ int mv_faults(mv_handle h, int32_t *out) {
 // totals since enable: {work items, instances read, instances with visible items, items, clipped items, triangles, batches, -}
 int mv_debug_raster_stats(mv_handle h, unsigned long long *out16, int enable) {
     MV_ON_DEVICE(h)
+    MV_NOT_IN_STREAM_MODE(h, "mv_debug_raster_stats")
     cudaStreamSynchronize(h->stream);
     if (out16 && h->d_rasterStats.p && cudaMemcpy(out16, h->d_rasterStats.p, 128, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     if (enable && !h->d_rasterStats.p) {
@@ -2651,6 +2772,7 @@ int mv_last_rays_ms(mv_handle h, float *out) { if (!h || !out) return MV_ERR_ARG
 int mv_close(mv_handle h) {
     if (!h) return MV_ERR_ARG;
     DeviceGuard dg__(h->device);  // not MV_ON_DEVICE: the engine is freed even when the switch fails
+    if (h->streamMode) cudaDeviceSynchronize();  // graph replays on the caller's streams may still use the engine's buffers
     delete h;
     return MV_OK;
 }
@@ -2702,6 +2824,7 @@ static int dumpLevel(const MvLevel &L, const MvBox *statics, const float *static
 
 int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
+    MV_SYNC_POINT(h)
     const size_t lid = h->liveRow(env);
     return dumpLevel(h->levels.level(lid), h->levels.statics(lid), h->levels.rotations(lid), h->A, false, out, cap);
 }
@@ -2709,6 +2832,7 @@ int mv_debug_get_level(mv_handle h, int env, int32_t *out, int cap) {
 int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     MvEnvState es;
     std::vector<MvAgent> ag(size_t(h->A));
     std::vector<MvObject> ob(MV_MAX_OBJECTS);
@@ -2760,6 +2884,7 @@ int mv_debug_get_state(mv_handle h, int env, float *out, int cap) {
 int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     MvEnvState es;
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(&es, &h->d_envs.p[env], sizeof es, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -2799,6 +2924,7 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
 int mv_debug_get_instances(mv_handle h, int env, float *out, int cap) {
     if (!h || env < 0 || env >= h->E || !h->didReset) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int32_t cnt[8];
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(cnt, h->d_instCounts.p + size_t(env) * 8, 32, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
@@ -2815,6 +2941,7 @@ int mv_debug_get_instances(mv_handle h, int env, float *out, int cap) {
 int mv_debug_get_view(mv_handle h, int env, int agent, float *out16) {
     if (!h || env < 0 || env >= h->E || agent < 0 || agent >= h->A || !h->didReset) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     cudaStreamSynchronize(h->stream);
     if (cudaMemcpy(out16, h->d_views.p + (size_t(env) * h->A + agent) * 16, 64, cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     return MV_OK;
@@ -2823,6 +2950,7 @@ int mv_debug_get_view(mv_handle h, int env, int agent, float *out16) {
 int mv_debug_view_order(mv_handle h, uint32_t *out, int cap) {
     if (!h || !out) return MV_ERR_ARG;
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     const size_t words = h->costItems() + size_t(h->E) + 1;
     if (size_t(cap) < words) return -int(words);
     if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMemcpy(out, h->d_viewCost.p, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost) != cudaSuccess) {
@@ -2834,6 +2962,7 @@ int mv_debug_view_order(mv_handle h, uint32_t *out, int cap) {
 
 int mv_debug_warp_agent(mv_handle h, int env, int agent, const float pos[3], const float basis9[9]) {
     MV_ON_DEVICE(h)
+    MV_SYNC_POINT(h)
     int rc = statesCallState(h, "mv_debug_warp_agent");
     if (rc) return rc;
     if (env < 0 || env >= h->E || agent < 0 || agent >= h->A) { h->setError("mv_debug_warp_agent: env / agent out of range"); return MV_ERR_ARG; }
