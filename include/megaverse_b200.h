@@ -137,6 +137,33 @@ int mv_final_obs_host(mv_handle h, const uint8_t **out);
 int mv_final_depth_host(mv_handle h, const float **out);
 int mv_final_obs_device(mv_handle h, uint8_t **d_final_obs);
 int mv_final_depth_device(mv_handle h, float **d_final_depth);
+/* Autoreset modes, option "autoreset" (before the first reset: MV_ERR_STATE after it, MV_ERR_ARG for any other value than 0, 1, 2; MV_ERR_ARG
+ * with option final_obs on, whichever is set first: under modes 1 and 2 the observation already is the terminal frame):
+ *   0 same-step (default, the reference's rule, Gymnasium's SAME_STEP): the call that ends an episode flips the env to its next level and
+ *     returns the new episode's first frame; option final_obs draws the ended one.
+ *   1 next-step (EnvPool's rule, Gymnasium >= 1.0's NEXT_STEP): the ending call returns the terminal frame with done; the env's next
+ *     active call runs no physics, starts the new episode and returns its first frame.
+ *   2 disabled: an ended env waits until mv_reset_envs (with or without seeds) or mv_reset restarts it (one-episode evaluation).
+ * An env is AWAITING from the call in which it ends until the call that starts its next episode.  The ending call defers the flip only:
+ * rewards (the ending tick pays 0), dones, reasons, true objectives and reward-component episode rows are what a same-step engine with
+ * final_obs reports; obs, depth, segmentation, state tensors, rays, views, level bounds and mv_level_ids show the ended episode's last
+ * state (the same-step engine's terminal frame, terminal rows and rays, and the finished episode's level).  An end at tick j < k of
+ * action_repeat k stops the ticks, as always.
+ * Next-step: an awaiting env that is ACTIVE in a call runs no tick -- its actions and end request are ignored -- takes its next level by
+ * the usual rule (the next slot of the ring; with a level set the caller's mv_set_next_levels entry, else the hash at the new episode's
+ * index) and reports what mv_reset_envs reports for a restarted env: reward 0, done 0, MV_END_NONE, its true objective unchanged,
+ * reward-component step rows 0, and the new episode's first frame, state rows, rays and level id.  An INACTIVE awaiting env (mv_step_envs,
+ * mv_step_device_active) stays awaiting.  The end-request rule of mv_step_device_ends counts ticks since the flip, and the restarting
+ * call runs none.
+ * Disabled: an awaiting env is stepped as an inactive env by every step call (reward 0, done 0, nothing runs, its frame and rows stay).
+ * The raster launch still draws its views unless the caller passes an active mask: !awaiting (mv_awaiting_reset_device) is the natural one.
+ * Everywhere: mv_reset and mv_reset_envs restart an awaiting env on the level its deferred flip would have taken and clear its flag; a
+ * state-store row carries the flag (a loaded awaiting env resumes as the saved one would have); an awaiting env holds its level-set row
+ * against mv_replace_levels, as an inactive env does.  Memory: E bytes in HBM and four times E pinned, against final_obs's buffers.
+ * mv_awaiting_reset_host / _device: uint8[num_envs], 1 where the env is awaiting after the last call, written by the step kernel beside
+ * dones and delivered like mv_done_reasons.  MV_ERR_ARG for a null argument or under mode 0, MV_ERR_STATE before mv_reset. */
+int mv_awaiting_reset_host(mv_handle h, const uint8_t **out);
+int mv_awaiting_reset_device(mv_handle h, uint8_t **d_awaiting);
 /* Segmentation, option "segmentation" (0/1, before the first reset: MV_ERR_STATE after it, MV_ERR_ARG for any other value; default 0).
  * uint16[N][h][w], view index env*A + agent, rows as in the observation tensor: the MV_SEG_* class of the drawable behind each pixel << 8 |
  * its index, 0 exactly where nothing was drawn (exactly where depth is 0).  The rasteriser names the drawable whose fragment won the pixel,
@@ -273,6 +300,8 @@ int mv_set_reward_shaping(mv_handle h, int env, int agent, const char *const *ke
  * otherwise leave the reference's level sequence; with 1 the env takes the next level of its stream instead and mv_levels_skipped
  * counts it),
  * "final_obs" (0/1, before the first reset, default 0: terminal frames of ended episodes, see mv_final_obs_host),
+ * "autoreset" (0/1/2, before the first reset, default 0: what an episode end does -- same-step, next-step or no autoreset, see
+ * mv_awaiting_reset_host),
  * "segmentation" (0/1, before the first reset, default 0: the class and index of the drawable behind every pixel, see
  * mv_segmentation_host),
  * "state_tensors" (0/1, before the first reset, default 0: agent, env, object and reward rows beside the frames, see mv_state_tensors_host),
@@ -446,8 +475,8 @@ int mv_stream(mv_handle h, void **stream);
  * is raised once to the largest level of the bank) + 80 B per decoration slot + three bit planes of the dense grid; DESIGN.md section 3
  * has the figures.  The per-env slot rings are not allocated.
  * mv_level_ids: host int32[num_envs], valid like mv_dones: the level each env is on after the last call -- for an env that just ended,
- *   the level of the NEW episode (the one the returned frame shows).  Inactive envs keep their value.  mv_level_ids_device: the same in
- *   HBM, written by the step kernel in stream order.
+ *   the level of the NEW episode (the one the returned frame shows; under option autoreset 1 and 2, the ended one's).  Inactive envs
+ *   keep their value.  mv_level_ids_device: the same in HBM, written by the step kernel in stream order.
  * mv_next_levels_device: device int32[num_envs], engine-owned, initially -1 everywhere.  The caller writes it in the order of mv_stream
  *   (a prioritised-replay sampler's output, say).  The array is input from outside the engine: the kernel bounds every entry before use,
  *   and a value outside [0, L) is ignored (the engine picks) and left as it is.

@@ -12,6 +12,7 @@ _lib = None
 
 MV_OK, MV_ERR_ARG, MV_ERR_CUDA, MV_ERR_CAPACITY, MV_ERR_STATE = 0, -1, -2, -3, -4
 MV_END_NONE, MV_END_TIME, MV_END_SOLVED, MV_END_REQUESTED = 0, 1, 2, 3  # done_reasons(): why an episode ended
+AUTORESET_SAME_STEP, AUTORESET_NEXT_STEP, AUTORESET_DISABLED = 0, 1, 2  # option "autoreset"
 # segmentation(): a pixel is class << 8 | index of the drawable behind it, 0 where nothing was drawn
 MV_SEG_NONE, MV_SEG_STATIC, MV_SEG_TERRAIN, MV_SEG_OBJECT, MV_SEG_AGENT, MV_SEG_REWARD = 0, 1, 2, 3, 4, 5
 MAX_OBJECTS, MAX_AGENTS, MAX_CAND = 128, 8, 96  # MV_MAX_OBJECTS, MV_MAX_AGENTS, MV_MAX_CAND (csrc/mv_types.h)
@@ -52,7 +53,7 @@ def lib():
                      "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_done_reasons", "mv_done_reasons_device",
                      "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device", "mv_final_depth_device",
                      "mv_segmentation_host", "mv_segmentation_device", "mv_level_ids", "mv_level_ids_device", "mv_next_levels_device",
-                     "mv_views_device"):
+                     "mv_views_device", "mv_awaiting_reset_host", "mv_awaiting_reset_device"):
             getattr(L, name).argtypes = [vp, C.POINTER(vp)]
         L.mv_get_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, C.POINTER(ci)]
         L.mv_set_reward_shaping.argtypes = [vp, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci]
@@ -114,6 +115,7 @@ EXPORTS = [
     "mv_debug_kcc", "mv_replace_levels", "mv_level_rows",
     "mv_reward_components_host", "mv_reward_components_device", "mv_reward_component_keys",
     "mv_step_stream",
+    "mv_awaiting_reset_host", "mv_awaiting_reset_device",
 ]
 
 STATE_TENSORS = ("agents", "envs", "objects", "rewards")  # the state tensors' order in the C calls (include/megaverse_b200.h)
@@ -338,12 +340,13 @@ class Engine:
         "next_levels" int32[E] (writable: the level an env plays next, -1 = the engine picks; write it on the engine's stream), and "views"
         float32[N,16] (the last step's view matrices, column-major: chase cameras on the device), and with rays (set_rays) "rays_dist"
         float32[N,R] / "rays_tag" uint16[N,R] and, with option final_obs too, "final_rays_dist" / "final_rays_tag", and with option
-        reward_components "reward_components" / "episode_reward_components" float32[N,8] (reward_components()).  Valid in the engine
-        stream's order (mv_stream) until mv_close."""
+        reward_components "reward_components" / "episode_reward_components" float32[N,8] (reward_components()), and with option
+        autoreset 1 or 2 "awaiting_reset" uint8[E] (awaiting_reset()).  Valid in the engine stream's order (mv_stream) until mv_close."""
         frame, px = (self.N, self.h, self.w, 4), (self.N, self.h, self.w)
         shapes = {"obs": (frame, "|u1"), "depth": (px, "<f4"), "rewards": ((self.N,), "<f4"), "dones": ((self.E,), "|u1"),
                   "done_reasons": ((self.E,), "|u1"), "true_objectives": ((self.N,), "<f4"), "final_obs": (frame, "|u1"), "final_depth": (px, "<f4"),
-                  "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4"), "views": ((self.N, 16), "<f4")}
+                  "segmentation": (px, "<u2"), "level_ids": ((self.E,), "<i4"), "next_levels": ((self.E,), "<i4"), "views": ((self.N, 16), "<f4"),
+                  "awaiting_reset": ((self.E,), "|u1")}
         for prefix in ("state_", "final_state_"):
             for k, shp in self._state_shapes().items():
                 shapes[prefix + k] = (shp, "<f4")
@@ -400,6 +403,11 @@ class Engine:
     def done_reasons(self):
         """uint8[E] MV_END_* of the last step: 0 not done, 1 time limit, 2 solved, 3 requested"""
         return self._host("mv_done_reasons", (self.E,), np.uint8)
+
+    def awaiting_reset(self):
+        """uint8[E] (option autoreset 1 or 2): 1 where the env's episode has ended and its next one has not started yet
+        (mv_awaiting_reset_host): under next-step its next active call restarts it, under disabled reset_envs does"""
+        return self._host("mv_awaiting_reset_host", (self.E,), np.uint8)
 
     def level_ids(self):
         """int32[E] (option level_set): the level of the set each env is on after the last call; for an env that just ended, the new episode's"""

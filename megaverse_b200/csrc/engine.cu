@@ -347,16 +347,19 @@ static ViewKernel viewKernelOf(mvr::Items items, bool seg, bool fast) {
     }
 }
 
-// the step kernel variant of a launch: level set, state tensors, reward components
+// the step kernel variant of a launch: level set, state tensors, reward components, autoreset mode
 using StepKernel = void (*)(mvk::StepParams);
-static StepKernel stepKernelOf(bool levelSet, bool state, bool rc) {
+template <int kAuto> static StepKernel stepKernelOf(bool levelSet, bool state, bool rc) {
     using mvk::stepKernel;
     if (rc) {
-        if (levelSet) return state ? stepKernel<true, true, true> : stepKernel<true, false, true>;
-        return state ? stepKernel<false, true, true> : stepKernel<false, false, true>;
+        if (levelSet) return state ? stepKernel<true, true, true, kAuto> : stepKernel<true, false, true, kAuto>;
+        return state ? stepKernel<false, true, true, kAuto> : stepKernel<false, false, true, kAuto>;
     }
-    if (levelSet) return state ? stepKernel<true, true> : stepKernel<true>;
-    return state ? stepKernel<false, true> : stepKernel<false>;
+    if (levelSet) return state ? stepKernel<true, true, false, kAuto> : stepKernel<true, false, false, kAuto>;
+    return state ? stepKernel<false, true, false, kAuto> : stepKernel<false, false, false, kAuto>;
+}
+static StepKernel stepKernelOf(bool levelSet, bool state, bool rc, int autoreset) {
+    return autoreset == 0 ? stepKernelOf<0>(levelSet, state, rc) : (autoreset == 1 ? stepKernelOf<1>(levelSet, state, rc) : stepKernelOf<2>(levelSet, state, rc));
 }
 
 struct mv_engine {
@@ -521,7 +524,7 @@ struct mv_engine {
     PinBuf<int32_t> h_faultWord;   // OR of all fault bits raised so far, written by the step kernel (system-scope atomic)
 
     // mv_step_device pipeline: results of step k are consumed by the host while steps k+1, k+2 already run
-    struct Pending { bool valid = false; uint64_t step = 0; int64_t call = 0; CudaEvent ev; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons; PinBuf<int32_t> levelIds; };
+    struct Pending { bool valid = false; uint64_t step = 0; int64_t call = 0; CudaEvent ev; PinBuf<float> rewards, trueObj; PinBuf<uint8_t> dones, reasons, awaiting; PinBuf<int32_t> levelIds; };
     std::vector<int64_t> lastAsyncDone;  // [E] asynchronous step index of the env's previous episode end
     bool asyncContractBroken = false;
     Pending ring[3];
@@ -564,6 +567,27 @@ struct mv_engine {
     DevBuf<float> d_finalDepth;     // [N][H][W], with option depth
     PinBuf<uint8_t> h_finalObs;
     PinBuf<float> h_finalDepth;
+
+    // autoreset (option "autoreset": 0 same-step, 1 next-step, 2 disabled).  Under 1 and 2 an ended env keeps its scene and is awaiting
+    // (MvEnvState::pad[1]) until its flip; the step kernel writes every stepped env's flag into d_awaiting beside dones (and into the ring
+    // slot's mirror), and the host keys its level bookkeeping on flips -- an env awaiting after the previous published call and not after
+    // this one -- instead of on dones.  Nothing is allocated under 0
+    int autoreset = 0;
+    DevBuf<uint8_t> d_awaiting;            // [E]
+    PinBuf<uint8_t> h_awaiting;            // [E] of the last published call, beside h_dones
+    std::vector<uint8_t> awaitPrev, flips;  // [E] h_awaiting as the previous published call left it; this call's flips
+    // the envs whose level bookkeeping advances with the call just published into h_dones / h_awaiting: the ended envs under same-step
+    // autoreset, else the flips (a call that flips an env runs no tick for it, so it cannot also end it)
+    const uint8_t *flipped() {
+        if (!autoreset) return h_dones.p;
+        for (int e = 0; e < E; ++e) flips[size_t(e)] = awaitPrev[size_t(e)] && !h_awaiting.p[e];
+        noteAwaiting();
+        return flips.data();
+    }
+    // a call that flips by itself (mv_reset, mv_reset_envs) or flips nothing (mv_states_load) was published: no flip to count
+    void noteAwaiting() {
+        if (autoreset) std::memcpy(awaitPrev.data(), h_awaiting.p, size_t(E));
+    }
 
     // state tensors (option "state_tensors", allocated at the first reset): the step kernel writes every stepped env's rows (layout in the
     // header) into one HBM block, agents [N][16], envs [E][16], objects [E][MV_MAX_OBJECTS][4], rewards [E][MV_MAX_REWARD][4], followed
@@ -814,6 +838,7 @@ struct mv_engine {
         sp.hostLevelIds = (mirror && levelSet) ? mirror->levelIds.p : nullptr;
         sp.rowPickable = d_rowPickable.p;
         sp.doneReasons = d_doneReasons.p; sp.hostDoneReasons = mirror ? mirror->reasons.p : nullptr;
+        sp.awaiting = autoreset ? d_awaiting.p : nullptr; sp.hostAwaiting = (autoreset && mirror) ? mirror->awaiting.p : nullptr;
         sp.termInstances = wantFinal ? d_termInst.p : nullptr; sp.termCounts = d_termCounts.p; sp.termViews = d_termViews.p;
         float *st = wantState ? d_state.p : nullptr, *termSt = wantFinal ? st : nullptr;
         sp.stAgents = stateTensor(st, 0, false); sp.stEnvs = stateTensor(st, 1, false); sp.stObjects = stateTensor(st, 2, false); sp.stRewards = stateTensor(st, 3, false);
@@ -832,7 +857,7 @@ struct mv_engine {
         const int blocks = (sp.E + warpsPerBlock - 1) / warpsPerBlock;
         const bool rc = sp.rcStep != nullptr;
         const size_t smem = (sizeof(mvk::WarpShared) + (rc ? mvk::kRcTickBytes : 0)) * warpsPerBlock;
-        stepKernelOf(sp.levelSet > 0, sp.stAgents != nullptr, rc)<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
+        stepKernelOf(sp.levelSet > 0, sp.stAgents != nullptr, rc, autoreset)<<<blocks, warpsPerBlock * 32, smem, stream>>>(sp);
         MV_CUDA(cudaGetLastError());
         launches += 1;
         return MV_OK;
@@ -1179,6 +1204,7 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(h_rewards.p, d_rewards.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_dones.p, d_dones.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_doneReasons.p, d_doneReasons.p, E, cudaMemcpyDeviceToHost, stream));
+        if (autoreset) MV_CUDA(cudaMemcpyAsync(h_awaiting.p, d_awaiting.p, E, cudaMemcpyDeviceToHost, stream));
         MV_CUDA(cudaMemcpyAsync(h_trueObj.p, d_trueObj.p, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
         if (const int rc = downloadRC(stream)) return rc;
         if (levelSet) {
@@ -1214,6 +1240,7 @@ struct mv_engine {
         std::memcpy(h_rewards.p, p.rewards.p, sizeof(float) * N);
         std::memcpy(h_dones.p, p.dones.p, E);
         std::memcpy(h_doneReasons.p, p.reasons.p, E);
+        if (autoreset) std::memcpy(h_awaiting.p, p.awaiting.p, E);
         std::memcpy(h_trueObj.p, p.trueObj.p, sizeof(float) * N);
         if (levelSet) { std::memcpy(h_levelIds.p, p.levelIds.p, sizeof(int32_t) * E); publishedCall = p.call; }
         p.valid = false;
@@ -1223,14 +1250,15 @@ struct mv_engine {
         // three calls deep (the kernel's request rule, num_frames >= 3 * repeat ticks, is the same three calls counted on the device).  With
         // four slots an env ends at most once per call, and the level replacing the end of call j is uploaded before kernel j + 3, when the
         // ends of calls j, j + 1 and j + 2 have used the three staged levels at most: there is nothing to check.  Nor with a level set,
-        // whose levels never arrive
+        // whose levels never arrive.  Under autoreset 1 and 2 the staged level is taken by the flip, not the end: the rule counts flips
         if (lastAsyncDone.empty()) lastAsyncDone.assign(size_t(E), -1000);
+        const uint8_t *fl = flipped();
         for (int e = 0; e < E; ++e)
-            if (h_dones.p[e]) {
+            if (fl[e]) {
                 if (levelSlots == 2 && !levelSet && int64_t(p.step) - lastAsyncDone[size_t(e)] < 3) asyncContractBroken = true;
                 lastAsyncDone[size_t(e)] = int64_t(p.step);
             }
-        afterFlip(h_dones.p);
+        afterFlip(fl);
         if (asyncContractBroken) { setError("mv_step_device: an episode lasted fewer than 3 steps -- outside the asynchronous call's contract; use mv_step"); return MV_ERR_STATE; }
         return MV_OK;
     }
@@ -1325,6 +1353,8 @@ struct mv_engine {
         MV_CUDA(cudaMemcpy(h_dones.p, d_dones.p, size_t(E), cudaMemcpyDeviceToHost));
         MV_CUDA(cudaMemcpy(h_doneReasons.p, d_doneReasons.p, size_t(E), cudaMemcpyDeviceToHost));
         MV_CUDA(cudaMemcpy(h_trueObj.p, d_trueObj.p, sizeof(float) * size_t(N), cudaMemcpyDeviceToHost));
+        if (autoreset) MV_CUDA(cudaMemcpy(h_awaiting.p, d_awaiting.p, size_t(E), cudaMemcpyDeviceToHost));
+        noteAwaiting();  // the level set's episode counters were just read back: no flip is left to count
         return MV_OK;
     }
 
@@ -1345,7 +1375,7 @@ struct mv_engine {
         rc = finishStep(copyObs, !split);
         if (rc) return rc;
         if (split) { hostStepPending = true; return MV_OK; }
-        afterFlip(h_dones.p);
+        afterFlip(flipped());
         return MV_OK;
     }
     // second half of a split host-facing step (mv_step_begin / mv_step_end): wait for the copies enqueued by stepCommon(split)
@@ -1355,7 +1385,7 @@ struct mv_engine {
         if (rc) return rc;
         hostStepPending = false;
         std::memset(h_actions.p, 0, sizeof(int32_t) * N);  // env.cpp:140-142: actions are cleared after every step
-        afterFlip(h_dones.p);
+        afterFlip(flipped());
         return MV_OK;
     }
     // mv_step, and mv_step_envs with the active mask in d_active: the action masks of mv_set_actions go up, one synchronous host-facing step
@@ -1494,7 +1524,16 @@ struct mv_engine {
     int statesLoad(StateStore &st, const int32_t *rows, const int32_t *envs, int n) {
         const int rc = quiesce();
         if (rc) return rc;
-        return redrawAndDeliver([&] { return copyStateRows(st, rows, envs, n, false); }, [&] { restoreHostRows(st, rows, envs, n); return MV_OK; });
+        const int rcl = redrawAndDeliver(
+            [&] {
+                const int rcc = copyStateRows(st, rows, envs, n, false);
+                // the loaded envs' flags (MvEnvState::pad[1], 0 or 1: its low byte) into the awaiting array, before it is delivered
+                if (!rcc && autoreset) MV_CUDA(cudaMemcpy2DAsync(d_awaiting.p, 1, &d_envs.p[0].pad[1], sizeof(MvEnvState), 1, size_t(E), cudaMemcpyDeviceToDevice, stream));
+                return rcc;
+            },
+            [&] { restoreHostRows(st, rows, envs, n); return MV_OK; });
+        if (!rcl) noteAwaiting();
+        return rcl;
     }
     // host state and mirrors; no episode end: no afterFlip, no generation job
     void restoreHostRows(const StateStore &st, const int32_t *rows, const int32_t *envs, int n) {
@@ -1532,7 +1571,7 @@ struct mv_engine {
         MV_CUDA(cudaMemcpyAsync(d_envList.p, h_envList.p, sizeof(uint32_t) * size_t(n), cudaMemcpyHostToDevice, stream));
         mvk::StepParams sp = stepParams(d_actions.p, true, nullptr, nullptr);
         sp.envOrder = d_envList.p; sp.E = n;
-        return redrawAndDeliver([&] { return launchStep(sp, false); }, [&] {
+        rc = redrawAndDeliver([&] { return launchStep(sp, false); }, [&] {
             std::vector<uint8_t> flipped(size_t(E), 0);
             for (int i = 0; i < n; ++i) {
                 flipped[size_t(envs[i])] = 1;
@@ -1541,6 +1580,8 @@ struct mv_engine {
             afterFlip(flipped.data());  // the levels after next, generated while the device draws
             return flushUploads();
         });
+        if (!rc) noteAwaiting();  // the restart's own flips are counted above
+        return rc;
     }
 
     // ------------------------------------------------------------------ level set
@@ -1698,10 +1739,10 @@ cudaError_t uploadPalette() {
 
 int setKernelAttrs(mv_engine *h) {
     cudaError_t err = cudaSuccess;
-    for (int v = 0; v < 8 && err == cudaSuccess; ++v) {
-        const bool rc = v >= 4;
+    for (int v = 0; v < 24 && err == cudaSuccess; ++v) {
+        const bool rc = (v & 4) != 0;
         const int smem = int((sizeof(mvk::WarpShared) + (rc ? mvk::kRcTickBytes : 0)) * 4);
-        err = cudaFuncSetAttribute(reinterpret_cast<const void *>(stepKernelOf(v & 1, v & 2, rc)), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        err = cudaFuncSetAttribute(reinterpret_cast<const void *>(stepKernelOf(v & 1, v & 2, rc, v >> 3)), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     }
     if (err != cudaSuccess) { h->setError(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err)); return MV_ERR_CUDA; }
     return MV_OK;
@@ -1908,7 +1949,25 @@ int mv_set_option(mv_handle h, const char *key, int value) {
     }
     if (k == "final_obs") {  // terminal frames of ended episodes; the buffers are allocated by the first reset (after "depth" / "static_cap")
         if (h->didReset) { h->setError("option final_obs must be set before the first reset"); return MV_ERR_STATE; }
+        if (value != 0 && h->autoreset) { h->setError("option final_obs needs option autoreset 0: under the other modes the observation is the terminal frame"); return MV_ERR_ARG; }
         h->wantFinal = value != 0;
+        return MV_OK;
+    }
+    if (k == "autoreset") {  // what an episode end does (see the header); the flag arrays are allocated here, only under modes 1 and 2
+        if (h->didReset) { h->setError("option autoreset must be set before the first reset"); return MV_ERR_STATE; }
+        if (value < 0 || value > 2) { h->setError("autoreset must be 0 (same-step), 1 (next-step) or 2 (disabled)"); return MV_ERR_ARG; }
+        if (value != 0 && h->wantFinal) { h->setError("option autoreset " + std::to_string(value) + " needs option final_obs 0: the observation is the terminal frame"); return MV_ERR_ARG; }
+        if (value != 0 && !h->d_awaiting.p) {
+            const size_t E = size_t(h->E);
+            bool ok = h->d_awaiting.alloc(E) == cudaSuccess && cudaMemset(h->d_awaiting.p, 0, E) == cudaSuccess && h->h_awaiting.alloc(E) == cudaSuccess;
+            for (auto &p : h->ring) ok = ok && p.awaiting.alloc(E) == cudaSuccess;
+            if (!ok) { h->d_awaiting.free(); h->setError("autoreset: allocation failed"); return MV_ERR_CUDA; }
+            std::memset(h->h_awaiting.p, 0, E);
+            for (auto &p : h->ring) std::memset(p.awaiting.p, 0, E);
+            h->awaitPrev.assign(E, 0);
+            h->flips.assign(E, 0);
+        }
+        h->autoreset = value;
         return MV_OK;
     }
     if (k == "state_tensors") {  // agent / env / object / reward rows beside the frames (see the header); allocated by the first reset
@@ -2104,6 +2163,7 @@ int mv_reset(mv_handle h) {
     rc = h->finishStep(h->obsToHost);
     if (rc) return rc;
     h->afterFlip(nullptr);
+    h->noteAwaiting();
     return MV_OK;
 }
 
@@ -2528,6 +2588,24 @@ int mv_rewards(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_A
 int mv_dones(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_dones.p; return MV_OK; }
 int mv_true_objectives(mv_handle h, const float **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_trueObj.p; return MV_OK; }
 int mv_done_reasons(mv_handle h, const uint8_t **out) { if (!h || !out) return MV_ERR_ARG; MV_SYNC_POINT(h) *out = h->h_doneReasons.p; return MV_OK; }
+static int awaitingBuffer(mv_handle h, const char *fn) {
+    if (!h->autoreset) { h->setError(std::string(fn) + ": option autoreset is 0 (no env ever awaits a reset)"); return MV_ERR_ARG; }
+    if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }
+    return MV_OK;
+}
+int mv_awaiting_reset_host(mv_handle h, const uint8_t **out) {
+    if (!h || !out) return MV_ERR_ARG;
+    if (const int rc = awaitingBuffer(h, "mv_awaiting_reset_host")) return rc;
+    MV_SYNC_POINT(h)
+    *out = h->h_awaiting.p;
+    return MV_OK;
+}
+int mv_awaiting_reset_device(mv_handle h, uint8_t **d) {
+    if (!h || !d) return MV_ERR_ARG;
+    if (const int rc = awaitingBuffer(h, "mv_awaiting_reset_device")) return rc;
+    *d = h->d_awaiting.p;
+    return MV_OK;
+}
 static int finalBuffer(mv_handle h, bool depth, const char *fn) {
     if (!h->wantFinal || (depth && !h->wantDepth)) { h->setError(std::string(fn) + ": option final_obs" + (depth ? " and option depth are" : " is") + " off"); return MV_ERR_ARG; }
     if (!h->didReset) { h->setError(std::string(fn) + " before mv_reset"); return MV_ERR_STATE; }

@@ -203,7 +203,8 @@ struct MvEnvState {
     int32_t positive_collected;  // Collect; Sokoban: numBoxesOnGoal
     int32_t bz_count, bz_nb, bz_next_resize;
     int16_t bz_items[MV_MAX_OBJECTS][4];
-    int32_t pad[2];          // pad[0]: with option "level_set" the env's pick seed (uint32 bits), set by the host, never by the kernel; pad[1]: 0
+    int32_t pad[2];          // pad[0]: with option "level_set" the env's pick seed (uint32 bits), set by the host, never by the kernel; pad[1]: with
+                             // option "autoreset" 1 or 2, 1 from the call in which the episode ended to the flip that starts the next (else 0)
 };
 
 // One drawable of an env, in the reference's draw order (mesh type major, insertion order minor,

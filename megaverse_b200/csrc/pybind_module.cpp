@@ -169,6 +169,13 @@ public:
         check(mv_done_reasons(h__, &d));
         return py::array_t<uint8_t>({numEnvs_}, d, py::none{});
     }
+    // (extension) option "autoreset" 1 or 2: uint8[num_envs], 1 where the env's episode ended and its next one has not started
+    py::array_t<uint8_t> getAwaitingReset() {
+        alive();
+        const uint8_t *d;
+        check(mv_awaiting_reset_host(h__, &d));
+        return py::array_t<uint8_t>({numEnvs_}, d, py::none{});
+    }
     // (extension) terminal frames, option "final_obs": [N,h,w,4], the views of env e hold the frame its last episode ended on
     py::array_t<uint8_t> getFinalObservations() {
         alive();
@@ -426,6 +433,7 @@ PYBIND11_MODULE(megaverse, m) {
         .def("get_dones", &MegaverseGym::getDones)
         .def("get_true_objectives", &MegaverseGym::getTrueObjectives)
         .def("get_done_reasons", &MegaverseGym::getDoneReasons, "uint8[num_envs] why each episode ended at the last step: 0 not done, 1 time limit, 2 solved, 3 requested")
+        .def("get_awaiting_reset", &MegaverseGym::getAwaitingReset, "uint8[num_envs] (option autoreset 1 or 2): 1 where the env's episode ended and its next one has not started")
         .def("get_final_observations", &MegaverseGym::getFinalObservations, "uint8[N,h,w,4] terminal frames (option final_obs): the frame each env's last episode ended on")
         .def("get_segmentation", &MegaverseGym::getSegmentation, "uint16[N,h,w] segmentation (option segmentation): class << 8 | index of the drawable behind each pixel, 0 where nothing was drawn")
         .def("obs_device_ptr", &MegaverseGym::obsDevicePtr)

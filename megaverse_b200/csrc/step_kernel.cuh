@@ -107,6 +107,9 @@ struct StepParams {
     // by the shaping slot whose weight paid it, the totals of the episodes that ended in the call, and the running totals of the episodes
     // under way (include/megaverse_b200.h has the rules)
     float *rcStep, *rcEpisode, *rcRun;
+    // option "autoreset" 1 or 2 (nullptr: mode 0; the stepKernel<.., .., .., 1|2> variants only): [E] MvEnvState::pad[1] after the call,
+    // 1 while the env's ended episode waits for its flip, written beside dones, and its optional pinned host mirror
+    uint8_t *awaiting, *hostAwaiting;
 };
 
 // option "reward_components": per warp, after the block's WarpShared records, one agent's tick columns per row -- what each shaping slot
@@ -1058,8 +1061,10 @@ __device__ void writeStateRows(const WarpShared &S, const MvLevel &L, const MvIn
 // kLevelSet: the level-set variant (StepParams::levelSet > 0).  A template parameter, not a run-time branch, so that the default
 // variant is the code it was before level sets existed.  kState: the state-tensor variant (StepParams::stAgents set), kRC: the
 // reward-component variant (StepParams::rcStep set, launched with kRcTickBytes more shared memory per warp), template parameters for the
-// same reason
-template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
+// same reason.  kAuto: option "autoreset" (0 same-step, 1 next-step, 2 disabled; StepParams::awaiting set for 1 and 2).  Under 1 and 2
+// an end does not flip: the env keeps the ended episode's scene in its live rows and is awaiting (MvEnvState::pad[1]) until the flip --
+// its next active call under 1 (the forced-reset path, no tick), a restart under 2, where it is stepped as an inactive env meanwhile
+template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> __global__ void __launch_bounds__(128) stepKernel(StepParams P) {
     extern __shared__ __align__(128) unsigned char smemRaw[];
     const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slotInGrid = blockIdx.x * (blockDim.x >> 5) + warpInBlock;
@@ -1067,7 +1072,8 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     asm volatile("griddepcontrol.launch_dependents;");
     if (slotInGrid >= P.E) return;
     const int env = P.envOrder ? int(__ldg(P.envOrder + slotInGrid)) : slotInGrid;
-    if (P.active && !P.active[env]) {
+    const bool awaiting = kAuto != 0 && P.envs[env].pad[1] != 0;
+    if ((P.active && !P.active[env]) || (kAuto == 2 && awaiting && !P.forceReset)) {
         // an inactive env: no staging, no tick, no write to its state.  It reports reward 0, not done and its unchanged true objective -- the
         // host mirror too, since a ring slot may still hold a value from three calls earlier -- and publishes its stamp for the raster launch
         for (int i = lane; i < P.A; i += 32) {
@@ -1084,11 +1090,18 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
             if (P.hostDones) P.hostDones[env] = 0;
             if (P.hostDoneReasons) P.hostDoneReasons[env] = MV_END_NONE;
             if (kLevelSet && P.hostLevelIds) P.hostLevelIds[env] = P.levelIds[env];  // unchanged; the ring slot may hold an older call's
+            if (kAuto) {
+                P.awaiting[env] = awaiting;
+                if (P.hostAwaiting) P.hostAwaiting[env] = awaiting;
+            }
             __threadfence();
             asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
         }
         return;
     }
+    // a flip without physics: mv_reset / mv_reset_envs, or under next-step autoreset an awaiting env's active call.  An expression, not a
+    // variable, so that under kAuto 0 every use reads P.forceReset as it did before the modes existed (and compiles to the same code)
+#define MV_FORCED (P.forceReset || (kAuto == 1 && awaiting))
     WarpShared &S = reinterpret_cast<WarpShared *>(smemRaw)[warpInBlock];
     const int A = P.A;
     const float dt = P.k.dt;
@@ -1101,7 +1114,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     MvObject *gObjects = P.objects + size_t(env) * MV_MAX_OBJECTS;
     if (lane == 0) {
         mbarInit(&S.mbar, 1);
-        if (!P.forceReset) {
+        if (!MV_FORCED) {
             const uint32_t bytes = uint32_t(P.maxObj) * uint32_t(sizeof(MvObject));
             mbarExpectTx(&S.mbar, bytes);
             if (bytes) bulkG2S(S.objects, gObjects, bytes, &S.mbar);
@@ -1122,9 +1135,9 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     const MvBox *statics = P.statics + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap);
     const float *staticRot = P.staticRot + levelRow<kLevelSet>(P, env, slot) * size_t(P.staticCap) * 2;
     int ns = L->n_static, no = L->n_obj;
-    if (!P.forceReset) mbarWait(&S.mbar, 0);
+    if (!MV_FORCED) mbarWait(&S.mbar, 0);
 
-    bool resetNow = P.forceReset != 0;
+    bool resetNow = MV_FORCED;
     bool doneFlag = false;
     // lane i < A: agent i's reward summed over the call's ticks, in tick order from 0 (the tick that ends the episode pays 0, as one step does)
     float rewardSum = 0.0f;
@@ -1133,7 +1146,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     float rcCall[2] = {0.0f, 0.0f};
     MV_PROBE(0);  // state staged
 
-    if (!P.forceReset) {
+    if (!MV_FORCED) {
         ColliderView cv;
         cv.S = &S; cv.L = L; cv.ns = ns; cv.no = no; cv.A = A; cv.nc = 0;
 
@@ -1593,7 +1606,9 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
             if (lane < A) rewardSum += S.lastReward[lane];
             if (kRC) { rcCall[0] += rcTick[lane]; rcCall[1] += rcTick[lane + 32]; }
         }
-        resetNow = doneFlag;
+        // same-step autoreset flips at the end; the other modes keep the ended episode live and mark the env awaiting its flip
+        resetNow = kAuto == 0 && doneFlag;
+        if (kAuto && doneFlag && lane == 0) S.env.pad[1] = 1;
         MV_PROBE(5);  // scenario logic
     }
 
@@ -1603,8 +1618,8 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     for (int i = lane; i < A; i += 32) {
         const size_t idx = size_t(env) * A + i;
         float to = P.trueObjectives[idx];
-        if (!P.forceReset && doneFlag) { to = L->scenario == MV_SCENARIO_TOWER ? float(S.env.highest_tower) : float(S.env.solved); P.trueObjectives[idx] = to; }
-        const float r = P.forceReset ? 0.0f : rewardSum;  // i == lane: A <= MV_MAX_AGENTS < 32
+        if (!MV_FORCED && doneFlag) { to = L->scenario == MV_SCENARIO_TOWER ? float(S.env.highest_tower) : float(S.env.solved); P.trueObjectives[idx] = to; }
+        const float r = MV_FORCED ? 0.0f : rewardSum;  // i == lane: A <= MV_MAX_AGENTS < 32
         P.rewards[idx] = r;
         if (P.hostRewards) { P.hostRewards[idx] = r; P.hostTrueObjectives[idx] = to; }
     }
@@ -1614,9 +1629,9 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
         for (int k = 0; k < 2; ++k) {
             const int i = lane + 32 * k;
             if (i < A * MV_R_COUNT) {
-                const float s = P.forceReset ? 0.0f : rcCall[k];
+                const float s = MV_FORCED ? 0.0f : rcCall[k];
                 P.rcStep[base + i] = s;
-                if (P.forceReset) {
+                if (MV_FORCED) {
                     P.rcRun[base + i] = 0.0f;
                 } else if (doneFlag) {
                     P.rcEpisode[base + i] = P.rcRun[base + i] + s;
@@ -1628,16 +1643,20 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
         }
     }
     if (lane == 0) {
-        const uint8_t dn = (!P.forceReset && doneFlag) ? 1 : 0;
+        const uint8_t dn = (!MV_FORCED && doneFlag) ? 1 : 0;
         P.dones[env] = dn;
         if (P.hostDones) P.hostDones[env] = dn;
         // solved first: doneWithTimer ran (also when a request arrives during its grace), then the clock, else the caller's request
         const uint8_t why = !dn ? uint8_t(MV_END_NONE) : (S.env.solved ? uint8_t(MV_END_SOLVED) : (S.env.episode_sec >= L->episode_len ? uint8_t(MV_END_TIME) : uint8_t(MV_END_REQUESTED)));
         P.doneReasons[env] = why;
         if (P.hostDoneReasons) P.hostDoneReasons[env] = why;
+        if (kAuto) {  // an env that ends awaits its flip; one that ran no tick flips below (or was not awaiting)
+            P.awaiting[env] = dn;
+            if (P.hostAwaiting) P.hostAwaiting[env] = dn;
+        }
     }
 
-    if (P.termInstances && !P.forceReset && doneFlag) {
+    if (kAuto == 0 && P.termInstances && !MV_FORCED && doneFlag) {
         // terminal row: the live row as the previous step left it, with this step's dynamic entries written on top from the still-live
         // level slot.  writeInstances only reads S, so this is exactly what a step that does not end writes, and the live path below
         // is untouched.
@@ -1662,6 +1681,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     }
 
     if (resetNow) {
+        if (kAuto && lane == 0) S.env.pad[1] = 0;
         if (kLevelSet) {
             // level set: the next level is a row of the bank, chosen here -- the caller's choice when it names a level of the set (used once),
             // else the hash of the env's pick seed and the new episode's index.  The entry comes from outside the engine: it is bounded
@@ -1720,7 +1740,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
     MV_PROBE(7);  // instance list + views
     if (kState) {  // the rows of the state the returned frame shows: after an end, the new episode's first
         __syncwarp();
-        writeStateRows(S, *L, P.instances + size_t(env) * P.instStride, A, resetNow, P.stAgents + size_t(env) * A * 16, P.stEnvs + size_t(env) * 16,
+        writeStateRows(S, *L, P.instances + size_t(env) * P.instStride, A, resetNow || (kAuto != 0 && doneFlag), P.stAgents + size_t(env) * A * 16, P.stEnvs + size_t(env) * 16,
                        P.stObjects + size_t(env) * MV_MAX_OBJECTS * 4, P.stRewards + size_t(env) * MV_MAX_REWARD * 4, lane);
     }
 
@@ -1746,6 +1766,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false> __global__ void
         __threadfence();
         asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(P.ready + env), "r"(P.readyStamp) : "memory");
     }
+#undef MV_FORCED
 #undef MV_PROBE
 }
 

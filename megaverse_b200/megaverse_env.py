@@ -69,10 +69,11 @@ class MegaverseEnv(Env):
     # step() / reset() fail instead of leaving the reference's level sequence; True takes the env's next level instead and counts it
     # (`levels_skipped()`, also reported in the infos).
     SKIP_UNFIT_LEVELS = False
+    AUTORESET_MODES = ("same_step", "next_step", "disabled")  # option "autoreset" 0, 1, 2
 
     def __init__(self, scenario_name, num_envs, num_agents_per_env, num_simulation_threads, use_vulkan=False, params=None, *, final_observation=False,
                  action_repeat=1, segmentation=False, num_levels=None, start_level=0, state_tensors=False,
-                 ray_directions=None, ray_max_distance=120.0, reward_components=False):
+                 ray_directions=None, ray_max_distance=120.0, reward_components=False, autoreset_mode="same_step"):
         # (extension) a sequence of num_envs names makes a mixed batch: env i runs scenario_name[i]
         # (extension) final_observation=True: the infos of done agents also carry the frame the episode ended on ('final_observation', CHW
         # like the observations) and whether it ended terminal ('terminated': solved) or was cut off ('truncated': time limit or request)
@@ -93,6 +94,16 @@ class MegaverseEnv(Env):
         # (extension) reward_components=True: reward_components() gives, per agent, what each shaping rule paid in the last step (columns
         # named by reward_component_keys()), and the infos of done agents carry 'reward_components', {key: the agent's total under that key
         # over the finished episode} (option "reward_components").  step()'s return values do not change
+        # (extension) autoreset_mode (option "autoreset"): "same_step" is the reference's rule (a done step returns the next episode's first
+        # frame).  "next_step" (EnvPool, Gymnasium >= 1.0): a done step returns the frame the episode ended on, and the env's next step runs
+        # no physics, starts the next episode and returns its first frame with reward 0 and done False.  "disabled": an env that is done
+        # stays on its terminal frame with reward 0 and done False until reset_envs restarts it.  Under both, the infos of done agents carry
+        # 'terminated' / 'truncated' and, with num_levels, 'level' (the level the frame shows), and awaiting_reset() tells which envs wait
+        if autoreset_mode not in self.AUTORESET_MODES:
+            raise ValueError('autoreset_mode must be one of %s, not %r' % (', '.join(self.AUTORESET_MODES), autoreset_mode))
+        if final_observation and autoreset_mode != "same_step":
+            raise ValueError('final_observation needs autoreset_mode "same_step": under %r the observation of a done step is the terminal frame'
+                             % autoreset_mode)
         if isinstance(scenario_name, str):
             scenario_name = scenario_name.casefold()
             self.scenarios = [scenario_name] * num_envs
@@ -140,6 +151,10 @@ class MegaverseEnv(Env):
         self.reward_components_enabled = bool(reward_components)
         if self.reward_components_enabled:
             self.env.set_option("reward_components", 1)
+        self.autoreset_mode = autoreset_mode
+        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
+        if autoreset_mode != "same_step":
+            self.env.set_option("autoreset", self.AUTORESET_MODES.index(autoreset_mode))
         self.action_repeat = int(action_repeat)
         self.env.set_option("action_repeat", self.action_repeat)
         self.num_levels = None if num_levels is None else int(num_levels)
@@ -214,8 +229,13 @@ class MegaverseEnv(Env):
         if self.num_levels is not None:
             self._levels_played = [int(j) for j in self.env.level_ids()]
 
+    def awaiting_reset(self):
+        """(extension, autoreset_mode "next_step" or "disabled") per env, True where its episode is done and the next has not started"""
+        return [bool(a) for a in self.env.get_awaiting_reset()]
+
     def level_ids(self):
-        """(extension, num_levels given) per env, the level of the set it is on now (after a done: the new episode's)"""
+        """(extension, num_levels given) per env, the level of the set it is on now (after a done: the new episode's under "same_step",
+        the finished one's under the other autoreset modes)"""
         return [int(j) for j in self.env.level_ids()]
 
     def set_next_levels(self, envs, levels):
@@ -281,8 +301,11 @@ class MegaverseEnv(Env):
 
     def _step_results(self):
         env_dones = self.env.get_dones()
-        if self.final_observation:
+        # the level a done agent's info names: the finished episode's, which the frame still shows unless the env flipped at once
+        levels_shown = self._levels_played if self.autoreset_mode == "same_step" else self.level_ids() if self.num_levels is not None else None
+        if self.final_observation or self.autoreset_mode != "same_step":
             reasons = self.env.get_done_reasons()
+        if self.final_observation:
             final = self.env.get_final_observations()
             final_state = self.env.get_final_state_tensors()['agents'] if self.state_tensors_enabled else None
             final_rays = self.env.get_final_rays() if self.num_rays else None
@@ -295,12 +318,16 @@ class MegaverseEnv(Env):
                 infos.extend([dict(true_reward=float(self.env.true_objective(env_i, j))) for j in range(self.num_agents_per_env)])
                 if self.num_levels is not None:
                     for j in range(self.num_agents_per_env):
-                        infos[env_i * self.num_agents_per_env + j]['level'] = self._levels_played[env_i]
+                        infos[env_i * self.num_agents_per_env + j]['level'] = levels_shown[env_i]
                 if episode_components is not None:
                     keys = reward_component_keys(self.scenarios[env_i])
                     for j in range(self.num_agents_per_env):
                         view = env_i * self.num_agents_per_env + j
                         infos[view]['reward_components'] = {k: float(episode_components[view, c]) for c, k in enumerate(keys) if k is not None}
+                if self.autoreset_mode != "same_step":
+                    for j in range(self.num_agents_per_env):
+                        infos[env_i * self.num_agents_per_env + j]['terminated'] = int(reasons[env_i]) == 2
+                        infos[env_i * self.num_agents_per_env + j]['truncated'] = int(reasons[env_i]) in (1, 3)
                 if self.final_observation:
                     for j in range(self.num_agents_per_env):
                         view = env_i * self.num_agents_per_env + j
@@ -407,7 +434,8 @@ class MegaverseEnv(Env):
     def reset_envs(self, envs, seeds=None):
         """(extension) envs[i] start a new episode now, the other envs keep going; with seeds, env envs[i] first takes seed seeds[i] and
         plays the first level of that stream.  Returns the observations of every agent, like reset().  With num_levels, a seed names a
-        pick sequence instead, and set_next_levels(envs, levels) before this call chooses the levels the envs start on."""
+        pick sequence instead, and set_next_levels(envs, levels) before this call chooses the levels the envs start on.  Under
+        autoreset_mode "disabled" this is how an env that is done starts its next episode."""
         self.env.reset_envs([int(e) for e in envs], None if seeds is None else [int(s) for s in seeds])
         self.check_faults()
         self._note_levels()
