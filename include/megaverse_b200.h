@@ -623,6 +623,10 @@ int mv_debug_kcc(const int32_t *hdr8, const float *boxes10, const float *agents3
  * episode `episode` (mv_debug_get_level layout, followed by each agent's 9 spawn-basis floats as bit patterns) */
 int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *param_keys,
                             const float *param_vals, int nparams, int32_t *out, int cap);
+/* host-only: the dense voxel grid of that same level, out6 = grid_org xyz, grid_dim xyz in voxels (the grid is the box
+ * [org, org + dim)).  Kept out of the mv_debug_get_level layout, which matches the oracle's. */
+int mv_debug_grid_box(const char *scenario, int num_agents, int env_seed, int episode, const char *const *param_keys,
+                      const float *param_vals, int nparams, int32_t *out6);
 /* libstdc++ unordered_set iteration-order emulation (bzset.h): ops[i] = {op(0 insert,1 erase,2 clear), x, y, z};
  * writes the final iteration order as xyz triples, returns the element count */
 /* per-env cycle stamps of the step kernel's phases: out = uint32[E][16] (0 staged, 1 actions, 2 candidate list, 3 controllers,

@@ -69,6 +69,7 @@ def lib():
         for name in ("mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances"):
             getattr(L, name).argtypes = [vp, ci, vp, ci]
         L.mv_debug_get_view.argtypes = [vp, ci, ci, vp]
+        L.mv_debug_grid_box.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(C.c_char_p), C.POINTER(cf), ci, vp]
         L.mv_debug_warp_agent.argtypes = [vp, ci, ci, vp, vp]
         L.mv_debug_render_instances.argtypes = [vp, vp, ci, ci, ci, vp, vp]
         L.mv_debug_render_instances_ex.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, vp, vp]
@@ -103,7 +104,7 @@ EXPORTS = [
     "mv_create", "mv_create_mixed", "mv_last_error", "mv_seed", "mv_seed_env", "mv_reset", "mv_set_actions", "mv_encode_action", "mv_step", "mv_step_begin", "mv_step_end", "mv_obs_host", "mv_depth_host",
     "mv_rewards", "mv_dones", "mv_true_objectives", "mv_get_reward_shaping", "mv_set_reward_shaping", "mv_set_option", "mv_step_device", "mv_set_obs_buffer",
     "mv_sync", "mv_fetch_obs", "mv_draw_hires", "mv_actions_device", "mv_obs_device", "mv_depth_device", "mv_rewards_device", "mv_dones_device", "mv_stream", "mv_faults", "mv_fault_word", "mv_kernel_launches",
-    "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_get_instances", "mv_debug_get_view", "mv_debug_warp_agent",
+    "mv_last_kernel_ms", "mv_close", "mv_debug_get_level", "mv_debug_get_state", "mv_debug_get_voxels", "mv_debug_grid_box", "mv_debug_get_instances", "mv_debug_get_view", "mv_debug_warp_agent",
     "mv_debug_render_instances", "mv_debug_render_instances_ex", "mv_debug_step_profile", "mv_debug_raster_config", "mv_debug_static_cap", "mv_debug_raster_stats", "mv_debug_color_tables", "mv_debug_defaults", "mv_debug_count_unfit_levels", "mv_levels_skipped", "mv_debug_bzset", "mv_debug_generate_level",
     "mv_states_create", "mv_states_save", "mv_states_load", "mv_states_destroy", "mv_state_row_bytes", "mv_step_device_ends", "mv_reset_envs",
     "mv_done_reasons", "mv_done_reasons_device", "mv_true_objectives_device", "mv_final_obs_host", "mv_final_depth_host", "mv_final_obs_device",
@@ -736,6 +737,18 @@ def generate_level(scenario, num_agents, env_seed, episode, params=None):
     if n < 0:
         raise MegaverseError(n, "mv_debug_generate_level failed")
     return out[:n].copy()
+
+
+def grid_box(scenario, num_agents, env_seed, episode, params=None):
+    """host-only: (grid_org, grid_dim) of generate_level's level -- the step kernel's dense voxel grid is the box [org, org + dim)"""
+    params = params or {}
+    keys = (C.c_char_p * max(1, len(params)))(*[k.encode() for k in params])
+    vals = (C.c_float * max(1, len(params)))(*[float(v) for v in params.values()])
+    out = np.zeros(6, dtype=np.int32)
+    rc = lib().mv_debug_grid_box(scenario.encode(), num_agents, env_seed, episode, keys, vals, len(params), out.ctypes.data)
+    if rc != MV_OK:
+        raise MegaverseError(rc, "mv_debug_grid_box failed")
+    return out[:3].copy(), out[3:].copy()
 
 
 def level_set_pick(pick_seed, episode, count):

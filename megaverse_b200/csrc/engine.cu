@@ -2972,6 +2972,8 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
     const MvBox *statics = h->levels.statics(lid);
     std::vector<uint8_t> og(size_t(h->gridCells));
     if (cudaMemcpy(og.data(), h->d_objGrid.p + size_t(env) * h->gridCells, og.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
+    std::vector<MvObject> ob(size_t(L.n_obj > 0 ? L.n_obj : 1));
+    if (cudaMemcpy(ob.data(), &h->d_objects.p[size_t(env) * MV_MAX_OBJECTS], sizeof(MvObject) * ob.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return MV_ERR_CUDA;
     // opacity is a property of the box a solid voxel belongs to
     std::vector<std::array<int32_t, 4>> v;
     for (int x = 0; x < L.grid_dim[0]; ++x)
@@ -2993,6 +2995,16 @@ int mv_debug_get_voxels(mv_handle h, int env, int32_t *out, int cap) {
                 if ((lavaBits[idx >> 5] >> (idx & 31)) & 1u) flags |= 2 << 8;
                 if (flags) v.push_back({x + L.grid_org[0], y + L.grid_org[1], z + L.grid_org[2], flags});
             }
+    // objects put down outside the grid live only in their translation (the step kernel's objAt); the scenarios without stacking
+    // keep their objects elsewhere (Sokoban's boxes on its 2-unit grid) or in no grid at all
+    const bool stacking = L.scenario == MV_SCENARIO_TOWER || L.scenario == MV_SCENARIO_OBSTACLES || L.scenario == MV_SCENARIO_COLLECT || L.scenario == MV_SCENARIO_REARRANGE;
+    for (int i = 0; i < L.n_obj && stacking; ++i) {
+        const MvObject &b = ob[size_t(i)];
+        if (b.parent >= 0) continue;
+        const int x = int(std::floor(b.t[0])), y = int(std::floor(b.t[1])), z = int(std::floor(b.t[2]));
+        const int gx = x - L.grid_org[0], gy = y - L.grid_org[1], gz = z - L.grid_org[2];
+        if (gx < 0 || gy < 0 || gz < 0 || gx >= L.grid_dim[0] || gy >= L.grid_dim[1] || gz >= L.grid_dim[2]) v.push_back({x, y, z, 4});
+    }
     std::sort(v.begin(), v.end());
     if (int(v.size()) * 4 > cap) return -int(v.size()) * 4;
     for (size_t i = 0; i < v.size(); ++i) std::memcpy(out + i * 4, v[i].data(), 16);
@@ -3234,20 +3246,37 @@ int mv_debug_kcc(const int32_t *hdr8, const float *boxes10, const float *agents3
 
 // host-only (no CUDA): run the product's level generator for env stream `env_seed` and dump episode `episode`'s level in
 // the mv_debug_get_level layout.  Lets the CPU test-suite compare level generation with the oracle without a GPU.
-int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys, const float *vals, int nparams,
-                            int32_t *out, int cap) {
+static int generateHostLevel(mv::LevelOut &lo, const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys,
+                             const float *vals, int nparams) {
     const int sc = scenario ? mv::scenarioFromName(scenario) : -1;
     if (sc < 0 || num_agents < 1 || num_agents > MV_MAX_AGENTS || episode < 0) return MV_ERR_ARG;
     mv::FloatParams params = mv::defaultFloatParams(scenario);
     for (int i = 0; i < nparams; ++i) params[keys[i]] = vals[i];
     mv::LevelGenerator gen(scenario, num_agents, params);
     gen.seed((unsigned long)env_seed);
-    mv::LevelOut lo;
     try {
         for (int ep = 0; ep <= episode; ++ep) gen.generate(lo, ep, 1 << 30);
     } catch (const std::exception &ex) { g_createError = ex.what(); return MV_ERR_CAPACITY; }  // mv_last_error(NULL) tells why
+    return MV_OK;
+}
+
+int mv_debug_generate_level(const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys, const float *vals, int nparams,
+                            int32_t *out, int cap) {
+    mv::LevelOut lo;
+    const int rc = generateHostLevel(lo, scenario, num_agents, env_seed, episode, keys, vals, nparams);
+    if (rc != MV_OK) return rc;
     // with the spawn yaw basis bits, so the float side of spawnAgents is pinned too
     return dumpLevel(lo.level, lo.statics.data(), lo.staticRot.data(), num_agents, true, out, cap);
+}
+
+int mv_debug_grid_box(const char *scenario, int num_agents, int env_seed, int episode, const char *const *keys, const float *vals, int nparams,
+                      int32_t *out6) {
+    if (!out6) return MV_ERR_ARG;
+    mv::LevelOut lo;
+    const int rc = generateHostLevel(lo, scenario, num_agents, env_seed, episode, keys, vals, nparams);
+    if (rc != MV_OK) return rc;
+    for (int a = 0; a < 3; ++a) { out6[a] = lo.level.grid_org[a]; out6[3 + a] = lo.level.grid_dim[a]; }
+    return MV_OK;
 }
 
 int mv_debug_bzset(const int32_t *ops, int nops, int32_t *out_xyz, int cap) {

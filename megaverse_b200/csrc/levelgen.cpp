@@ -281,9 +281,9 @@ int decoCapacity(int scenario) {
 
 int gridCapacity(int scenario) {
     // TowerBuilding rooms are at most 29 x (6+18) x 24; Obstacles chains of up to 7 platforms (+ transitions, start, exit)
-    // with the y range starting at -30 (objects dropped into gaps sink to y = -30, component_object_stacking.hpp:96-100)
-    // Collect: <= 41 x 41 landscape, heights <= 18, 16 cells of margin (objects can be put down beyond the edge), y from -30
-    // Rearrange: 19 x (6+18) x 14 room
+    // with the y range starting at -30; Collect: <= 41 x 41 landscape, heights <= 18, 16 cells of margin, y from -30;
+    // Rearrange: 19 x (6+18) x 14 room.  None of these bounds holds every put-down: an object that ends outside the grid (beyond
+    // the level's edge, sunk to y = -30 in the void, above the head-room) is found by the step kernel through its translation
     if (scenario == MV_SCENARIO_HEX_EXPLORE || scenario == MV_SCENARIO_EMPTY) return 128;  // no voxel grid
     if (scenario == MV_SCENARIO_HEX_MEMORY) return 64 * 4 * 64;  // one layer of cells over a maze of radius <= 7 * 3.5 * sqrt(3)
     // Sokoban: Boxoban rooms are 10 x 10 cells (voxel size 2), y in [-2, 6)
@@ -1364,8 +1364,8 @@ void LevelGenerator::generateCollect(LevelOut &out) {
     for (const auto &kv : grid) maxY = std::max(maxY, voxUnkey(kv.first).y);
     for (auto &c : objs) maxY = std::max(maxY, c.y);
     for (auto &c : rewards) maxY = std::max(maxY, c.y);
-    // margin: an agent that walks off the edge keeps its horizontal speed while it falls to y = -20 and can still put
-    // an object down out there (it sinks to y = -30)
+    // margin and y from -30: objects put down near the landscape's edge, or sunk to y = -30 off it, stay in the grid; those
+    // beyond it are exact too (the step kernel's objAt), the margin only keeps them on the grid's fast path
     L.grid_org[0] = -16; L.grid_org[1] = -30; L.grid_org[2] = -16;
     L.grid_dim[0] = length + 32; L.grid_dim[1] = maxY + 30 + 1 + 12; L.grid_dim[2] = width + 32;
     fillPlanes(out, &grid);
@@ -1783,7 +1783,8 @@ void LevelGenerator::generateObstacles(LevelOut &out) {
     L.episode_len = std::max(fp.at("episodeLengthSec"), float(numPlatforms) * 35 + float(objs.size()) * 1);
     L.n_movable = numPlatforms;  // reported by the level dump
 
-    // dense grid bounds: every voxel entry, objects, rewards; y from -30 (objects dropped into gaps sink there)
+    // dense grid bounds: every voxel entry, objects, rewards, one cell around; y from -30 (objects dropped into gaps sink
+    // there).  Objects put down beyond the box are exact too (the step kernel's objAt finds them by their translation)
     int mn[3] = {1 << 20, -30, 1 << 20}, mx[3] = {-(1 << 20), -(1 << 20), -(1 << 20)};
     auto grow = [&](int x, int y, int z) { mn[0] = std::min(mn[0], x); mn[2] = std::min(mn[2], z); mx[0] = std::max(mx[0], x); mx[1] = std::max(mx[1], y); mx[2] = std::max(mx[2], z); };
     for (const auto &kv : grid) { const I3 c = voxUnkey(kv.first); grow(c.x, c.y, c.z); }

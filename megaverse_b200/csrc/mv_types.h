@@ -84,7 +84,8 @@
 // fault bits (per env, sticky): the engine never exit()s, it reports
 #define MV_FAULT_LEVEL_NOT_READY 1   // episode ended before the host delivered the next level
 #define MV_FAULT_TRI_OVERFLOW 2      // a view produced more triangles than the rasteriser's shared-memory list holds
-#define MV_FAULT_GRID_RANGE 4        // an object was placed outside the dense voxel grid
+#define MV_FAULT_GRID_RANGE 4        // a Sokoban box was pushed outside the dense voxel grid (walled rooms: not expected); objects put
+                                     // down outside the grid are exact (the step kernel finds them by their translation)
 #define MV_FAULT_NAN 8               // NaN position (agent.cpp:82-93 guard)
 #define MV_FAULT_CAND_OVERFLOW 32     // more than MV_MAX_CAND colliders near one agent
 #define MV_FAULT_ENVELOPE 16         // an agent left the per-step collision envelope the candidate colliders were culled against

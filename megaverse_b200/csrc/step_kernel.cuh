@@ -1304,6 +1304,17 @@ template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> 
                 };
                 const bool interactTick = tick == 0;  // action repeat: Interact acts on the call's first tick only
                 const bool hasStacking = L->scenario != MV_SCENARIO_SOKOBAN && L->scenario != MV_SCENARIO_HEX_EXPLORE && L->scenario != MV_SCENARIO_HEX_MEMORY && L->scenario != MV_SCENARIO_EMPTY;
+                // the object in voxel (x, y, z), grid index g.  The reference's voxel map is unbounded, the dense grid is not: outside it
+                // (g < 0: put down beyond the level's edge, sunk into the void, or above the head-room) the object is the resting one
+                // whose translation floors to the voxel -- every resting object sits at its voxel + 0.5
+                auto objAt = [&](int g, int x, int y, int z) {
+                    if (g >= 0) return int(objGrid[g]);
+                    for (int k = 0; k < L->n_obj; ++k) {
+                        const MvObject &ob = S.objects[k];
+                        if (ob.parent < 0 && int(floorf(ob.t[0])) == x && int(floorf(ob.t[1])) == y && int(floorf(ob.t[2])) == z) return k;
+                    }
+                    return int(MV_NO_OBJECT);
+                };
                 for (int i = 0; i < A && hasStacking && interactTick; ++i) {  // ObjectStackingComponent (Sokoban and the hex mazes have none)
                     if (!(P.actions[size_t(env) * A + i] & MV_A_INTERACT)) continue;
                     MvAgent &a = S.agents[i];
@@ -1326,8 +1337,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> 
                         }
                         const uint32_t *sol = P.solid + levelRow<kLevelSet>(P, env, slot) * 3 * P.gridWords;
                         auto solidAt = [&](int g) { return g >= 0 && ((sol[g >> 5] >> (g & 31)) & 1u); };
-                        auto objAt = [&](int g) { return g >= 0 ? int(objGrid[g]) : int(MV_NO_OBJECT); };
-                        const bool empty = !solidAt(gi) && objAt(gi) == MV_NO_OBJECT;
+                        const bool empty = !solidAt(gi) && objAt(gi, vx, vy, vz) == MV_NO_OBJECT;
                         // canPlaceObject: TowerBuilding only inside the building zone, default true elsewhere
                         bool canPlace = true;
                         if (L->scenario == MV_SCENARIO_TOWER) canPlace = inBuildingZone(*L, vx, vz);
@@ -1338,11 +1348,11 @@ template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> 
                                 const int by = vy - 1;
                                 if (by < -30) break;
                                 const int gb = gridIndex(*L, vx, by, vz);
-                                if (solidAt(gb) || objAt(gb) != MV_NO_OBJECT) break;
+                                if (solidAt(gb) || objAt(gb, vx, by, vz) != MV_NO_OBJECT) break;
                                 vy = by;
                             }
                             const int gp = gridIndex(*L, vx, vy, vz);
-                            if (gp >= 0) objGrid[gp] = uint8_t(oi); else e.faults |= MV_FAULT_GRID_RANGE;
+                            if (gp >= 0) objGrid[gp] = uint8_t(oi);  // outside the grid the object's own translation records it
                             const V3 sc = scalingOf(local);
                             o.parent = -1;
                             o.s[0] = sc.x * carryingScaleInverse; o.s[1] = sc.y * carryingScaleInverse; o.s[2] = sc.z * carryingScaleInverse;
@@ -1368,8 +1378,8 @@ template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> 
                         int pickupHeight = 0;
                         while (pickupHeight <= 1) {
                             const int g = gridIndex(*L, vx, vy, vz), ga = gridIndex(*L, vx, vy + 1, vz);
-                            const int here = g >= 0 ? int(objGrid[g]) : int(MV_NO_OBJECT);
-                            const bool hasAbove = ga >= 0 && objGrid[ga] != MV_NO_OBJECT;
+                            const int here = objAt(g, vx, vy, vz);
+                            const bool hasAbove = objAt(ga, vx, vy + 1, vz) != MV_NO_OBJECT;
                             if (here != MV_NO_OBJECT && !hasAbove) {
                                 MvObject &o = S.objects[here];
                                 o.enabled = !o.enabled;
@@ -1379,7 +1389,7 @@ template <bool kLevelSet, bool kState = false, bool kRC = false, int kAuto = 0> 
                                 o.t[0] = 0.0f; o.t[1] = -0.3f; o.t[2] = 0.0f;
                                 o.parent = i;
                                 a.carrying = here;
-                                objGrid[g] = MV_NO_OBJECT;
+                                if (g >= 0) objGrid[g] = MV_NO_OBJECT;
                                 markDirty(here);
                                 if (L->scenario == MV_SCENARIO_TOWER) {  // pickedObject (scenario_tower_building.cpp:216-225)
                                     if (inBuildingZone(*L, vx, vz)) mvBzErase(e, vx, vy, vz);

@@ -265,20 +265,17 @@ def plan_warps(run, e, rng, t):
     hold = {}
     objs = run.objects(e)
     choice = rng.random()
-    if fam in FALLS and choice < 0.08:  # below y = -20, or off the level's edge
-        # only agents with empty hands: an object put down in the void lands at y = -30 in the reference, below the engine's dense
-        # grid (MV_FAULT_GRID_RANGE)
-        free_hands = [a for a in range(A) if run.agent(e, a)[22] < 0]
-        if not free_hands:
-            return hold
-        a = free_hands[int(rng.integers(len(free_hands)))]
+    if fam in FALLS and choice < 0.08:  # below y = -20, or off the level's edge; an agent that carries something may put it down
+        # out there, where it sinks to y = -30, outside the engine's dense grid beyond its margin
+        a = int(rng.integers(A))
         p = run.agent(e, a)
         if rng.random() < 0.5:
             run.warp(e, a, p[0], -25.0, p[2], 0.0)
+            hold[a] = 0
         else:
             v = run.o.voxels(e)
             run.warp(e, a, v[:, 0].min() - 6.0, p[1] + 1.0, p[2], 0.0)
-        hold[a] = 0
+            hold[a] = INTERACT if p[22] >= 0 else 0
         return hold
     if fam == "tower":
         for a in range(A):
